@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — frames/s of the TokenFlow edit on B200(s).  Default workload = BASELINE.json configs[1] ("C2"):
+"""bench.py — frames/s of the TokenFlow edit on H100(s).  Default workload = BASELINE.json configs[1] ("C2"):
 40-frame 512x512 SD1.5 PnP 50-step edit, keyframe stride B=8 -> K=5 keyframes per step, random-init
 SD1.5-shape UNet in fp16, synthetic latents (no SD weights / VAE / CLIP exist offline).
 
@@ -7,7 +7,8 @@ A "step" is one denoising step of the edit = the pivotal samples (extended atten
 frames (NN field + propagation) + CFG + DDIM update.  frames/s = N / (n_steps * mean step time), measured over
 --steps consecutive denoising steps.
 
-  python bench.py [--gpus N --steps K --warmup W]            our arm (CUDA kernels, sm_100a), config C2
+  python bench.py [--gpus N --steps K --warmup W]            our arm (CUDA kernels, sm_90a), config C2
+  python bench.py --dump-outputs DIR                         + the latents of the last timed step as DIR/latents.npy
   python bench.py --config {C2,C3,C4,C5s4,C5s8,C5s16}        the other BASELINE.json configs
   python bench.py --verify                                   + N-rank vs 1-rank (and graph vs eager) result check
   python bench.py --impl reference ...                       the reference's algorithm on host cores
@@ -76,7 +77,8 @@ def measured_peaks():
             p = json.load(f)
         return {"hbm_gbs": p["hbm_gbs"], "tf_burst": p["bf16_tflops"], "tf_sustained": p.get("bf16_tflops_sustained", p["bf16_tflops"]),
                 "source": "measured"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "source": "fallback"}
+    # H100 SXM data sheet (700 W): HBM3 bandwidth and dense fp16 tensor rate; not measured here
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "source": "fallback"}
 
 
 class ClockSampler:
@@ -226,7 +228,7 @@ def run_verify(args, device, world, rank, ed, x0, cfg_name, steps=2):
 
 
 def time_gpu_reference(args, device, cfg_name, unet, steps):
-    """The reference's GPU arithmetic on the same B200: this repo's hook plumbing with the ORACLE ops (plain
+    """The reference's GPU arithmetic on the same GPU: this repo's hook plumbing with the ORACLE ops (plain
     torch bmm / softmax / argmax / gather, as tokenflow_utils.py:114-199, :329-397 issue them) under
     torch.autocast(fp16), eager, the reference's schedule (pivotal pass + N/B frame passes)."""
     from oracle.oracle_ops import OracleOps
@@ -248,7 +250,7 @@ def time_gpu_reference(args, device, cfg_name, unet, steps):
     finally:
         tfu._install_ops_for_testing(None)
     return {"what": "reference GPU arithmetic (oracle ops on CUDA, autocast fp16, eager, pivotal pass + N/B frame passes) "
-                    "on the same UNet and B200", "steps": steps, "ms_per_step": round(ms, 2),
+                    "on the same UNet and GPU", "steps": steps, "ms_per_step": round(ms, 2),
             "value": round(c["n_frames"] / (c["n_steps"] * ms / 1e3), 4), "unit": "frames/s",
             "peak_mem_gib": round(peak_gb, 1)}
 
@@ -269,7 +271,7 @@ def run_ours(args):
             from tokenflow_b200.ops import Communicator
             comm = Communicator(world, rank)                    # tf_comm_init / tf_allgather (C ABI)
     from tokenflow_b200 import tokenflow_utils as tfu
-    ops = tfu._ops()                                     # CudaOps: raises if the .so / B200 is missing
+    ops = tfu._ops()                                     # CudaOps: raises if the .so / H100 is missing
     torch.backends.cudnn.benchmark = bool(args.cudnn_benchmark)
     ed, x0, src = build_editor(device, cfg_name, world, rank, channels_last=not args.no_channels_last,
                                frames_per_pass=args.frames_per_pass, fused_pass=bool(args.fused_pass),
@@ -323,6 +325,8 @@ def run_ours(args):
     ops.enable_timing(False)
     clocks = sampler.stop() if rank == 0 else None
     finite = bool(torch.isfinite(x.float()).all().item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, x)
 
     # ---- end-to-end through the public call with pinned host latents (`e2e`) ----
     ms_e2e = float("nan")
@@ -398,12 +402,13 @@ def run_ours(args):
             achieved = kt["work"] / (kt["ms"] * 1e-3) / 1e12
             roofline = {"kernel": dom, "bound": "tensor", "achieved": round(achieved, 2), "peak": peaks["tf_sustained"],
                         "unit": "TFLOP/s", "frac": round(achieved / peaks["tf_sustained"], 4), "traffic": traffic,
-                        "peak_source": f"{peaks['source']} sustained cuBLAS bf16 (kernel timed inside a long step)"}
+                        "peak_source": "measured sustained cuBLAS bf16 (kernel timed inside a long step)"
+                        if peaks["source"] == "measured" else "H100 SXM data sheet, dense fp16"}
         else:
             achieved = kt["work"] / (kt["ms"] * 1e-3) / 1e9
             roofline = {"kernel": dom, "bound": "hbm", "achieved": round(achieved, 1), "peak": peaks["hbm_gbs"],
                         "unit": "GB/s", "frac": round(achieved / peaks["hbm_gbs"], 4), "traffic": traffic,
-                        "peak_source": f"{peaks['source']} HBM copy"}
+                        "peak_source": "measured HBM copy" if peaks["source"] == "measured" else "H100 SXM data sheet, HBM3"}
         roofline["launches"] = kt["launches"]
         roofline["avg_launch_ms"] = round(kt["ms"] / max(1, kt["launches"]), 4)
         roofline["timing"] = ("event-record nodes inside the captured step graph, last replay of the timed region"
@@ -455,6 +460,14 @@ def run_ours(args):
         line["cpu_baseline"] = cpu
     print(json.dumps(line), flush=True)
     finish(world)
+
+
+def dump_outputs(out_dir, x):
+    """The latents the last timed step returned, as float32 `out_dir/latents.npy` (inputs are seeded, so two builds
+    run with the same arguments can be compared output for output)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "latents.npy"), x.detach().float().cpu().numpy())
 
 
 def finish(world):
@@ -673,6 +686,8 @@ def main():
                     help="1: one UNet call per step and GPU ([pivotal samples | frames], keyframe caches filled and "
                          "consumed inside each block); 0: the reference's pivotal pass + frame passes")
     ap.add_argument("--cudnn-benchmark", type=int, default=1, help="torch.backends.cudnn.benchmark for the UNet body convs")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the latents of the last timed step to DIR/latents.npy (float32)")
     args = ap.parse_args()
     if not args.fused_pass:
         args.graph = 0                                   # graphs capture the fused step only

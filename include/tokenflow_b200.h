@@ -1,4 +1,4 @@
-/* tokenflow_b200 — C ABI of the B200-native TokenFlow hot path.
+/* tokenflow_b200 — C ABI of the H100-native TokenFlow hot path.
  *
  * The reference (omerbt/TokenFlow @ 5dd6a69) is pure Python and has no FFI layer; its boundary for
  * this path is the hook surface of tokenflow_utils.py.  This library is what a replacement for those
@@ -15,7 +15,7 @@
  *     kernels by value); "device" pointers must be valid on the current device.
  *   - fp16 activations, int32 indices.  dim and head_dim must be multiples of 8; device pointers
  *     16-byte aligned; tensors contiguous unless a stride argument says otherwise.
- *   - compiled for sm_100a only; the kernels use tcgen05 / TMEM / TMA.
+ *   - compiled for sm_90a only; the kernels use wgmma / TMA / mbarrier.
  */
 #ifndef TOKENFLOW_B200_H_
 #define TOKENFLOW_B200_H_

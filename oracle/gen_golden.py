@@ -1,10 +1,12 @@
-"""ORACLE (test infrastructure) — generate tests/golden/*.pt by running the UNMODIFIED reference
-hooks (/root/reference/tokenflow_utils.py, imported through oracle/ref_shim.py) on seeded inputs.
+"""ORACLE (test infrastructure) — generate tests/golden/ by running the UNMODIFIED reference
+hooks (the original TokenFlow checkout's tokenflow_utils.py, imported through oracle/ref_shim.py) on
+seeded inputs.
 
-Run in the build container only:   python -m oracle.gen_golden
+Run where that checkout exists:   TOKENFLOW_REFERENCE_DIR=/path/to/TokenFlow python -m oracle.gen_golden
 The reference ships no golden vectors of its own (SURVEY.md §4); these files are the pin for the
 oracle and for the CUDA path.  Everything is fp32 on CPU (the reference's CPU-runnable configuration,
-BASELINE config C1), deterministic in the seeds below.  Files are small (< 1.5 MB total).
+BASELINE config C1), deterministic in the seeds below.  Every file stays under 1 MB: larger goldens are
+stored as a directory of parts (oracle/golden.py).
 """
 from __future__ import annotations
 
@@ -18,6 +20,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if REPO not in sys.path:
     sys.path.insert(0, REPO)
 
+from oracle import golden  # noqa: E402
 from oracle.ref_shim import load_reference  # noqa: E402
 from tokenflow_b200 import sd_unet  # noqa: E402
 from tokenflow_b200.editor import TokenFlowEditor, synthetic_inputs  # noqa: E402
@@ -132,6 +135,34 @@ def unet_case(ref, mode, seed=1, n_frames=4, batch_size=2, n_timesteps=2, latent
             "x0": x, "steps": steps, "out": out}
 
 
+LIVE_ATTN = [(101, 2, 24, 32, 2, False, False), (102, 4, 20, 64, 4, True, True), (103, 4, 20, 64, 4, True, False),
+             (104, 13, 8, 32, 4, True, True)]      # (seed, n, S, dim, heads, pnp, inject)
+
+
+def live_cases(ref, ref_util):
+    """Outputs of the reference hooks / helpers on the inputs tests/test_reference_live.py re-creates."""
+    attn = {}
+    for seed, n, S, dim, heads, pnp, inject in LIVE_ATTN:
+        torch.manual_seed(seed)
+        block = sd_unet.BasicTransformerBlock(dim, heads, dim // heads, 16).eval()
+        model = _Wrap(_OneBlockUNet(block))
+        if pnp:
+            ref.register_extended_attention_pnp(model, [981] if inject else [])
+            block.attn1.t = 981
+        else:
+            ref.register_extended_attention(model)
+        x = torch.randn(3 * n, S, dim)
+        with torch.no_grad():
+            want = block.attn1(x)
+        attn[seed] = {"state_dict": {k_: v_.clone() for k_, v_ in block.attn1.state_dict().items()}, "x": x, "out": want}
+    torch.manual_seed(5)
+    x, y = torch.randn(50, 24), torch.randn(30, 24)
+    blk = sd_unet.BasicTransformerBlock(16, 2, 8, 8)
+    names = ("BasicTransformerBlock", "Module", "Attention", "object")
+    return {"attn": attn, "cosine": {"x": x, "y": y, "sim": ref_util.batch_cosine_sim(x, y)},
+            "isinstance_str": {nm: ref_util.isinstance_str(blk, nm) for nm in names}}
+
+
 def main():
     ref, ref_util = load_reference()
     os.makedirs(GOLDEN_DIR, exist_ok=True)
@@ -143,12 +174,16 @@ def main():
         attention_case(ref, "pnp_n13_loop", 13, 16, 32, 2, True, 981, [981], seed=15),    # K>12 per-frame loop
         attention_case(ref, "sdedit_n2_d40", 2, 32, 80, 2, False, 0, [], seed=16),        # head dim 40
     ]
-    torch.save(attn, os.path.join(GOLDEN_DIR, "ext_attn.pt"))
-    torch.save(block_case(ref, ref_util), os.path.join(GOLDEN_DIR, "block_passes.pt"))
+    golden.save_parts(GOLDEN_DIR, "ext_attn.pt", [[c] for c in attn])          # one case per part
+    blk = block_case(ref, ref_util)
+    golden.save_parts(GOLDEN_DIR, "block_passes.pt", [{k_: v_ for k_, v_ in blk.items() if k_ != "frames"},
+                                                      {"frames": blk["frames"]}])
     torch.save(unet_case(ref, "pnp"), os.path.join(GOLDEN_DIR, "unet_c1_pnp.pt"))
     torch.save(unet_case(ref, "sdedit", n_timesteps=10), os.path.join(GOLDEN_DIR, "unet_c1_sdedit.pt"))
-    for f in sorted(os.listdir(GOLDEN_DIR)):
-        print(f, os.path.getsize(os.path.join(GOLDEN_DIR, f)))
+    torch.save(live_cases(ref, ref_util), os.path.join(GOLDEN_DIR, "reference_live.pt"))
+    for root, _, files in sorted(os.walk(GOLDEN_DIR)):
+        for f in sorted(files):
+            print(os.path.relpath(os.path.join(root, f), GOLDEN_DIR), os.path.getsize(os.path.join(root, f)))
 
 
 if __name__ == "__main__":

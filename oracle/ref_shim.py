@@ -1,9 +1,8 @@
-"""ORACLE (test infrastructure) — import the UNMODIFIED reference hooks from /root/reference.
+"""ORACLE (test infrastructure) — import the UNMODIFIED reference hooks from a checkout of the
+original TokenFlow repository named by $TOKENFLOW_REFERENCE_DIR.
 
-Only usable in the build container (the GPU box has no /root/reference); used by
-`oracle/gen_golden.py` to produce `tests/golden/*.pt` and by `tests/test_reference_live.py`
-(skipped when the reference tree is absent).  Nothing is copied: the reference files are imported
-from where they lie.
+Used by `oracle/gen_golden.py` to produce `tests/golden/`; the tests themselves only read those
+goldens.  Nothing is copied: the reference files are imported from where they lie.
 
 Why a shim is needed (SURVEY.md §8c): reference util.py:8 imports torchvision.io.read_video /
 write_video (removed in torchvision 0.26) and util.py:14-15 import kornia (not installed).
@@ -16,7 +15,7 @@ import os
 import sys
 import types
 
-REFERENCE_DIR = os.environ.get("TOKENFLOW_REFERENCE_DIR", "/root/reference")
+REFERENCE_DIR = os.environ.get("TOKENFLOW_REFERENCE_DIR", "")
 
 
 def reference_available() -> bool:

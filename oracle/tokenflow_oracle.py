@@ -6,10 +6,9 @@ and `bench.py`'s CPU-baseline / `--impl reference` legs may import this package;
 (`tokenflow_b200/`) never does and has no CPU fallback.
 
 Pinning: the reference has no tests / golden vectors of its own (SURVEY.md §4), so this oracle is
-pinned against the *unmodified* reference hooks executed live in the build container through
-`oracle/ref_shim.py`; the vectors that run produced are committed under `tests/golden/` together
-with `oracle/gen_golden.py`, and `tests/test_oracle_golden.py` re-checks the oracle against them
-everywhere (the GPU box has no /root/reference).
+pinned against the *unmodified* reference hooks, executed through `oracle/ref_shim.py` by
+`oracle/gen_golden.py`; the vectors that run produced are committed under `tests/golden/`, and
+`tests/test_oracle_golden.py` re-checks the oracle against them everywhere.
 
 Each function cites the reference lines it restates.  The functions are device agnostic: on CPU
 they run in the dtype they are given (fp32 for BASELINE config C1, fp64 for closed-form checks); on

@@ -1,5 +1,5 @@
 """CPU tier: bench.py's reference / cpu_baseline leg (the oracle port composed with the C2 op counts) on a
-toy UNet, and the JSON contract of the `--impl reference` line.  (The GPU arm needs a B200.)"""
+toy UNet, and the JSON contract of the `--impl reference` line.  (The GPU arm needs an H100.)"""
 import json
 import os
 import sys

@@ -56,14 +56,14 @@ def test_argument_validation_needs_no_gpu(lib):
     assert lib.tf_nn_field(None, None, kf, None, 0, 16, 32, 3, None, None, None) == 0
 
 
-def test_library_is_sm100a_and_uses_tcgen05():
-    """The shipped cubin is sm_100a and the hot kernels really use tcgen05 / TMEM / TMA."""
+def test_library_is_sm90a_and_uses_wgmma():
+    """The shipped cubin is sm_90a and the hot kernels really use wgmma / TMA / mbarrier."""
     import shutil
     import subprocess
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", str(ops.library_path())], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM", "STTM"):
+    assert "sm_90a" in sass and "sm_100" not in sass
+    for mnemonic in ("HGMMA.64x128x16.F32", "UTMALDG.4D", "UTMALDG.3D", "SYNCS.PHASECHK"):
         assert mnemonic in sass, mnemonic

@@ -1,4 +1,4 @@
-"""GPU tier (-m gpu): the sm_100a kernels, called through the C ABI (tokenflow_b200.ops.CudaOps →
+"""GPU tier (-m gpu): the sm_90a kernels, called through the C ABI (tokenflow_b200.ops.CudaOps →
 libtokenflow_b200.so), against the oracle on the same seeded inputs, against the committed golden
 vectors, and — at BASELINE full sizes — through size-independent properties.
 
@@ -9,13 +9,13 @@ deviation is inside a *tie class*: two candidates whose fp16 similarity differs 
 where the winner depends on the fp32 accumulation order of the GEMM (cuBLAS's own order is not
 specified either).  Such rows are counted, bounded, and every one of them is checked.
 """
-import os
 
 import pytest
 import torch
 
 from oracle import tokenflow_oracle as O
 from oracle.oracle_ops import OracleOps
+from oracle import golden
 
 pytestmark = pytest.mark.gpu
 
@@ -27,7 +27,7 @@ def ops():
 
 
 def _load(golden_dir, name):
-    return torch.load(os.path.join(golden_dir, name), weights_only=False)
+    return golden.load(golden_dir, name)
 
 
 def _video_like(F, K, S, dim, seed, noise=0.3, device="cuda"):

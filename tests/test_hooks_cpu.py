@@ -1,7 +1,6 @@
 """CPU tier: this package's hook layer (tokenflow_b200.tokenflow_utils) with the oracle ops installed,
 against golden vectors produced by the unmodified reference hooks — i.e. the host logic / plumbing
 of the drop-in, with no GPU compute.  BASELINE config C1 in miniature."""
-import os
 
 import pytest
 import torch
@@ -12,10 +11,11 @@ from tokenflow_b200 import sd_unet
 from tokenflow_b200 import tokenflow_utils as tfu
 from tokenflow_b200.editor import TokenFlowEditor, synthetic_inputs
 from tokenflow_b200.scheduler import DDIMScheduler
+from oracle import golden
 
 
 def _load(golden_dir, name):
-    return torch.load(os.path.join(golden_dir, name), weights_only=False)
+    return golden.load(golden_dir, name)
 
 
 class _OneBlockUNet(nn.Module):

@@ -1,6 +1,5 @@
 """CPU tier: the oracle restatement against the golden vectors the UNMODIFIED reference produced
 (oracle/gen_golden.py), and against the independent numpy closed form."""
-import os
 
 import numpy as np
 import pytest
@@ -8,10 +7,11 @@ import torch
 
 from oracle import closed_form as CF
 from oracle import tokenflow_oracle as O
+from oracle import golden
 
 
 def _load(golden_dir, name):
-    return torch.load(os.path.join(golden_dir, name), weights_only=False)
+    return golden.load(golden_dir, name)
 
 
 @pytest.fixture(scope="module")

@@ -1,4 +1,4 @@
-"""tokenflow_b200 — B200-native (sm_100a) implementation of TokenFlow's per-denoise-step hot path.
+"""tokenflow_b200 — H100-native (sm_90a) implementation of TokenFlow's per-denoise-step hot path.
 
 Layout (only what the path needs):
     csrc/               CUDA kernels + the C-ABI (include/tokenflow_b200.h)

@@ -31,10 +31,10 @@ int check_cuda(cudaError_t e, const char* what) {
 int sm_count() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -278,11 +278,10 @@ int tf_ext_attn_fwd_rows(const void* q, int q_slabs, int64_t q_tok_stride, const
     }
   }
   // Samples that share q and k (PnP q/k injection: the uncond and cond sample of a keyframe, reference :124-130) have
-  // identical scores and probabilities: pair them and let one kernel compute S / P once and P [V_a | V_b] together.
+  // identical scores and probabilities: pair them and let one kernel compute S / P once and both P V products.
   std::vector<int> partner(n_out, -1);
   int n_pairs = 0;
-  const int rows_here = (q_row0 + q_nrows < S ? q_row0 + q_nrows : S) - q_row0;
-  if (ext_attn_pairs_supported(rows_here, d)) {
+  if (ext_attn_pairs_supported(d)) {
     for (int i = 0; i < n_out; ++i) {
       if (partner[i] >= 0) continue;
       for (int j = i + 1; j < n_out; ++j) {

@@ -1,10 +1,9 @@
-// tokenflow_b200 — shared device/host helpers for the sm_100a kernels.
+// tokenflow_b200 — shared device/host helpers for the sm_90a kernels.
 //
-// Thin inline-PTX wrappers for the Blackwell primitives the kernels use: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / st / fences) and the UMMA shared
-// memory + instruction descriptors.  Bit layouts follow the PTX ISA "tcgen05 matrix descriptor"
-// and "instruction descriptor" tables (cross-checked against the field lists in CUTLASS 4.x
-// cute/arch/mma_sm100_desc.hpp; nothing is included from CUTLASS).
+// Thin inline-PTX wrappers for the Hopper primitives the kernels use: mbarrier, TMA
+// (cp.async.bulk.tensor) and wgmma (shared-memory matrix descriptors, fences, commit / wait; the
+// MMA wrappers themselves are in tf_wgmma.cuh).  Bit layouts follow the PTX ISA "matrix descriptor"
+// table of the asynchronous warpgroup MMA section.
 #pragma once
 
 #include <cuda.h>
@@ -45,27 +44,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31u; }
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-
-// Warp-specialised register budgets: a whole warpgroup (4 consecutive warps) gives registers back to the
-// SM's pool or takes more (multiples of 8, 24..256).  ptxas sizes the code that follows for the new budget.
-template <int kRegs>
-__device__ __forceinline__ void warpgroup_reg_dec() {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs));
-}
-template <int kRegs>
-__device__ __forceinline__ void warpgroup_reg_inc() {
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs));
-}
 
 // ------------------------------------------------------------------------------------------
 // mbarrier
@@ -109,11 +87,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if ((++spins & 2047u) == 0) {
       const uint64_t now = global_timer_ns();
       if (t0 == 0) t0 = now;
-      if (now - t0 > 2000000000ull) {
-        printf("tokenflow_b200: mbarrier wait timed out (block %d thread %d smem 0x%x parity %u)\n",
-               (int)blockIdx.x, (int)threadIdx.x, smem_u32(bar), parity);
-        __trap();
-      }
+      if (now - t0 > 2000000000ull) __trap();   // no printf here: a call inside the loop serialises wgmma
     }
   }
 }
@@ -144,157 +118,38 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
 }
 
 // ------------------------------------------------------------------------------------------
-// tcgen05: tensor memory + MMA
-// ------------------------------------------------------------------------------------------
-// Allocate `ncols` (power of two, 32..512) TMEM columns; whole warp must execute.  The base
-// address is written to *smem_result.
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-               ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// Arrive on `bar` once every tcgen05.mma previously issued by this thread has completed.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-               ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]      (kind::f16: fp16/bf16 operands, fp32 or fp16 accumulator)
-__device__ __forceinline__ void tc_mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void tc_mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive 32-bit columns: thread `lane` of warp w reads TMEM lane 32*(w%4)+lane.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-        "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-        "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld1(uint32_t taddr, uint32_t& r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-      "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-      "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-
-// ------------------------------------------------------------------------------------------
-// UMMA descriptors
+// wgmma (warpgroup MMA): shared-memory descriptors, fences, commit / wait
 // ------------------------------------------------------------------------------------------
 // Shared-memory matrix descriptor, 128-byte swizzle, tile rows of exactly 128 bytes (64 x 16-bit):
 //   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1 (sm_100)
-//   bits [49,52) base offset = 0 (tiles are 1024-byte aligned)      bits [61,64) layout: 2 = SWIZZLE_128B
+//   bits [32,46) stride byte offset >> 4   bits [49,52) base offset = 0 (tiles are 1024-byte aligned)
+//   bits [62,64) layout: 1 = SWIZZLE_128B
 // K-major operand  : rows (M or N index) are 128 B apart inside an 8-row group, groups are SBO apart
-//                    (1024 B for a dense tile); LBO is unused for swizzled K-major (encoded as 1).
+//                    (1024 B for a dense tile); LBO is unused for swizzled K-major (encoded as 1).  The
+//                    k-th 16-element slice of a 64-wide chunk starts 32*k bytes into the tile.
 // MN-major operand : 64 MN-elements are contiguous (one 128 B row), consecutive K indices are 128 B
 //                    apart inside a group of 8, groups of 8 K are SBO apart (1024 B dense), and the
 //                    next 64 MN-elements start LBO bytes further.
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-
-// The same descriptor split in two 32-bit words, for issue loops that only advance the start address:
-//   lo = start address >> 4 | (LBO >> 4) << 16        hi = SBO >> 4 | version 1 | SWIZZLE_128B
-__device__ __forceinline__ uint32_t umma_desc_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return ((smem_addr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
+// Orders register accesses of the accumulators before the wgmma that follows (whole warpgroup).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory");
 }
-__host__ __device__ constexpr uint32_t umma_desc_hi(uint32_t sbo_bytes) {
-  return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14) | (2u << 29);
-}
-__device__ __forceinline__ void tc_mma_ss_lh(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo,
-                                             uint32_t b_hi, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}\n"
-      ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_mma_ts_lh(uint32_t d_tmem, uint32_t a_tmem, uint32_t b_lo, uint32_t b_hi,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 db;\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %4, p;\n\t}\n"
-      ::"r"(d_tmem), "r"(a_tmem), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Instruction descriptor for kind::f16 with fp16 operands and an fp32 accumulator.
-//   [4,6) D format (1 = f32)   [7,10) A format (0 = f16)   [10,13) B format (0 = f16)
-//   [15] A major (0 = K)       [16] B major (0 = K, 1 = MN)  [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t M, uint32_t N, uint32_t b_mn_major) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (0u << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
+// Keeps the compiler from moving accesses of an accumulator register across wgmma issue / wait.
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
 
 // ------------------------------------------------------------------------------------------
@@ -304,11 +159,6 @@ __device__ __forceinline__ uint32_t pack_f16x2_rn(float lo, float hi) {
   uint32_t r;
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));   // d = {hi: first src, lo: second src}
   return r;
-}
-__device__ __forceinline__ float fmax3(float a, float b, float c) {     // FMNMX3 (sm_100+): one instruction
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
 }
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;

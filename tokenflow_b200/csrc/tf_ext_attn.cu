@@ -9,18 +9,21 @@
 // 40-frame SD1.5 top level), replicates K and V n times and shuffles heads through ~10 copies
 // (SURVEY.md §2.1 k1-k6).  Here none of that exists: one CTA owns a 128-query tile of one
 // (sample, head), streams the key/value tiles of every attended keyframe through shared memory
-// with TMA, keeps scores, probabilities and the output accumulator in tensor memory, and addresses
+// with TMA, keeps scores, probabilities and the output accumulator in registers, and addresses
 // heads by stride inside the [sample, S, heads, d] tensors.  PnP q/k injection (:124-130) is pure
 // aliasing: the per-sample table names which q / k slab to read.
 //
-// CTA = 6 warps:   warp 0  TMA producer (Q tile once, then a ring of {K tile, V tile} stages)
-//                  warp 1  tcgen05.mma issuer:  S[b] = Q K_t^T (SS),  O += P_t V_t (TS, P read from TMEM)
-//                  warps 2-5  softmax, one thread per query row: tcgen05.ld S -> running max / exp2 /
-//                             row sum -> fp16 P written back over S with tcgen05.st; lazy O rescale
-//                             (only when the running max grows by > 2^8, FA4-style); final O / l.
-// TMEM (512 cols): S/P buffers 2 x kBlockN fp32 columns, O accumulator d_pad columns.
-// QK(t+1) is issued before PV(t) waits for P(t), so the tensor pipe computes the next score tile
-// while the softmax warps work on the current one.
+// CTA = 2 warpgroups, 64 query rows each (FlashAttention-2 online softmax, fp32 statistics):
+//   S = Q K_t^T      wgmma, both operands from shared memory (K-major, 128-byte swizzle)
+//   P = exp2(S * scale*log2e - m)   in registers, rounded to fp16 into the wgmma A-fragment layout
+//   O += P V_t       wgmma, P from registers, V from shared memory (MN-major)
+// Thread 0 also issues the TMA loads: the Q tile once, then a ring of {K tile, V tile} stages; a
+// stage is refilled one tile after both warpgroups released it, so neither waits on the other.
+// The two warpgroups' softmax and MMA phases interleave on the SM.
+//
+// Paired samples (PnP q/k injection: the uncond and cond sample of a keyframe share q and k, so
+// their scores and probabilities are identical): one CTA computes P once and P V_u, P V_c into two
+// accumulators.
 //
 // Head dims that are not a multiple of 64 (SD1.5: 40, 80, 160) are zero-padded by TMA out-of-bound
 // fill: the tensor maps describe [d, heads, S, samples] with the true inner extent d and a 64-wide
@@ -28,47 +31,30 @@
 //
 // Roofline: tensor-bound, 4*S_q*S_kv*d flops per (sample, head); HBM traffic is q,k,v,out once
 // (K/V tiles re-read by the other query tiles hit L2).
-#include <cstdlib>
+#include <cmath>
 #include <type_traits>
 
 #include "tf_common.cuh"
 #include "tf_kernels.h"
+#include "tf_wgmma.cuh"
 
 namespace tf {
 namespace {
 
 constexpr int kBlockM = 128;
-constexpr float kRescaleThreshold = 8.0f;
-
-// Optional event trace (build with -DTF_TRACE): clock64 stamps of CTA 0's roles for the first tiles.
-// layout: g_attn_trace[role][tile][event], role 0/1 = softmax tile A/B (warp quadrant 0, lane 0), 2 = MMA issuer
-#ifdef TF_TRACE
-constexpr int kTraceTiles = 40, kTraceEvents = 8;
-__device__ long long g_attn_trace[3 * kTraceTiles * kTraceEvents];
-#define TF_TRACE_EV(role, tile, ev)                                                              \
-  do {                                                                                           \
-    if (blockIdx.x == 0 && (tile) < kTraceTiles)                                                 \
-      g_attn_trace[((role) * kTraceTiles + (tile)) * kTraceEvents + (ev)] = clock64();           \
-  } while (0)
-#else
-#define TF_TRACE_EV(role, tile, ev) do {} while (0)
-#endif      // log2 units: P stays <= 2^8 without touching O
+constexpr int kMaxStages = 8;
+constexpr int kSmemBudget = 227 * 1024;
 
 struct AttnCtl {
   uint64_t q_full;
-  uint64_t kv_full[8];
-  uint64_t kv_empty[8];
-  uint64_t s_full[2];
-  uint64_t p_full[2];
-  uint64_t pv_done;
-  uint32_t tmem_base;
+  uint64_t full[kMaxStages];
+  uint64_t empty[kMaxStages];
 };
 
 struct AttnParams {
-  int S, heads, d, n_out;
+  int S, heads, d;
   int tiles_m;            // query tiles per (sample, head)
   int stages;
-  int handoff;            // ping-pong kernel: chunk index after which the MUFU token is handed over
   float scale_log2;       // scale * log2(e)
   long long out_tok_stride;   // elements between consecutive tokens of `out` (= heads*d)
   int q_row0;             // first query token this launch computes (multi-GPU: query rows are split across ranks)
@@ -76,20 +62,35 @@ struct AttnParams {
   int out_rows;           // rows per slab of `out`: out is [slabs, out_rows, heads*d], row = token - q_row0
 };
 
-template <int kDChunks, int kBlockN>
-__global__ void __launch_bounds__(192, 1)
+// One CTA's sample, single or paired (out_c / v_c0 unused for a single sample).
+struct Item {
+  int out_u, out_c, q, k0, v_u0, v_c0, n_kv;
+};
+__device__ __forceinline__ Item item_of(const AttnTable& t, int i) {
+  const AttnSample& s = t.s[i];
+  return {s.out_sample, -1, s.q_sample, s.k_sample0, s.v_sample0, -1, s.n_kv};
+}
+__device__ __forceinline__ Item item_of(const AttnPairTable& t, int i) {
+  const AttnPair& p = t.p[i];
+  return {p.out_u, p.out_c, p.q_sample, p.k_sample0, p.v_u0, p.v_c0, p.n_kv};
+}
+
+// kDChunks: 64-channel chunks of the head dim; kBlockN: keys per tile; kNPV: head dim rounded up to 16
+// (N of the P V MMA).
+template <int kDChunks, int kBlockN, int kNPV, class Tab>
+__global__ void __launch_bounds__(256, 1)
 ext_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-                const __grid_constant__ CUtensorMap map_v, const AttnTable tab, const AttnParams prm,
+                const __grid_constant__ CUtensorMap map_v, const __grid_constant__ Tab tab, const AttnParams prm,
                 __half* __restrict__ out) {
+  constexpr int kNV = std::is_same<Tab, AttnPairTable>::value ? 2 : 1;   // value tensors per stage
   constexpr int kQChunkBytes = kBlockM * 128;
   constexpr int kKVChunkBytes = kBlockN * 128;
   constexpr int kQBytes = kDChunks * kQChunkBytes;
   constexpr int kTileBytes = kDChunks * kKVChunkBytes;         // one K tile or one V tile
-  constexpr int kStageBytes = 2 * kTileBytes;
-  constexpr int kSCols = kBlockN;                               // fp32 score columns per buffer
-  constexpr int kOCol = 2 * kSCols;                             // O accumulator starts after the S buffers
-  constexpr int kDPad = 64 * kDChunks;
-  static_assert(kOCol + kDPad <= 512, "tensor memory overflow");
+  constexpr int kStageBytes = (1 + kNV) * kTileBytes;
+  constexpr int kS = kBlockN / 2;                               // score registers per thread
+  constexpr int kO = kNPV / 2;                                  // output registers per thread and value tensor
+  static_assert(kNPV <= 64 * kDChunks, "P V width exceeds the loaded channels");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -100,2155 +101,196 @@ ext_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
   // ---- work item: heavy (extended) samples first so the tail of the grid is made of light items ----
   const int S = prm.S, d = prm.d, stages = prm.stages;
   const int per_sample = prm.heads * prm.tiles_m;
-  const int sample_slot = blockIdx.x / per_sample;
-  const int rem = blockIdx.x - sample_slot * per_sample;
+  const int slot = blockIdx.x / per_sample;
+  const int rem = blockIdx.x - slot * per_sample;
   const int head = rem / prm.tiles_m;
   const int m0 = prm.q_row0 + (rem - head * prm.tiles_m) * kBlockM;
-  const AttnSample smp = tab.s[sample_slot];
-  const int out_sample = smp.out_sample;
-  const int q_slab = smp.q_sample;
+  const Item it = item_of(tab, slot);
   const int tiles_per_slab = (S + kBlockN - 1) / kBlockN;
-  const int T = smp.n_kv * tiles_per_slab;
+  const int T = it.n_kv * tiles_per_slab;
   const int ksteps = (d + 15) / 16;                             // QK^T k-steps (zero padded to 16)
-  const int n_pv = ((d + 15) / 16) * 16;                        // PV MMA N (multiple of 16)
 
-  const int warp = threadIdx.x >> 5;
-  if (warp == 0 && elect_one()) {
+  auto load_tile = [&](int t) {
+    const int st = t % stages;
+    const int slab = t / tiles_per_slab;
+    const int n0 = (t - slab * tiles_per_slab) * kBlockN;
+    uint8_t* dst = ring + st * kStageBytes;
+    mbar_arrive_expect_tx(&ctl->full[st], (uint32_t)kStageBytes);
+#pragma unroll
+    for (int c = 0; c < kDChunks; ++c) {
+      tma_load_4d(dst + c * kKVChunkBytes, &map_k, &ctl->full[st], c * 64, head, n0, it.k0 + slab);
+      tma_load_4d(dst + kTileBytes + c * kKVChunkBytes, &map_v, &ctl->full[st], c * 64, head, n0, it.v_u0 + slab);
+      if (kNV == 2)
+        tma_load_4d(dst + 2 * kTileBytes + c * kKVChunkBytes, &map_v, &ctl->full[st], c * 64, head, n0,
+                    it.v_c0 + slab);
+    }
+  };
+
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_q);
     tma_prefetch_desc(&map_k);
     tma_prefetch_desc(&map_v);
     mbar_init(&ctl->q_full, 1);
     for (int i = 0; i < stages; ++i) {
-      mbar_init(&ctl->kv_full[i], 1);
-      mbar_init(&ctl->kv_empty[i], 1);
+      mbar_init(&ctl->full[i], 1);
+      mbar_init(&ctl->empty[i], 8);                             // one arrival per warp
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&ctl->s_full[i], 1);
-      mbar_init(&ctl->p_full[i], 4);
-    }
-    mbar_init(&ctl->pv_done, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(&ctl->tmem_base, 512);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = ctl->tmem_base;
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(&ctl->q_full, (uint32_t)kQBytes);
+#pragma unroll
+    for (int c = 0; c < kDChunks; ++c) tma_load_4d(q_smem + c * kQChunkBytes, &map_q, &ctl->q_full, c * 64, head, m0, it.q);
+    for (int t = 0; t < stages && t < T; ++t) load_tile(t);
+  }
+  __syncwarp();
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      mbar_arrive_expect_tx(&ctl->q_full, (uint32_t)kQBytes);
+  const int wg = threadIdx.x >> 7;
+  const int lane = threadIdx.x & 31;
+  const int wrow = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // first of the thread's two rows in the warpgroup
+  const int qcol = 2 * (lane & 3);                                // first of the thread's two columns in an n8 block
+
+  float o[kNV][kO];
 #pragma unroll
-      for (int c = 0; c < kDChunks; ++c)
-        tma_load_4d(q_smem + c * kQChunkBytes, &map_q, &ctl->q_full, c * 64, head, m0, q_slab);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = 0; t < T; ++t) {
-        const int slab = t / tiles_per_slab;
-        const int n0 = (t - slab * tiles_per_slab) * kBlockN;
-        mbar_wait(&ctl->kv_empty[stage], phase ^ 1);
-        uint8_t* st = ring + stage * kStageBytes;
-        mbar_arrive_expect_tx(&ctl->kv_full[stage], (uint32_t)kStageBytes);
+  for (int v = 0; v < kNV; ++v)
 #pragma unroll
-        for (int c = 0; c < kDChunks; ++c) {
-          tma_load_4d(st + c * kKVChunkBytes, &map_k, &ctl->kv_full[stage], c * 64, head, n0, smp.k_sample0 + slab);
-          tma_load_4d(st + kTileBytes + c * kKVChunkBytes, &map_v, &ctl->kv_full[stage], c * 64, head, n0,
-                      smp.v_sample0 + slab);
-        }
-        if (++stage == stages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const uint32_t idesc_qk = umma_idesc_f16(128, kBlockN, 0);
-    const uint32_t idesc_pv = umma_idesc_f16(128, (uint32_t)n_pv, 1);     // B = V tile, MN-major
-    const uint32_t q_addr = smem_u32(q_smem);
-    auto issue_qk = [&](int t, int stage) {        // S[t&1] = Q K_t^T
-      const uint32_t k_addr = smem_u32(ring + stage * kStageBytes);
-      const uint32_t s_tmem = tmem_base + (uint32_t)((t & 1) * kSCols);
-      for (int ks = 0; ks < ksteps; ++ks) {
-        const int c = ks >> 2, k4 = ks & 3;
-        const uint64_t da = umma_smem_desc(q_addr + c * kQChunkBytes + k4 * 32, 16, 1024);
-        const uint64_t db = umma_smem_desc(k_addr + c * kKVChunkBytes + k4 * 32, 16, 1024);
-        tc_mma_ss(s_tmem, da, db, idesc_qk, ks > 0 ? 1u : 0u);
-      }
-      tc_commit(&ctl->s_full[t & 1]);
-    };
-    mbar_wait(&ctl->q_full, 0);
-    mbar_wait(&ctl->kv_full[0], 0);
-    tc_fence_after_sync();
-    if (elect_one()) issue_qk(0, 0);
+    for (int i = 0; i < kO; ++i) o[v][i] = 0.f;
+  float m_r[2] = {-INFINITY, -INFINITY}, l_r[2] = {0.f, 0.f};
+  const float sl2 = prm.scale_log2;
+
+  const uint32_t q_addr = smem_u32(q_smem) + wg * 64 * 128;
+  const uint32_t ring_addr = smem_u32(ring);
+  mbar_wait(&ctl->q_full, 0);
+  __syncwarp();
+
+  for (int t = 0; t < T; ++t) {
+    const int st = t % stages;
+    mbar_wait(&ctl->full[st], (uint32_t)(t / stages) & 1u);
     __syncwarp();
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int t = 0; t < T; ++t) {
-      int nstage = stage + 1;
-      uint32_t nphase = phase;
-      if (nstage == stages) { nstage = 0; nphase ^= 1; }
-      if (t + 1 < T) {                              // next score tile first: overlaps softmax(t)
-        mbar_wait(&ctl->kv_full[nstage], nphase);
-        tc_fence_after_sync();
-        if (elect_one()) issue_qk(t + 1, nstage);
-        __syncwarp();
-      }
-      mbar_wait(&ctl->p_full[t & 1], (uint32_t)((t >> 1) & 1));
-      tc_fence_after_sync();
-      if (elect_one()) {                            // O (+)= P_t V_t,  P_t = fp16 [128 x kBlockN] in TMEM
-        const uint32_t v_addr = smem_u32(ring + stage * kStageBytes + kTileBytes);
-        const uint32_t p_tmem = tmem_base + (uint32_t)((t & 1) * kSCols);
-#pragma unroll
-        for (int k = 0; k < kBlockN / 16; ++k) {
-          const uint64_t db = umma_smem_desc(v_addr + k * (16 * 128), (uint32_t)kKVChunkBytes, 1024);
-          tc_mma_ts(tmem_base + kOCol, p_tmem + k * 8, db, idesc_pv, (t > 0 || k > 0) ? 1u : 0u);
-        }
-        tc_commit(&ctl->kv_empty[stage]);
-        tc_commit(&ctl->pv_done);
-      }
-      __syncwarp();
-      stage = nstage;
-      phase = nphase;
+    const uint32_t k_addr = ring_addr + st * kStageBytes;
+
+    // ---- S = Q K^T ----
+    float s[kS];
+    wgmma_fence();
+    for (int kk = 0; kk < ksteps; ++kk) {
+      const uint32_t off = (kk & 3) * 32;
+      wgmma_ss<kBlockN>(s, wgmma_desc(q_addr + (kk >> 2) * kQChunkBytes + off, 16, 1024),
+                        wgmma_desc(k_addr + (kk >> 2) * kKVChunkBytes + off, 16, 1024), kk > 0 ? 1u : 0u);
     }
-  } else {
-    // ===================== softmax / correction / epilogue: one thread per query row ==============
-    const int quad = warp & 3;
-    const int row = quad * 32 + (int)lane_id();
-    const uint32_t t_lane = (uint32_t)(quad * 32) << 16;
-    const float sl2 = prm.scale_log2;
-    float m_run = 0.f;       // running max in scaled log2 units
-    float l_run = 0.f;
-    for (int t = 0; t < T; ++t) {
-      const int slab_tile = t % tiles_per_slab;
-      const int valid = min(kBlockN, S - slab_tile * kBlockN);   // key columns of this tile inside the slab
-      const uint32_t s_addr = tmem_base + t_lane + (uint32_t)((t & 1) * kSCols);
-      mbar_wait(&ctl->s_full[t & 1], (uint32_t)((t >> 1) & 1));
-      tc_fence_after_sync();
-      // ---- pass 1: tile max ----
-      float mt = -INFINITY;
-#pragma unroll 1
-      for (int c0 = 0; c0 < kBlockN; c0 += 32) {
-        if (c0 >= valid) break;
-        uint32_t v[32];
-        tmem_ld32(s_addr + c0, v);
-        tmem_wait_ld();
-        if (valid - c0 >= 32) {
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+
+    // ---- keys past the end of the keyframe (ragged last tile of a slab) ----
+    const int n0 = (t % tiles_per_slab) * kBlockN;
+    if (n0 + kBlockN > S) {
+      const int valid = S - n0;
 #pragma unroll
-          for (int i = 0; i < 32; ++i) mt = fmaxf(mt, __uint_as_float(v[i]));
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) if (c0 + i < valid) mt = fmaxf(mt, __uint_as_float(v[i]));
-        }
-      }
-      const float mt_s = mt * sl2;
-      if (t == 0) {
-        m_run = mt_s;
-      } else {
-        const bool need = mt_s > m_run + kRescaleThreshold;
-        if (__any_sync(0xffffffffu, need)) {       // warp-uniform: tcgen05.ld/st are warp-collective
-          mbar_wait(&ctl->pv_done, (uint32_t)((t - 1) & 1));     // PV(t-1) retired: O is quiescent
-          tc_fence_after_sync();
-          const float m_new = fmaxf(m_run, mt_s);
-          const float alpha = fast_exp2(m_run - m_new);
-          l_run *= alpha;
-          m_run = m_new;
-          for (int c0 = 0; c0 < n_pv; c0 += 16) {
-            uint32_t o[16];
-            tmem_ld16(tmem_base + t_lane + kOCol + c0, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(tmem_base + t_lane + kOCol + c0, o);
-          }
-          tmem_wait_st();
-        }
-      }
-      // ---- pass 2: p = 2^(s*scale*log2e - m), row sum, fp16 P written over the score columns ----
-      float lsum = 0.f;
-#pragma unroll 1
-      for (int c0 = 0; c0 < kBlockN; c0 += 32) {
-        uint32_t pk[16];
-        if (c0 < valid) {
-          uint32_t v[32];
-          tmem_ld32(s_addr + c0, v);
-          tmem_wait_ld();
-          float p[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            p[i] = fast_exp2(fmaf(__uint_as_float(v[i]), sl2, -m_run));
-            if (valid - c0 < 32 && c0 + i >= valid) p[i] = 0.f;
-            lsum += p[i];
-          }
-#pragma unroll
-          for (int i = 0; i < 16; ++i) pk[i] = pack_f16x2_rn(p[2 * i], p[2 * i + 1]);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) pk[i] = 0u;
-        }
-        tmem_st16(s_addr + (c0 >> 1), pk);
-      }
-      l_run += lsum;
-      tmem_wait_st();
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane_id() == 0) mbar_arrive(&ctl->p_full[t & 1]);
-    }
-    // ---- final: O / l -> fp16 -> out[sample, p, head, :] ----
-    mbar_wait(&ctl->pv_done, (uint32_t)((T - 1) & 1));
-    tc_fence_after_sync();
-    const float inv_l = 1.0f / l_run;
-    const int p_tok = m0 + row;
-    __half* orow = out + ((long long)out_sample * prm.out_rows + (p_tok - prm.q_row0)) * prm.out_tok_stride + (long long)head * d;
-    for (int c0 = 0; c0 < n_pv; c0 += 16) {
-      uint32_t o[16];
-      tmem_ld16(tmem_base + t_lane + kOCol + c0, o);
-      tmem_wait_ld();
-      if (p_tok < prm.q_row_end) {
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          if (c0 + g * 8 < d) {                     // d is a multiple of 8: whole 16-byte groups
-            uint4 w;
-            w.x = pack_f16x2_rn(__uint_as_float(o[g * 8 + 0]) * inv_l, __uint_as_float(o[g * 8 + 1]) * inv_l);
-            w.y = pack_f16x2_rn(__uint_as_float(o[g * 8 + 2]) * inv_l, __uint_as_float(o[g * 8 + 3]) * inv_l);
-            w.z = pack_f16x2_rn(__uint_as_float(o[g * 8 + 4]) * inv_l, __uint_as_float(o[g * 8 + 5]) * inv_l);
-            w.w = pack_f16x2_rn(__uint_as_float(o[g * 8 + 6]) * inv_l, __uint_as_float(o[g * 8 + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(orow + c0 + g * 8) = w;
-          }
-        }
+      for (int j = 0; j < kBlockN / 8; ++j) {
+        const int c = 8 * j + qcol;
+        if (c >= valid) { s[4 * j] = -INFINITY; s[4 * j + 2] = -INFINITY; }
+        if (c + 1 >= valid) { s[4 * j + 1] = -INFINITY; s[4 * j + 3] = -INFINITY; }
       }
     }
-  }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-
-// ================================================================================================
-// Ping-pong kernel (head dim <= 64): two 128-query tiles per CTA.
-//
-// The softmax inner loop is MUFU-bound on this chip (ex2: 8.1 cycles per warp instruction per SM
-// sub-partition, profiles/r01_pipe_throughput_ubench.txt; at d = 40 the two MMAs of a 128x128 tile
-// need only ~450 tensor cycles against ~1040 MUFU cycles), and a tcgen05.mma costs its issuing thread
-// 45-100 cycles whatever its shape (profiles/r01_ext_attn_trace.md).  The structure follows from that:
-//   * two query tiles A and B share every K/V tile (fetched once per 256 queries);
-//   * one MMA-issuer warp per query tile, so the two issue streams run in parallel; operands stay
-//     warp-uniform so ptxas emits back-to-back UTCHMMA;
-//   * each softmax thread holds its whole score row in registers (one TMEM read per tile), takes the
-//     row max with FMNMX3, rescales O lazily, writes fp16 P over the score columns and keeps the row
-//     sum in a register;
-//   * the two softmax warps that share an SM sub-partition (and its MUFU) take turns in their exp2
-//     phase through an mbarrier token, handed over at 3/4 of the loop.
-// kBlockN = 128 (default): one score buffer per query tile, S_X[t+1] issued right after P_X[t] V_t.
-// kBlockN = 64: two score buffers per query tile, S_X[t+2] issued after P_X[t] V_t (more, smaller MMAs:
-// measured slower at d = 40; kept selectable with TF_EXT_ATTN_MODE=pp64).
-//   warp 0: TMA   warps 1,2: MMA issue for tile A / B   warp 3: spare   warps 4-7: softmax A   warps 8-11: softmax B
-// TMEM: score buffers [0,256), O_A [256,320), O_B [320,384)
-// ================================================================================================
-constexpr int kPPStagesMax = 12;
-constexpr bool kDefaultOnes = true;        // measured choices (profiles/r02_ext_attn_variants.md)
-constexpr int kDefaultPolyOnes = 3, kDefaultPoly = 4, kDefaultPolyPair = 4, kDefaultPolyH2 = 3;
-constexpr bool kDefaultOneTile = false;
-constexpr int kDefaultTurn = 0;
-struct AttnCtl2 {
-  uint64_t q_full;
-  uint64_t kv_full[kPPStagesMax];
-  uint64_t kv_empty[kPPStagesMax];
-  uint64_t s_full[2][2];
-  uint64_t p_full[2][2];
-  uint64_t xu_turn[2][4];    // [next tile X][SM sub-partition]: exp2-phase token passed between the two softmax
-                             // warps that share a sub-partition (and therefore its MUFU)
-  uint64_t pv_done[2][2];    // [tile X][t & 1]: two alternating barriers, so a softmax warp that runs two
-                             // tiles ahead of the tensor pipe can still name "P V of tile t" unambiguously
-  uint64_t v_ready[kPPStagesMax];   // kOnes: the V tile of this stage carries its column of ones (warp 3)
-  uint32_t tmem_base;
-};
-
-// 2^x for x <= ~2^8 on the FMA/ALU pipes (no MUFU): Cody-Waite split x = n + r with the round-to-nearest
-// magic constant, degree-3 minimax polynomial for 2^r on [-0.5, 0.5] (max relative error 1.0e-4, five times
-// below the fp16 rounding the probabilities get anyway), exponent inserted with one shift-add.
-__device__ __forceinline__ float poly_exp2(float x) {
-  x = fmaxf(x, -125.0f);                               // keeps the exponent arithmetic in range (and -inf -> ~0)
-  const float t = x + 12582912.0f;                     // 1.5 * 2^23: integer part of x in the low mantissa bits
-  const float r = x - (t - 12582912.0f);               // r in [-0.5, 0.5]
-  float p = fmaf(0.05500871315598488f, r, 0.24221068620681763f);
-  p = fmaf(p, r, 0.6932829022407532f);
-  p = fmaf(p, r, 1.0f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
-}
-// which of 16 consecutive row elements take the polynomial: k of 16, evenly spread
-__host__ __device__ constexpr bool poly_slot(int e, int k16) { return ((e % 16 + 1) * k16) / 16 != ((e % 16) * k16) / 16; }
-
-// kPoly16: of every 16 probabilities, this many are evaluated with poly_exp2 instead of MUFU.EX2 (the exp2
-//          loop is MUFU-bound at small head dims; FA4-style split of the work over two pipes).
-// kOnes:   row sums by the tensor core — warp 3 writes 1.0 into the (zero padded) column d of every V tile, so
-//          column d of the O accumulator is sum_c P[:, c]; needs d % 16 != 0 (a free padding column inside the
-//          P V MMA's N).  Saves one FADD per probability on the FMA pipe that the polynomial needs.
-template <int kBlockN, int kPoly16, bool kOnes>
-__global__ void __launch_bounds__(384, 1)
-ext_attn_pp_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-                   const __grid_constant__ CUtensorMap map_v, const AttnTable tab, const AttnParams prm,
-                   __half* __restrict__ out) {
-  constexpr int kNBuf = 128 / kBlockN;                // score buffers per query tile (TMEM columns [0,256) in total)
-  constexpr int kChunks = kBlockN / 32;
-  constexpr int kQTileBytes = kBlockM * 128;          // one 128-query tile, 64-wide d chunk
-  constexpr int kQBytes = 2 * kQTileBytes;
-  constexpr int kOnesBytes = 0;
-  constexpr int kTileBytes = kBlockN * 128;
-  constexpr int kStageBytes = 2 * kTileBytes;
-  constexpr int kOCol = 256;
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* q_smem = smem;
-  uint8_t* ring = smem + kQBytes + kOnesBytes;
-  AttnCtl2* ctl = reinterpret_cast<AttnCtl2*>(ring + prm.stages * kStageBytes);
-
-  const int S = prm.S, d = prm.d, stages = prm.stages;
-  const int per_sample = prm.heads * prm.tiles_m;              // tiles_m = 256-query tile pairs here
-  const int sample_slot = blockIdx.x / per_sample;
-  const int rem = blockIdx.x - sample_slot * per_sample;
-  const int head = rem / prm.tiles_m;
-  const int m0 = prm.q_row0 + (rem - head * prm.tiles_m) * (2 * kBlockM);
-  const AttnSample smp = tab.s[sample_slot];
-  const int tiles_per_slab = (S + kBlockN - 1) / kBlockN;
-  const int T = smp.n_kv * tiles_per_slab;
-  const int ksteps = (d + 15) / 16;
-  const int n_pv = ((d + 15) / 16) * 16;
-
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&map_q);
-    tma_prefetch_desc(&map_k);
-    tma_prefetch_desc(&map_v);
-    mbar_init(&ctl->q_full, 1);
-    for (int i = 0; i < stages; ++i) {
-      mbar_init(&ctl->kv_full[i], 1);
-      mbar_init(&ctl->kv_empty[i], 2);
-      mbar_init(&ctl->v_ready[i], 1);
+    // ---- online softmax (log2 domain) ----
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int j = 0; j < kBlockN / 8; ++j) {
+      mx[0] = fmaxf(mx[0], fmaxf(s[4 * j], s[4 * j + 1]));
+      mx[1] = fmaxf(mx[1], fmaxf(s[4 * j + 2], s[4 * j + 3]));
     }
-    for (int x = 0; x < 2; ++x) {
-      for (int b = 0; b < 2; ++b) {
-        mbar_init(&ctl->s_full[x][b], 1);
-        mbar_init(&ctl->p_full[x][b], 4);
-      }
-      mbar_init(&ctl->pv_done[x][0], 1);
-      mbar_init(&ctl->pv_done[x][1], 1);
-      for (int qd = 0; qd < 4; ++qd) mbar_init(&ctl->xu_turn[x][qd], 1);
+    float corr[2], mneg[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float m_new = fmaxf(m_r[r], mx[r] * sl2);
+      corr[r] = fast_exp2(m_r[r] - m_new);
+      m_r[r] = m_new;
+      mneg[r] = -m_new;
+      l_r[r] *= corr[r];
     }
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc(&ctl->tmem_base, 512);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, ctl->tmem_base, 0);     // warp-uniform for the compiler
-
-  // register budgets: the 4 service warps (TMA, 2 MMA issuers, ones writer) need few registers, the 8 softmax
-  // warps hold a 128-element score row each plus the polynomial's temporaries: 4*32*96 + 8*32*200 = 62 K registers
-  if (warp < 4) {
-  warpgroup_reg_dec<96>();
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      mbar_arrive_expect_tx(&ctl->q_full, (uint32_t)kQBytes);
-      tma_load_4d(q_smem, &map_q, &ctl->q_full, 0, head, m0, smp.q_sample);
-      tma_load_4d(q_smem + kQTileBytes, &map_q, &ctl->q_full, 0, head, m0 + kBlockM, smp.q_sample);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = 0; t < T; ++t) {
-        const int slab = t / tiles_per_slab;
-        const int n0 = (t - slab * tiles_per_slab) * kBlockN;
-        mbar_wait(&ctl->kv_empty[stage], phase ^ 1);
-        uint8_t* st = ring + stage * kStageBytes;
-        mbar_arrive_expect_tx(&ctl->kv_full[stage], (uint32_t)kStageBytes);
-        tma_load_4d(st, &map_k, &ctl->kv_full[stage], 0, head, n0, smp.k_sample0 + slab);
-        tma_load_4d(st + kTileBytes, &map_v, &ctl->kv_full[stage], 0, head, n0, smp.v_sample0 + slab);
-        if (++stage == stages) { stage = 0; phase ^= 1; }
-      }
+    uint32_t pa[kBlockN / 16][4];
+#pragma unroll
+    for (int j = 0; j < kBlockN / 8; ++j) {
+      const float p0 = fast_exp2(fmaf(s[4 * j], sl2, mneg[0]));
+      const float p1 = fast_exp2(fmaf(s[4 * j + 1], sl2, mneg[0]));
+      const float p2 = fast_exp2(fmaf(s[4 * j + 2], sl2, mneg[1]));
+      const float p3 = fast_exp2(fmaf(s[4 * j + 3], sl2, mneg[1]));
+      l_r[0] += p0 + p1;
+      l_r[1] += p2 + p3;
+      pa[j >> 1][(j & 1) * 2 + 0] = pack_f16x2_rn(p0, p1);
+      pa[j >> 1][(j & 1) * 2 + 1] = pack_f16x2_rn(p2, p3);
     }
-  } else if (warp == 1 || warp == 2) {
-    // ===================== MMA issuers: one warp per query tile (warp 1 -> A, warp 2 -> B) ==============
-    // Measured (profiles/r01_ext_attn_trace.md): with one issuer serving both query tiles the issue path
-    // (8 small P V MMAs + 3 Q K^T MMAs + commits + barrier polls per tile and query tile) was the
-    // bottleneck and the softmax warps spent half their time waiting for the next score tile.  Two
-    // issuers run the two streams in parallel (all hazards — P_X[t] V before S_X[t+kNBuf] — are inside
-    // one stream).  Control flow and operands stay warp-uniform (the whole warp runs the loop, values
-    // derive from shfl-broadcast / kernel parameters) so that ptxas keeps descriptors in uniform
-    // registers and emits back-to-back UTCHMMA instead of an ELECT/R2UR loop around every MMA.
-    const int X = warp - 1;
-    const uint32_t idesc_qk = umma_idesc_f16(128, kBlockN, 0);
-    const uint32_t idesc_pv = umma_idesc_f16(128, (uint32_t)n_pv, 1);
-    constexpr uint32_t hi_kmaj = umma_desc_hi(1024);
-    const uint32_t q_lo = umma_desc_lo(smem_u32(q_smem + X * kQTileBytes), 16);
-    const uint32_t ring_k_lo = umma_desc_lo(smem_u32(ring), 16);                       // K tile of stage 0
-    const uint32_t ring_v_lo = umma_desc_lo(smem_u32(ring + kTileBytes), kTileBytes);  // V tile of stage 0
-    constexpr uint32_t kStageStep = kStageBytes >> 4;
-    const uint32_t o_tmem = tmem_base + kOCol + X * 64;
-    // S_X[buf] = Q_X K^T against the K tile in ring stage `st` (called by the elected lane only)
-    auto issue_qk = [&](int st, int buf) {
-      const uint32_t k_lo = ring_k_lo + (uint32_t)st * kStageStep;
-      const uint32_t s_tmem = tmem_base + (uint32_t)((X * kNBuf + buf) * kBlockN);
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks)               // head dim <= 64: at most 4 k-steps of 16
-        if (ks < ksteps) tc_mma_ss_lh(s_tmem, q_lo + ks * 2, hi_kmaj, k_lo + ks * 2, hi_kmaj, idesc_qk, ks > 0 ? 1u : 0u);
-      tc_commit(&ctl->s_full[X][buf]);
-    };
-    mbar_wait(&ctl->q_full, 0);
-    // Tile B starts once tile A's first probabilities have arrived: that staggers the two softmax warps
-    // of every SM sub-partition by about half a period instead of letting them convoy.
-    if (X == 1) mbar_wait(&ctl->p_full[0][0], 0);
-    // ring position of the next K tile to be used by a Q K^T (tile t + kNBuf in the main loop)
-    int qk_stage = 0;
-    uint32_t qk_phase = 0;
-    for (int t0 = 0; t0 < kNBuf && t0 < T; ++t0) {
-      mbar_wait(&ctl->kv_full[qk_stage], qk_phase);
-      tc_fence_after_sync();
-      if (elect_one()) issue_qk(qk_stage, t0);
-      __syncwarp();
-      if (++qk_stage == stages) { qk_stage = 0; qk_phase ^= 1; }
-    }
-    int stage = 0;                                 // ring position of tile t (its V tile feeds P V)
-    uint32_t pv_phase = 0;
-    for (int t = 0; t < T; ++t) {
-      const int buf = t % kNBuf;                   // kNBuf is 1 or 2
-      const bool refill = t + kNBuf < T;
-      if (refill) mbar_wait(&ctl->kv_full[qk_stage], qk_phase);   // K tile of the refill, polled while idle anyway
-      if (kOnes) mbar_wait(&ctl->v_ready[stage], pv_phase);       // the V tile has its ones column
-      if (X == 0 && lane_id() == 0) TF_TRACE_EV(2, t, 0);
-      mbar_wait(&ctl->p_full[X][buf], (uint32_t)((t / kNBuf) & 1));
-      tc_fence_after_sync();
-      if (X == 0 && lane_id() == 0) TF_TRACE_EV(2, t, 1);
-      if (elect_one()) {
-        const uint32_t v_lo = ring_v_lo + (uint32_t)stage * kStageStep;
-        const uint32_t p_tmem = tmem_base + (uint32_t)((X * kNBuf + buf) * kBlockN);
+    for (int v = 0; v < kNV; ++v)
 #pragma unroll
-        for (int k = 0; k < kBlockN / 16; ++k)      // O_X (+)= P_X[:, 16k:16k+16] V[16k:16k+16, :]
-          tc_mma_ts_lh(o_tmem, p_tmem + k * 8, v_lo + k * 128, hi_kmaj, idesc_pv, (t > 0 || k > 0) ? 1u : 0u);
-        tc_commit(&ctl->pv_done[X][t & 1]);
-        tc_commit(&ctl->kv_empty[stage]);          // count 2: the stage is free once both tiles' MMAs retired
-        if (refill) issue_qk(qk_stage, buf);        // refill the score buffer P_X[t] vacates
+      for (int j = 0; j < kO / 4; ++j) {
+        o[v][4 * j] *= corr[0]; o[v][4 * j + 1] *= corr[0];
+        o[v][4 * j + 2] *= corr[1]; o[v][4 * j + 3] *= corr[1];
       }
-      __syncwarp();
-      if (X == 0 && lane_id() == 0) TF_TRACE_EV(2, t, 3);
-      if (++stage == stages) { stage = 0; pv_phase ^= 1; }
-      if (refill && ++qk_stage == stages) { qk_stage = 0; qk_phase ^= 1; }
-    }
-  } else if (warp == 3) {
-    // ===================== ones column (kOnes): V[:, d] = 1 so that O[:, d] accumulates the row sums ============
-    if constexpr (kOnes) {
-      const uint32_t col_byte = (uint32_t)d * 2u;                 // d % 8 == 0: the column starts a 16-byte chunk or its half
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = 0; t < T; ++t) {
-        mbar_wait(&ctl->kv_full[stage], phase);
-        uint8_t* vt = ring + stage * kStageBytes + kTileBytes;
-#pragma unroll
-        for (int r = (int)lane_id(); r < kBlockN; r += 32) {      // 128-byte swizzle: 16-byte chunk index ^ (row & 7)
-          const uint32_t off = (uint32_t)r * 128u + ((((col_byte >> 4) ^ ((uint32_t)r & 7u))) << 4) + (col_byte & 15u);
-          *reinterpret_cast<__half*>(vt + off) = __float2half_rn(1.0f);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the MMA
-        __syncwarp();
-        if (lane_id() == 0) mbar_arrive(&ctl->v_ready[stage]);
-        if (++stage == stages) { stage = 0; phase ^= 1; }
-      }
-    }
-  }
-  } else {                             // (warps 4..11 sit on TMEM lane quadrants warp % 4)
-    warpgroup_reg_inc<200>();
-    // ===================== softmax warps: tile X = (warp - 4) / 4 =====================
-    const int X = (warp - 4) >> 2;
-    const int quad = warp & 3;
-    const int row = quad * 32 + (int)lane_id();
-    const uint32_t t_lane = (uint32_t)(quad * 32) << 16;
-    const uint32_t o_addr = tmem_base + t_lane + kOCol + X * 64;
-    const float sl2 = prm.scale_log2;
-    float m_run = 0.f;
-    float l_run = 0.f;       // row sum of the (unrounded) probabilities, same scale as O
-    int slab_tile = 0;
-    for (int t = 0; t < T; ++t) {
-      const int valid = min(kBlockN, S - slab_tile * kBlockN);
-      if (++slab_tile == tiles_per_slab) slab_tile = 0;
-      const uint32_t s_addr = tmem_base + t_lane + (uint32_t)((X * kNBuf + (t % kNBuf)) * kBlockN);
-      const bool tracer = (quad == 0 && lane_id() == 0);
-      if (tracer) TF_TRACE_EV(X, t, 0);
-      mbar_wait(&ctl->s_full[X][t % kNBuf], (uint32_t)((t / kNBuf) & 1));
-      tc_fence_after_sync();
-      if (tracer) TF_TRACE_EV(X, t, 1);
-      uint32_t v[kChunks][32];
-#pragma unroll
-      for (int c = 0; c < kChunks; ++c) tmem_ld32(s_addr + 32 * c, v[c]);
-      tmem_wait_ld();
-      if (tracer) TF_TRACE_EV(X, t, 2);
-      if (valid < kBlockN) {                       // ragged last tile of a keyframe: mask the padding keys
-#pragma unroll
-        for (int c = 0; c < kChunks; ++c)
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (32 * c + i >= valid) v[c][i] = 0xFF800000u;
-      }
-      float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};     // 4 independent FMNMX3 chains
-#pragma unroll
-      for (int c = 0; c < kChunks; ++c)
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          mx[0] = fmax3(mx[0], __uint_as_float(v[c][i + 0]), __uint_as_float(v[c][i + 1]));
-          mx[1] = fmax3(mx[1], __uint_as_float(v[c][i + 2]), __uint_as_float(v[c][i + 3]));
-          mx[2] = fmax3(mx[2], __uint_as_float(v[c][i + 4]), __uint_as_float(v[c][i + 5]));
-          mx[3] = fmax3(mx[3], __uint_as_float(v[c][i + 6]), __uint_as_float(v[c][i + 7]));
-        }
-      const float mt = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-      const float mt_s = mt * sl2;
-      if (t == 0) {
-        m_run = mt_s;
-      } else {
-        const bool need = mt_s > m_run + kRescaleThreshold;
-        if (__any_sync(0xffffffffu, need)) {
-          mbar_wait(&ctl->pv_done[X][(t - 1) & 1], (uint32_t)(((t - 1) >> 1) & 1));   // P V of tile t-1 retired
-          tc_fence_after_sync();
-          const float m_new = fmaxf(m_run, mt_s);
-          const float alpha = fast_exp2(m_run - m_new);
-          m_run = m_new;
-          l_run *= alpha;
-          for (int c0 = 0; c0 < n_pv; c0 += 16) {
-            uint32_t o[16];
-            tmem_ld16(o_addr + c0, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(o_addr + c0, o);
-          }
-          tmem_wait_st();
-        }
-      }
-      if (tracer) TF_TRACE_EV(X, t, 3);
-      // exp2 phase, MUFU-bound: the two warps of a sub-partition take turns (A t, B t, A t+1, ...) instead
-      // of running their exp2 loops concurrently at half speed each and then idling together while the
-      // tensor pipe produces their next score tiles (profiles/r01_ext_attn_trace.md).
-      if (X == 0) {
-        if (t > 0) mbar_wait(&ctl->xu_turn[0][quad], (uint32_t)((t - 1) & 1));
-      } else {
-        mbar_wait(&ctl->xu_turn[1][quad], (uint32_t)(t & 1));
-      }
-      const float neg_m = -m_run;
-      float ls[4] = {0.f, 0.f, 0.f, 0.f};
-      // Software-pipelined by hand: the exp2 of chunk c are issued interleaved with the row-sum / fp16 pack /
-      // TMEM store of chunk c-1, so every consumer sits >= 32 instructions behind its MUFU.EX2 and one warp
-      // alone keeps the MUFU pipe streaming (ptxas otherwise schedules "MUFU, MUFU, FADD of those two",
-      // which stalls on the MUFU latency after every pair: profiles/r01_ext_attn_trace.md).
-#pragma unroll
-      for (int c = 0; c <= kChunks; ++c) {
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          if (c < kChunks) {
-            const float x0 = fmaf(__uint_as_float(v[c][2 * i]), sl2, neg_m);
-            const float x1 = fmaf(__uint_as_float(v[c][2 * i + 1]), sl2, neg_m);
-            v[c][2 * i] = __float_as_uint(poly_slot(2 * i, kPoly16) ? poly_exp2(x0) : fast_exp2(x0));
-            v[c][2 * i + 1] = __float_as_uint(poly_slot(2 * i + 1, kPoly16) ? poly_exp2(x1) : fast_exp2(x1));
-          }
-          if (c > 0) {
-            const float p0 = __uint_as_float(v[c - 1][2 * i]), p1 = __uint_as_float(v[c - 1][2 * i + 1]);
-            if (!kOnes) ls[i & 3] += p0 + p1;
-            pk[i] = pack_f16x2_rn(p0, p1);
-          }
-        }
-        if (c > 0) tmem_st16(s_addr + 16 * (c - 1), pk);
-        if (c == prm.handoff) {      // hand the MUFU over while the later chunks are still in flight: their tail
-          __syncwarp();              // (dependent FADD / F2FP / TMEM store latencies) overlaps the other warp's start
-          if (lane_id() == 0) mbar_arrive(&ctl->xu_turn[1 - X][quad]);
-        }
-      }
-      l_run += (ls[0] + ls[1]) + (ls[2] + ls[3]);
-      if (tracer) TF_TRACE_EV(X, t, 4);
-      tmem_wait_st();
-      if (tracer) TF_TRACE_EV(X, t, 5);
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane_id() == 0) mbar_arrive(&ctl->p_full[X][t % kNBuf]);
-      if (tracer) TF_TRACE_EV(X, t, 6);
-    }
-    // ---- final: O / L -> fp16 ----
-    mbar_wait(&ctl->pv_done[X][(T - 1) & 1], (uint32_t)(((T - 1) >> 1) & 1));
-    tc_fence_after_sync();
-    if (kOnes) {                                   // the row sum is column d of the accumulator (sum of the fp16 P)
-      uint32_t lsum;
-      tmem_ld1(o_addr + d, lsum);
-      tmem_wait_ld();
-      l_run = __uint_as_float(lsum);
-    }
-    const float inv_l = 1.0f / l_run;
-    const int p_tok = m0 + X * kBlockM + row;
-    __half* orow = out + ((long long)smp.out_sample * prm.out_rows + (p_tok - prm.q_row0)) * prm.out_tok_stride + (long long)head * d;
-    for (int c0 = 0; c0 < n_pv; c0 += 16) {
-      uint32_t o[16];
-      tmem_ld16(o_addr + c0, o);
-      tmem_wait_ld();
-      if (p_tok < prm.q_row_end) {
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          if (c0 + g * 8 < d) {
-            uint4 w;
-            w.x = pack_f16x2_rn(__uint_as_float(o[g * 8 + 0]) * inv_l, __uint_as_float(o[g * 8 + 1]) * inv_l);
-            w.y = pack_f16x2_rn(__uint_as_float(o[g * 8 + 2]) * inv_l, __uint_as_float(o[g * 8 + 3]) * inv_l);
-            w.z = pack_f16x2_rn(__uint_as_float(o[g * 8 + 4]) * inv_l, __uint_as_float(o[g * 8 + 5]) * inv_l);
-            w.w = pack_f16x2_rn(__uint_as_float(o[g * 8 + 6]) * inv_l, __uint_as_float(o[g * 8 + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(orow + c0 + g * 8) = w;
-          }
-        }
-      }
-    }
-  }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
+    // ---- O += P V ----
+#pragma unroll
+    for (int v = 0; v < kNV; ++v) reg_fence(o[v]);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kBlockN / 16; ++kk)
+#pragma unroll
+      for (int v = 0; v < kNV; ++v)
+        wgmma_rs<kNPV>(o[v], pa[kk], wgmma_desc(k_addr + (1 + v) * kTileBytes + kk * 16 * 128, kKVChunkBytes, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int v = 0; v < kNV; ++v) reg_fence(o[v]);
 
-template <int kBlockN, int kPoly16, bool kOnes>
-int launch_pp(const void* q, const void* k, const void* v, long long q_tok_stride, long long kv_tok_stride,
-              int q_samples_total, int kv_samples_total, const AttnTable& tab, int n_out, int S, int heads, int d,
-              float scale, void* out, int q_row0, int q_nrows, cudaStream_t stream) {
-  constexpr int kQBytes = 2 * kBlockM * 128, kOnesBytes = 0, kStageBytes = 2 * kBlockN * 128;
-  int stages = (227 * 1024 - 2048 - kQBytes - kOnesBytes) / kStageBytes;
-  if (stages > kPPStagesMax) stages = kPPStagesMax;
-  const size_t smem_bytes = 1024 + kQBytes + kOnesBytes + (size_t)stages * kStageBytes + sizeof(AttnCtl2);
-  CUtensorMap map_q, map_k, map_v;
-  auto make = [&](CUtensorMap* m, const void* base, long long tok_stride, int samples, int box_rows) -> int {
-    const uint64_t dims[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)S, (uint64_t)samples};
-    const uint64_t strides[3] = {(uint64_t)d * 2, (uint64_t)tok_stride * 2, (uint64_t)S * tok_stride * 2};
-    const uint32_t box[4] = {64, 1, (uint32_t)box_rows, 1};
-    CUresult r = encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, box,
-                              CU_TENSOR_MAP_SWIZZLE_128B);
-    if (r != CUDA_SUCCESS) { set_last_error("tf_ext_attn: cuTensorMapEncodeTiled failed: %d", (int)r); return TF_ERR_DRIVER; }
-    return TF_OK;
-  };
-  if (int e = make(&map_q, q, q_tok_stride, q_samples_total, kBlockM)) return e;
-  if (int e = make(&map_k, k, kv_tok_stride, kv_samples_total, kBlockN)) return e;
-  if (int e = make(&map_v, v, kv_tok_stride, kv_samples_total, kBlockN)) return e;
-  AttnParams prm;
-  prm.S = S; prm.heads = heads; prm.d = d; prm.n_out = n_out;
-  prm.q_row0 = q_row0; prm.q_row_end = (q_row0 + q_nrows < S) ? q_row0 + q_nrows : S; prm.out_rows = q_nrows;
-  prm.tiles_m = (prm.q_row_end - q_row0 + 2 * kBlockM - 1) / (2 * kBlockM);
-  static const char* env_handoff = getenv("TF_EXT_ATTN_HANDOFF");     // tuning knob (profiling)
-  prm.handoff = env_handoff ? atoi(env_handoff) : (kBlockN / 32 - 2);
-  prm.stages = stages;
-  prm.scale_log2 = scale * 1.4426950408889634f;
-  prm.out_tok_stride = (long long)heads * d;
-  auto kern = ext_attn_pp_kernel<kBlockN, kPoly16, kOnes>;
-  if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes),
-                 "tf_ext_attn smem attribute"))
-    return TF_ERR_CUDA;
-  const long long grid = (long long)n_out * heads * prm.tiles_m;
-  kern<<<(unsigned)grid, 384, smem_bytes, stream>>>(map_q, map_k, map_v, tab, prm, static_cast<__half*>(out));
-  return check_cuda(cudaGetLastError(), "tf_ext_attn launch");
-}
-
-// ================================================================================================
-// Quad-stream kernel (head dim <= 64): two 128-query tiles per CTA x two 64-key halves of every key tile
-// = four independent online-softmax streams, 16 softmax warps (four per SM sub-partition).
-//
-// Why (profiles/r02_ext_attn_variants.md): in the ping-pong kernel one warp per sub-partition runs the exp2
-// phase at a time, and ONE warp cannot issue faster than about one instruction every three cycles — the
-// exp2 phase ran at 13-15 cycles per probability against a MUFU cost of 8.1, so neither the MUFU (68 %) nor
-// the tensor pipe (26 %) was busy, and moving exp2 work to the FMA pipe only lengthened the phase.  The
-// remedy is issue parallelism, not fewer MUFU operations:
-//   * every score row is split between two threads (keys 0-63 / 64-127 of the tile) in different warps;
-//     each half is its own flash-attention stream with its own running max, row sum and accumulator
-//     (O_XL, O_XR: the P V MMA's eight 16-key steps are simply issued as 4 + 4 into two accumulators), merged
-//     once at the end — no cross-thread traffic inside the loop, four warps per sub-partition in flight;
-//   * x * scale - max is evaluated two elements at a time with FFMA2 (packed fp32, sm_100);
-//   * row sums come from the tensor core (a column of ones in V, kOnes) so no FADD per probability;
-//   * a fraction of the exp2 (kPoly16 of 16) may go to the FMA pipe once the MUFU is the limiter.
-//   warp 0: TMA   warps 1,2: MMA issue for tile A / B   warp 3: ones column   warps 4-19: softmax (X, half, quadrant)
-// TMEM (512 columns): S_A [0,128)  S_B [128,256)  O_AL O_AR O_BL O_BR [256,512) in 64-column slots.
-// fp16 P_XL overwrites S_X columns [0,32), P_XR columns [64,96) (each half only overwrites scores it has read).
-// ================================================================================================
-struct AttnCtl4 {
-  uint64_t q_full;
-  uint64_t kv_full[kPPStagesMax];
-  uint64_t kv_empty[kPPStagesMax];
-  uint64_t v_ready[kPPStagesMax];
-  uint64_t s_full[2];          // [tile X]
-  uint64_t p_full[2][2];       // [tile X][half]
-  uint64_t pv_done[2][2][2];   // [tile X][half][t & 1]
-  uint64_t fin[2];             // [tile X]: the R half published its (max, sum) for the final merge
-  uint64_t turn[2];            // [tile X]: all 8 softmax warps of tile X finished the exp2 phase of their current tile
-  float2 ml_r[2][128];         // [tile X][row]: running max and row sum of the R half
-  uint32_t tmem_base;
-};
-
-__device__ __forceinline__ void ffma2(float& y0, float& y1, float a0, float a1, float b, float c) {
-  uint64_t ra, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a0), "f"(a1));
-  asm("{\n\t.reg .b64 rb, rc;\n\tmov.b64 rb, {%2, %2};\n\tmov.b64 rc, {%3, %3};\n\t"
-      "fma.rn.f32x2 %0, %1, rb, rc;\n\t}"
-      : "=l"(rd) : "l"(ra), "f"(b), "f"(c));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(y0), "=f"(y1) : "l"(rd));
-}
-
-// kTiles = 2: two query tiles per CTA, one CTA per SM (640 threads, all 512 TMEM columns).
-// kTiles = 1: one query tile per CTA, TWO independent CTAs per SM (384 threads, 256 TMEM columns, two smem stages each):
-//             the two tiles' streams are then not coupled through a shared K/V ring and drift out of phase instead
-//             of running their exp2 phases and their score round trips in lockstep.
-template <int kPoly16, bool kOnes, int kTiles>
-__global__ void __launch_bounds__(kTiles == 2 ? 640 : 384, kTiles == 2 ? 1 : 2)
-ext_attn_q4_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-                   const __grid_constant__ CUtensorMap map_v, const AttnTable tab, const AttnParams prm,
-                   __half* __restrict__ out) {
-  constexpr int kBlockN = 128;
-  constexpr int kQTileBytes = kBlockM * 128;
-  constexpr int kQBytes = kTiles * kQTileBytes;
-  constexpr int kTileBytes = kBlockN * 128;
-  constexpr int kStageBytes = 2 * kTileBytes;
-  constexpr int kOCol = kTiles * 128;                         // accumulators start after the score buffers
-  constexpr uint32_t kTmemCols = kTiles * 256;
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* q_smem = smem;
-  uint8_t* ring = smem + kQBytes;
-  AttnCtl4* ctl = reinterpret_cast<AttnCtl4*>(ring + prm.stages * kStageBytes);
-
-  const int S = prm.S, d = prm.d, stages = prm.stages;
-  const int per_sample = prm.heads * prm.tiles_m;              // tiles_m = 256-query tile pairs
-  const int sample_slot = blockIdx.x / per_sample;
-  const int rem = blockIdx.x - sample_slot * per_sample;
-  const int head = rem / prm.tiles_m;
-  const int m0 = prm.q_row0 + (rem - head * prm.tiles_m) * (kTiles * kBlockM);
-  const AttnSample smp = tab.s[sample_slot];
-  const int tiles_per_slab = (S + kBlockN - 1) / kBlockN;
-  const int T = smp.n_kv * tiles_per_slab;
-  const int ksteps = (d + 15) / 16;
-  const int n_pv = ((d + 15) / 16) * 16;
-
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&map_q);
-    tma_prefetch_desc(&map_k);
-    tma_prefetch_desc(&map_v);
-    mbar_init(&ctl->q_full, 1);
-    for (int i = 0; i < stages; ++i) {
-      mbar_init(&ctl->kv_full[i], 1);
-      mbar_init(&ctl->kv_empty[i], kTiles);
-      mbar_init(&ctl->v_ready[i], 1);
-    }
-    for (int x = 0; x < 2; ++x) {
-      mbar_init(&ctl->s_full[x], 1);
-      mbar_init(&ctl->fin[x], 4);
-      mbar_init(&ctl->turn[x], 8);
-      for (int hh = 0; hh < 2; ++hh) {
-        mbar_init(&ctl->p_full[x][hh], 4);
-        mbar_init(&ctl->pv_done[x][hh][0], 1);
-        mbar_init(&ctl->pv_done[x][hh][1], 1);
-      }
-    }
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc(&ctl->tmem_base, kTmemCols);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, ctl->tmem_base, 0);
-
-  if (warp < 4) {
-    warpgroup_reg_dec<(kTiles == 2 ? 64 : 40)>();   // per-CTA pool: 128*40 + 256*96 <= 384*80
-    if (warp == 0) {
-      // ===================== TMA producer =====================
-      if (elect_one()) {
-        mbar_arrive_expect_tx(&ctl->q_full, (uint32_t)kQBytes);
-        tma_load_4d(q_smem, &map_q, &ctl->q_full, 0, head, m0, smp.q_sample);
-        if (kTiles == 2) tma_load_4d(q_smem + kQTileBytes, &map_q, &ctl->q_full, 0, head, m0 + kBlockM, smp.q_sample);
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int t = 0; t < T; ++t) {
-          const int slab = t / tiles_per_slab;
-          const int n0 = (t - slab * tiles_per_slab) * kBlockN;
-          mbar_wait(&ctl->kv_empty[stage], phase ^ 1);
-          uint8_t* st = ring + stage * kStageBytes;
-          mbar_arrive_expect_tx(&ctl->kv_full[stage], (uint32_t)kStageBytes);
-          tma_load_4d(st, &map_k, &ctl->kv_full[stage], 0, head, n0, smp.k_sample0 + slab);
-          tma_load_4d(st + kTileBytes, &map_v, &ctl->kv_full[stage], 0, head, n0, smp.v_sample0 + slab);
-          if (++stage == stages) { stage = 0; phase ^= 1; }
-        }
-      }
-    } else if (warp == 1 || (warp == 2 && kTiles == 2)) {
-      // ===================== MMA issuers: one warp per query tile (warp 1 -> A, warp 2 -> B) ==============
-      const int X = warp - 1;
-      const uint32_t idesc_qk = umma_idesc_f16(128, kBlockN, 0);
-      const uint32_t idesc_pv = umma_idesc_f16(128, (uint32_t)n_pv, 1);
-      constexpr uint32_t hi_kmaj = umma_desc_hi(1024);
-      const uint32_t q_lo = umma_desc_lo(smem_u32(q_smem + X * kQTileBytes), 16);
-      const uint32_t ring_k_lo = umma_desc_lo(smem_u32(ring), 16);
-      const uint32_t ring_v_lo = umma_desc_lo(smem_u32(ring + kTileBytes), kTileBytes);
-      constexpr uint32_t kStageStep = kStageBytes >> 4;
-      const uint32_t s_tmem = tmem_base + (uint32_t)(X * kBlockN);
-      const uint32_t o_l = tmem_base + kOCol + (uint32_t)(X * 2) * 64;
-      const uint32_t o_r = o_l + 64;
-      auto issue_qk = [&](int st) {
-        const uint32_t k_lo = ring_k_lo + (uint32_t)st * kStageStep;
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks)
-          if (ks < ksteps) tc_mma_ss_lh(s_tmem, q_lo + ks * 2, hi_kmaj, k_lo + ks * 2, hi_kmaj, idesc_qk, ks > 0 ? 1u : 0u);
-        tc_commit(&ctl->s_full[X]);
-      };
-      mbar_wait(&ctl->q_full, 0);
-      // tile B starts once the first half of tile A's first probabilities exists: staggers the streams
-      if (kTiles == 2 && X == 1) mbar_wait(&ctl->p_full[0][0], 0);
-      int qk_stage = 0;
-      uint32_t qk_phase = 0;
-      mbar_wait(&ctl->kv_full[0], 0);
-      tc_fence_after_sync();
-      if (elect_one()) issue_qk(0);
-      __syncwarp();
-      if (++qk_stage == stages) { qk_stage = 0; qk_phase ^= 1; }
-      int stage = 0;
-      uint32_t pv_phase = 0;
-      for (int t = 0; t < T; ++t) {
-        const bool refill = t + 1 < T;
-        const uint32_t par = (uint32_t)(t & 1);
-        if (refill) mbar_wait(&ctl->kv_full[qk_stage], qk_phase);
-        if (kOnes) mbar_wait(&ctl->v_ready[stage], pv_phase);
-        const uint32_t v_lo = ring_v_lo + (uint32_t)stage * kStageStep;
-        mbar_wait(&ctl->p_full[X][0], par);
-        tc_fence_after_sync();
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k)                 // O_XL (+)= P_X[:, keys 16k..16k+15] V[16k.., :]
-            tc_mma_ts_lh(o_l, s_tmem + k * 8, v_lo + k * 128, hi_kmaj, idesc_pv, (t > 0 || k > 0) ? 1u : 0u);
-          tc_commit(&ctl->pv_done[X][0][par]);
-        }
-        __syncwarp();
-        mbar_wait(&ctl->p_full[X][1], par);
-        tc_fence_after_sync();
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k)                 // O_XR (+)= P_X[:, keys 64+16k..] V[64+16k.., :]
-            tc_mma_ts_lh(o_r, s_tmem + 64 + k * 8, v_lo + (4 + k) * 128, hi_kmaj, idesc_pv, (t > 0 || k > 0) ? 1u : 0u);
-          tc_commit(&ctl->pv_done[X][1][par]);
-          tc_commit(&ctl->kv_empty[stage]);
-          if (refill) issue_qk(qk_stage);             // both halves of P_X are consumed in order before S_X is rewritten
-        }
-        __syncwarp();
-        if (++stage == stages) { stage = 0; pv_phase ^= 1; }
-        if (refill && ++qk_stage == stages) { qk_stage = 0; qk_phase ^= 1; }
-      }
-    } else if (warp == 3) {
-      // ===================== ones column (kOnes): V[:, d] = 1 so that O[:, d] accumulates the row sums ============
-      if constexpr (kOnes) {
-        const uint32_t col_byte = (uint32_t)d * 2u;
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int t = 0; t < T; ++t) {
-          mbar_wait(&ctl->kv_full[stage], phase);
-          uint8_t* vt = ring + stage * kStageBytes + kTileBytes;
-#pragma unroll
-          for (int r = (int)lane_id(); r < kBlockN; r += 32) {
-            const uint32_t off = (uint32_t)r * 128u + ((((col_byte >> 4) ^ ((uint32_t)r & 7u))) << 4) + (col_byte & 15u);
-            *reinterpret_cast<__half*>(vt + off) = __float2half_rn(1.0f);
-          }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          __syncwarp();
-          if (lane_id() == 0) mbar_arrive(&ctl->v_ready[stage]);
-          if (++stage == stages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    warpgroup_reg_inc<(kTiles == 2 ? 104 : 96)>();
-    // ===================== softmax streams: (tile X, key half H, lane quadrant) =====================
-    const int sid = warp - 4;
-    const int X = sid >> 3;
-    const int H = (sid >> 2) & 1;
-    const int quad = warp & 3;
-    const int row = quad * 32 + (int)lane_id();
-    const uint32_t t_lane = (uint32_t)(quad * 32) << 16;
-    const uint32_t s_addr = tmem_base + t_lane + (uint32_t)(X * kBlockN + H * 64);     // own 64 score columns; P at their start
-    const uint32_t o_addr = tmem_base + t_lane + kOCol + (uint32_t)(X * 2 + H) * 64;
-    const float sl2 = prm.scale_log2;
-    float m_run = 0.f;
-    float l_run = 0.f;
-    int slab_tile = 0;
-    for (int t = 0; t < T; ++t) {
-      const int valid = min(64, S - slab_tile * kBlockN - H * 64);          // key columns of this half inside the slab
-      if (++slab_tile == tiles_per_slab) slab_tile = 0;
-      mbar_wait(&ctl->s_full[X], (uint32_t)(t & 1));
-      tc_fence_after_sync();
-      // The tile body exists twice (generic lambda): full tiles never execute the 128 compare/select instructions of
-      // the key mask (written as a plain `if (valid < 64)` the compiler drops the outer test — the inner per-column
-      // tests imply it — and runs the selects on every tile: 128 ALU-pipe instructions per thread and tile).
-      auto tile_body = [&](auto masked_tag) {
-      constexpr bool kMasked = decltype(masked_tag)::value;
-      uint32_t v[2][32];
-      tmem_ld32(s_addr, v[0]);
-      tmem_ld32(s_addr + 32, v[1]);
-      tmem_wait_ld();
-      if constexpr (kMasked) {                     // ragged last key tile of a slab: -inf for the padding keys
-#pragma unroll
-        for (int c = 0; c < 2; ++c)
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (32 * c + i >= valid) v[c][i] = 0xFF800000u;
-      }
-      float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-      for (int c = 0; c < 2; ++c)
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          mx[0] = fmax3(mx[0], __uint_as_float(v[c][i + 0]), __uint_as_float(v[c][i + 1]));
-          mx[1] = fmax3(mx[1], __uint_as_float(v[c][i + 2]), __uint_as_float(v[c][i + 3]));
-          mx[2] = fmax3(mx[2], __uint_as_float(v[c][i + 4]), __uint_as_float(v[c][i + 5]));
-          mx[3] = fmax3(mx[3], __uint_as_float(v[c][i + 6]), __uint_as_float(v[c][i + 7]));
-        }
-      // a fully masked half tile (ragged last tile) has max = -inf: keep the running max finite
-      const float mt_s = fmaxf(fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])) * sl2, -1.0e30f);
-      if (t == 0) {
-        m_run = mt_s;
-      } else {
-        const bool need = mt_s > m_run + kRescaleThreshold;
-        if (__any_sync(0xffffffffu, need)) {
-          mbar_wait(&ctl->pv_done[X][H][(t - 1) & 1], (uint32_t)(((t - 1) >> 1) & 1));
-          tc_fence_after_sync();
-          const float m_new = fmaxf(m_run, mt_s);
-          const float alpha = fast_exp2(m_run - m_new);
-          m_run = m_new;
-          l_run *= alpha;
-          for (int c0 = 0; c0 < n_pv; c0 += 16) {
-            uint32_t o[16];
-            tmem_ld16(o_addr + c0, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(o_addr + c0, o);
-          }
-          tmem_wait_st();
-        }
-      }
-      // exp2 phases of the two query tiles take turns (prm.handoff): tile B's phase of key tile t starts when tile A's
-      // is done and tile A's phase of t+1 when tile B's of t is done, so that one tile's score round trip (P V, the
-      // next Q K^T, commit, wake-up: ~900 cycles) runs under the other tile's exp2 phase instead of both tiles
-      // computing together and then waiting together (profiles/r02_ext_attn_variants.md)
-      if (kTiles == 2 && prm.handoff) {
-        if (X == 0) { if (t > 0) mbar_wait(&ctl->turn[1], (uint32_t)((t - 1) & 1)); }
-        else mbar_wait(&ctl->turn[0], (uint32_t)(t & 1));
-      }
-      const float neg_m = -m_run;
-      float ls[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int c = 0; c <= 2; ++c) {
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          if (c < 2) {
-            float x0, x1;
-            ffma2(x0, x1, __uint_as_float(v[c][2 * i]), __uint_as_float(v[c][2 * i + 1]), sl2, neg_m);
-            v[c][2 * i] = __float_as_uint(poly_slot(2 * i, kPoly16) ? poly_exp2(x0) : fast_exp2(x0));
-            v[c][2 * i + 1] = __float_as_uint(poly_slot(2 * i + 1, kPoly16) ? poly_exp2(x1) : fast_exp2(x1));
-          }
-          if (c > 0) {
-            const float p0 = __uint_as_float(v[c - 1][2 * i]), p1 = __uint_as_float(v[c - 1][2 * i + 1]);
-            if (!kOnes) ls[i & 3] += p0 + p1;
-            pk[i] = pack_f16x2_rn(p0, p1);
-          }
-        }
-        if (c > 0) tmem_st16(s_addr + 16 * (c - 1), pk);
-      }
-      if (!kOnes) l_run += (ls[0] + ls[1]) + (ls[2] + ls[3]);
-      if (kTiles == 2 && prm.handoff) {            // exp2 instructions issued: the other tile may start its phase
-        __syncwarp();
-        if (lane_id() == 0) mbar_arrive(&ctl->turn[X]);
-      }
-      tmem_wait_st();
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane_id() == 0) mbar_arrive(&ctl->p_full[X][H]);
-      };
-      if (valid < 64) tile_body(std::true_type{}); else tile_body(std::false_type{});
-    }
-    // ---- final merge of the two key halves of a row, O / L -> fp16 ----
-    mbar_wait(&ctl->pv_done[X][H][(T - 1) & 1], (uint32_t)(((T - 1) >> 1) & 1));
-    tc_fence_after_sync();
-    if (kOnes) {
-      uint32_t lsum;
-      tmem_ld1(o_addr + d, lsum);
-      tmem_wait_ld();
-      l_run = __uint_as_float(lsum);
-    }
-    if (H == 1) {
-      ctl->ml_r[X][row] = make_float2(m_run, l_run);
-      __syncwarp();
-      if (lane_id() == 0) mbar_arrive(&ctl->fin[X]);
-    } else {
-      mbar_wait(&ctl->pv_done[X][1][(T - 1) & 1], (uint32_t)(((T - 1) >> 1) & 1));     // O_XR complete
-      mbar_wait(&ctl->fin[X], 0);
-      tc_fence_after_sync();
-      const float2 mr = ctl->ml_r[X][row];
-      const float m = fmaxf(m_run, mr.x);
-      const float a_l = fast_exp2(m_run - m), a_r = fast_exp2(mr.x - m);
-      const float inv_l = 1.0f / (a_l * l_run + a_r * mr.y);
-      const float w_l = a_l * inv_l, w_r = a_r * inv_l;
-      const int p_tok = m0 + X * kBlockM + row;
-      __half* orow = out + ((long long)smp.out_sample * prm.out_rows + (p_tok - prm.q_row0)) * prm.out_tok_stride + (long long)head * d;
-      for (int c0 = 0; c0 < n_pv; c0 += 16) {
-        uint32_t ol[16], orr[16];
-        tmem_ld16(o_addr + c0, ol);
-        tmem_ld16(o_addr + 64 + c0, orr);
-        tmem_wait_ld();
-        if (p_tok < prm.q_row_end) {
-#pragma unroll
-          for (int g = 0; g < 2; ++g) {
-            if (c0 + g * 8 < d) {
-              float f[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e)
-                f[e] = fmaf(w_l, __uint_as_float(ol[g * 8 + e]), w_r * __uint_as_float(orr[g * 8 + e]));
-              uint4 w;
-              w.x = pack_f16x2_rn(f[0], f[1]);
-              w.y = pack_f16x2_rn(f[2], f[3]);
-              w.z = pack_f16x2_rn(f[4], f[5]);
-              w.w = pack_f16x2_rn(f[6], f[7]);
-              *reinterpret_cast<uint4*>(orow + c0 + g * 8) = w;
-            }
-          }
-        }
-      }
-    }
-  }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
-}
-
-template <int kPoly16, bool kOnes, int kTiles>
-int launch_q4(const void* q, const void* k, const void* v, long long q_tok_stride, long long kv_tok_stride,
-              int q_samples_total, int kv_samples_total, const AttnTable& tab, int n_out, int S, int heads, int d,
-              float scale, void* out, int q_row0, int q_nrows, cudaStream_t stream) {
-  constexpr int kBlockN = 128;
-  constexpr int kQBytes = kTiles * kBlockM * 128, kStageBytes = 2 * kBlockN * 128;
-  int stages = (227 * 1024 - 1024 - (int)sizeof(AttnCtl4) - 64 - kQBytes) / kStageBytes;
-  if (stages > kPPStagesMax) stages = kPPStagesMax;
-  if (kTiles == 1) stages = 2;                           // two CTAs per SM: 1 KB + 16 KB Q + 2 x 32 KB ring + control each
-  const size_t smem_bytes = 1024 + kQBytes + (size_t)stages * kStageBytes + sizeof(AttnCtl4);
-  CUtensorMap map_q, map_k, map_v;
-  auto make = [&](CUtensorMap* m, const void* base, long long tok_stride, int samples, int box_rows) -> int {
-    const uint64_t dims[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)S, (uint64_t)samples};
-    const uint64_t strides[3] = {(uint64_t)d * 2, (uint64_t)tok_stride * 2, (uint64_t)S * tok_stride * 2};
-    const uint32_t box[4] = {64, 1, (uint32_t)box_rows, 1};
-    CUresult r = encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, box,
-                              CU_TENSOR_MAP_SWIZZLE_128B);
-    if (r != CUDA_SUCCESS) { set_last_error("tf_ext_attn: cuTensorMapEncodeTiled failed: %d", (int)r); return TF_ERR_DRIVER; }
-    return TF_OK;
-  };
-  if (int e = make(&map_q, q, q_tok_stride, q_samples_total, kBlockM)) return e;
-  if (int e = make(&map_k, k, kv_tok_stride, kv_samples_total, kBlockN)) return e;
-  if (int e = make(&map_v, v, kv_tok_stride, kv_samples_total, kBlockN)) return e;
-  AttnParams prm;
-  prm.S = S; prm.heads = heads; prm.d = d; prm.n_out = n_out;
-  prm.q_row0 = q_row0; prm.q_row_end = (q_row0 + q_nrows < S) ? q_row0 + q_nrows : S; prm.out_rows = q_nrows;
-  prm.tiles_m = (prm.q_row_end - q_row0 + kTiles * kBlockM - 1) / (kTiles * kBlockM);
-  static const char* env_turn = getenv("TF_EXT_ATTN_TURN");
-  prm.handoff = env_turn ? atoi(env_turn) : kDefaultTurn;
-  prm.stages = stages;
-  prm.scale_log2 = scale * 1.4426950408889634f;
-  prm.out_tok_stride = (long long)heads * d;
-  auto kern = ext_attn_q4_kernel<kPoly16, kOnes, kTiles>;
-  if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes),
-                 "tf_ext_attn smem attribute"))
-    return TF_ERR_CUDA;
-  const long long grid = (long long)n_out * heads * prm.tiles_m;
-  kern<<<(unsigned)grid, kTiles == 2 ? 640 : 384, smem_bytes, stream>>>(map_q, map_k, map_v, tab, prm, static_cast<__half*>(out));
-  return check_cuda(cudaGetLastError(), "tf_ext_attn launch");
-}
-
-// ================================================================================================
-// Quad-stream kernel, shared accumulators ("q4s", head dim <= 64) — the default.
-//
-// Same 16 softmax warps as above (two query tiles x two key halves), but:
-//   * the fp16 probabilities get their OWN tensor-memory region instead of overwriting the scores, so the
-//     next score tile S_X[t+1] = Q_X K_{t+1}^T is issued as soon as the softmax warps have pulled S_X[t] into
-//     registers (barrier s_free) — not after P_X[t] V_t.  The score round trip (P V -> Q K^T -> commit ->
-//     wake-up, ~500 cycles during which the 8 warps of a query tile sat idle in the kernel above) disappears:
-//     every softmax warp streams tile after tile and the exp2 phase of all four warps of a sub-partition overlap;
-//   * the two key halves of a row share one accumulator O_X and therefore one running max: the two threads of
-//     a row (same lane, two warps on the same SM sub-partition) exchange their half-row maxima through shared
-//     memory and a 64-thread named barrier once per tile (~40 cycles against a ~1000-cycle phase); the lazy
-//     rescale decision is then identical in both warps and each rescales alternate 16-column chunks of O_X.
-// TMEM (512 columns): S_A [0,128)  S_B [128,256)  P_A [256,320)  P_B [320,384)  O_A [384,448)  O_B [448,512).
-// ================================================================================================
-struct AttnCtl4s {
-  uint64_t q_full;
-  uint64_t kv_full[kPPStagesMax];
-  uint64_t kv_empty[kPPStagesMax];
-  uint64_t v_ready[kPPStagesMax];
-  uint64_t s_full[2];          // [tile X]  Q K^T committed
-  uint64_t s_free[2];          // [tile X]  all 8 softmax warps hold S_X[t] in registers
-  uint64_t p_full[2];          // [tile X]  all 8 softmax warps stored their part of P_X[t]
-  uint64_t pv_done[2][2];      // [tile X][t & 1]
-  float xch[2][2][2][128];     // [t & 1][tile X][half][row]: half-row maxima (and, at the end, row sums)
-  uint32_t tmem_base;
-};
-
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-template <int kPoly16, bool kOnes>
-__global__ void __launch_bounds__(640, 1)
-ext_attn_q4s_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-                    const __grid_constant__ CUtensorMap map_v, const AttnTable tab, const AttnParams prm,
-                    __half* __restrict__ out) {
-  constexpr int kBlockN = 128;
-  constexpr int kQTileBytes = kBlockM * 128;
-  constexpr int kQBytes = 2 * kQTileBytes;
-  constexpr int kTileBytes = kBlockN * 128;
-  constexpr int kStageBytes = 2 * kTileBytes;
-  constexpr int kPCol = 256, kOCol = 384;
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* q_smem = smem;
-  uint8_t* ring = smem + kQBytes;
-  AttnCtl4s* ctl = reinterpret_cast<AttnCtl4s*>(ring + prm.stages * kStageBytes);
-
-  const int S = prm.S, d = prm.d, stages = prm.stages;
-  const int per_sample = prm.heads * prm.tiles_m;
-  const int sample_slot = blockIdx.x / per_sample;
-  const int rem = blockIdx.x - sample_slot * per_sample;
-  const int head = rem / prm.tiles_m;
-  const int m0 = prm.q_row0 + (rem - head * prm.tiles_m) * (2 * kBlockM);
-  const AttnSample smp = tab.s[sample_slot];
-  const int tiles_per_slab = (S + kBlockN - 1) / kBlockN;
-  const int T = smp.n_kv * tiles_per_slab;
-  const int ksteps = (d + 15) / 16;
-  const int n_pv = ((d + 15) / 16) * 16;
-
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&map_q);
-    tma_prefetch_desc(&map_k);
-    tma_prefetch_desc(&map_v);
-    mbar_init(&ctl->q_full, 1);
-    for (int i = 0; i < stages; ++i) {
-      mbar_init(&ctl->kv_full[i], 1);
-      mbar_init(&ctl->kv_empty[i], 2);
-      mbar_init(&ctl->v_ready[i], 1);
-    }
-    for (int x = 0; x < 2; ++x) {
-      mbar_init(&ctl->s_full[x], 1);
-      mbar_init(&ctl->s_free[x], 8);
-      mbar_init(&ctl->p_full[x], 8);
-      mbar_init(&ctl->pv_done[x][0], 1);
-      mbar_init(&ctl->pv_done[x][1], 1);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc(&ctl->tmem_base, 512);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, ctl->tmem_base, 0);
-
-  if (warp < 4) {
-    warpgroup_reg_dec<64>();
-    if (warp == 0) {
-      // ===================== TMA producer =====================
-      if (elect_one()) {
-        mbar_arrive_expect_tx(&ctl->q_full, (uint32_t)kQBytes);
-        tma_load_4d(q_smem, &map_q, &ctl->q_full, 0, head, m0, smp.q_sample);
-        tma_load_4d(q_smem + kQTileBytes, &map_q, &ctl->q_full, 0, head, m0 + kBlockM, smp.q_sample);
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int t = 0; t < T; ++t) {
-          const int slab = t / tiles_per_slab;
-          const int n0 = (t - slab * tiles_per_slab) * kBlockN;
-          mbar_wait(&ctl->kv_empty[stage], phase ^ 1);
-          uint8_t* st = ring + stage * kStageBytes;
-          mbar_arrive_expect_tx(&ctl->kv_full[stage], (uint32_t)kStageBytes);
-          tma_load_4d(st, &map_k, &ctl->kv_full[stage], 0, head, n0, smp.k_sample0 + slab);
-          tma_load_4d(st + kTileBytes, &map_v, &ctl->kv_full[stage], 0, head, n0, smp.v_sample0 + slab);
-          if (++stage == stages) { stage = 0; phase ^= 1; }
-        }
-      }
-    } else if (warp == 1 || warp == 2) {
-      // ===================== MMA issuers: one warp per query tile (warp 1 -> A, warp 2 -> B) ==============
-      const int X = warp - 1;
-      const uint32_t idesc_qk = umma_idesc_f16(128, kBlockN, 0);
-      const uint32_t idesc_pv = umma_idesc_f16(128, (uint32_t)n_pv, 1);
-      constexpr uint32_t hi_kmaj = umma_desc_hi(1024);
-      const uint32_t q_lo = umma_desc_lo(smem_u32(q_smem + X * kQTileBytes), 16);
-      const uint32_t ring_k_lo = umma_desc_lo(smem_u32(ring), 16);
-      const uint32_t ring_v_lo = umma_desc_lo(smem_u32(ring + kTileBytes), kTileBytes);
-      constexpr uint32_t kStageStep = kStageBytes >> 4;
-      const uint32_t s_tmem = tmem_base + (uint32_t)(X * kBlockN);
-      const uint32_t p_tmem = tmem_base + kPCol + (uint32_t)(X * 64);
-      const uint32_t o_tmem = tmem_base + kOCol + (uint32_t)(X * 64);
-      auto issue_qk = [&](int st) {
-        const uint32_t k_lo = ring_k_lo + (uint32_t)st * kStageStep;
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks)
-          if (ks < ksteps) tc_mma_ss_lh(s_tmem, q_lo + ks * 2, hi_kmaj, k_lo + ks * 2, hi_kmaj, idesc_qk, ks > 0 ? 1u : 0u);
-        tc_commit(&ctl->s_full[X]);
-      };
-      mbar_wait(&ctl->q_full, 0);
-      if (X == 1) mbar_wait(&ctl->s_free[0], 0);     // tile B starts a little after tile A: staggers the streams
-      int qk_stage = 0;
-      uint32_t qk_phase = 0;
-      mbar_wait(&ctl->kv_full[0], 0);
-      tc_fence_after_sync();
-      if (elect_one()) issue_qk(0);
-      __syncwarp();
-      if (++qk_stage == stages) { qk_stage = 0; qk_phase ^= 1; }
-      int stage = 0;
-      uint32_t pv_phase = 0;
-      for (int t = 0; t < T; ++t) {
-        const uint32_t par = (uint32_t)(t & 1);
-        // ---- next score tile as soon as this one sits in the softmax warps' registers ----
-        if (t + 1 < T) {
-          mbar_wait(&ctl->kv_full[qk_stage], qk_phase);
-          mbar_wait(&ctl->s_free[X], par);
-          tc_fence_after_sync();
-          if (elect_one()) issue_qk(qk_stage);
-          __syncwarp();
-          if (++qk_stage == stages) { qk_stage = 0; qk_phase ^= 1; }
-        }
-        // ---- O_X (+)= P_X[t] V_t ----
-        if (kOnes) mbar_wait(&ctl->v_ready[stage], pv_phase);
-        const uint32_t v_lo = ring_v_lo + (uint32_t)stage * kStageStep;
-        mbar_wait(&ctl->p_full[X], par);
-        tc_fence_after_sync();
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < kBlockN / 16; ++k)
-            tc_mma_ts_lh(o_tmem, p_tmem + k * 8, v_lo + k * 128, hi_kmaj, idesc_pv, (t > 0 || k > 0) ? 1u : 0u);
-          tc_commit(&ctl->pv_done[X][par]);
-          tc_commit(&ctl->kv_empty[stage]);
-        }
-        __syncwarp();
-        if (++stage == stages) { stage = 0; pv_phase ^= 1; }
-      }
-    } else {
-      // ===================== ones column (kOnes): V[:, d] = 1 so that O[:, d] accumulates the row sums ============
-      if constexpr (kOnes) {
-        const uint32_t col_byte = (uint32_t)d * 2u;
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int t = 0; t < T; ++t) {
-          mbar_wait(&ctl->kv_full[stage], phase);
-          uint8_t* vt = ring + stage * kStageBytes + kTileBytes;
-#pragma unroll
-          for (int r = (int)lane_id(); r < kBlockN; r += 32) {
-            const uint32_t off = (uint32_t)r * 128u + ((((col_byte >> 4) ^ ((uint32_t)r & 7u))) << 4) + (col_byte & 15u);
-            *reinterpret_cast<__half*>(vt + off) = __float2half_rn(1.0f);
-          }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          __syncwarp();
-          if (lane_id() == 0) mbar_arrive(&ctl->v_ready[stage]);
-          if (++stage == stages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    warpgroup_reg_inc<104>();
-    // ===================== softmax streams: (tile X, key half H, lane quadrant) =====================
-    const int sid = warp - 4;
-    const int X = sid >> 3;
-    const int H = (sid >> 2) & 1;
-    const int quad = warp & 3;
-    const int row = quad * 32 + (int)lane_id();
-    const int bar_id = 1 + X * 4 + quad;                                      // the two warps that share these rows
-    const uint32_t t_lane = (uint32_t)(quad * 32) << 16;
-    const uint32_t s_addr = tmem_base + t_lane + (uint32_t)(X * kBlockN + H * 64);
-    const uint32_t p_addr = tmem_base + t_lane + kPCol + (uint32_t)(X * 64 + H * 32);
-    const uint32_t o_addr = tmem_base + t_lane + kOCol + (uint32_t)(X * 64);
-    const float sl2 = prm.scale_log2;
-    float m_run = 0.f;
-    float l_run = 0.f;
-    int slab_tile = 0;
-    for (int t = 0; t < T; ++t) {
-      const int valid = min(64, S - slab_tile * kBlockN - H * 64);
-      if (++slab_tile == tiles_per_slab) slab_tile = 0;
-      mbar_wait(&ctl->s_full[X], (uint32_t)(t & 1));
-      tc_fence_after_sync();
-      uint32_t v[2][32];
-      tmem_ld32(s_addr, v[0]);
-      tmem_ld32(s_addr + 32, v[1]);
-      tmem_wait_ld();
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane_id() == 0) mbar_arrive(&ctl->s_free[X]);                        // S_X[t] is in registers: Q K^T of t+1 may run
-      if (valid < 64) {
-#pragma unroll
-        for (int c = 0; c < 2; ++c)
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (32 * c + i >= valid) v[c][i] = 0xFF800000u;
-      }
-      float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-      for (int c = 0; c < 2; ++c)
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          mx[0] = fmax3(mx[0], __uint_as_float(v[c][i + 0]), __uint_as_float(v[c][i + 1]));
-          mx[1] = fmax3(mx[1], __uint_as_float(v[c][i + 2]), __uint_as_float(v[c][i + 3]));
-          mx[2] = fmax3(mx[2], __uint_as_float(v[c][i + 4]), __uint_as_float(v[c][i + 5]));
-          mx[3] = fmax3(mx[3], __uint_as_float(v[c][i + 6]), __uint_as_float(v[c][i + 7]));
-        }
-      const float mt_half = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-      ctl->xch[t & 1][X][H][row] = mt_half;                                    // half-row max -> the row's other thread
-      named_bar_sync(bar_id, 64);
-      const float mt = fmaxf(mt_half, ctl->xch[t & 1][X][1 - H][row]);
-      const float mt_s = fmaxf(mt * sl2, -1.0e30f);
-      if (t == 0) {
-        m_run = mt_s;
-      } else {
-        const bool need = mt_s > m_run + kRescaleThreshold;                    // identical in both warps of the row
-        mbar_wait(&ctl->pv_done[X][(t - 1) & 1], (uint32_t)(((t - 1) >> 1) & 1));   // P V of t-1 retired: O_X quiescent,
-        tc_fence_after_sync();                                                      // the P region may be rewritten
-        if (__any_sync(0xffffffffu, need)) {
-          const float m_new = fmaxf(m_run, mt_s);
-          const float alpha = fast_exp2(m_run - m_new);
-          m_run = m_new;
-          l_run *= alpha;
-          for (int c0 = 16 * H; c0 < n_pv; c0 += 32) {                         // alternate 16-column chunks per half
-            uint32_t o[16];
-            tmem_ld16(o_addr + c0, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(o_addr + c0, o);
-          }
-          tmem_wait_st();
-        }
-      }
-      const float neg_m = -m_run;
-      float ls[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int c = 0; c <= 2; ++c) {
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          if (c < 2) {
-            float x0, x1;
-            ffma2(x0, x1, __uint_as_float(v[c][2 * i]), __uint_as_float(v[c][2 * i + 1]), sl2, neg_m);
-            v[c][2 * i] = __float_as_uint(poly_slot(2 * i, kPoly16) ? poly_exp2(x0) : fast_exp2(x0));
-            v[c][2 * i + 1] = __float_as_uint(poly_slot(2 * i + 1, kPoly16) ? poly_exp2(x1) : fast_exp2(x1));
-          }
-          if (c > 0) {
-            const float p0 = __uint_as_float(v[c - 1][2 * i]), p1 = __uint_as_float(v[c - 1][2 * i + 1]);
-            if (!kOnes) ls[i & 3] += p0 + p1;
-            pk[i] = pack_f16x2_rn(p0, p1);
-          }
-        }
-        if (c > 0) tmem_st16(p_addr + 16 * (c - 1), pk);
-      }
-      if (!kOnes) l_run += (ls[0] + ls[1]) + (ls[2] + ls[3]);
-      tmem_wait_st();
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane_id() == 0) mbar_arrive(&ctl->p_full[X]);
-    }
-    // ---- final: O / L -> fp16; the two halves write alternate 16-column chunks ----
-    mbar_wait(&ctl->pv_done[X][(T - 1) & 1], (uint32_t)(((T - 1) >> 1) & 1));
-    tc_fence_after_sync();
-    float l_tot;
-    if (kOnes) {
-      uint32_t lsum;
-      tmem_ld1(o_addr + d, lsum);
-      tmem_wait_ld();
-      l_tot = __uint_as_float(lsum);
-    } else {
-      ctl->xch[T & 1][X][H][row] = l_run;
-      named_bar_sync(bar_id, 64);
-      l_tot = l_run + ctl->xch[T & 1][X][1 - H][row];
-    }
-    const float inv_l = 1.0f / l_tot;
-    const int p_tok = m0 + X * kBlockM + row;
-    __half* orow = out + ((long long)smp.out_sample * prm.out_rows + (p_tok - prm.q_row0)) * prm.out_tok_stride + (long long)head * d;
-    for (int c0 = 16 * H; c0 < n_pv; c0 += 32) {
-      uint32_t o[16];
-      tmem_ld16(o_addr + c0, o);
-      tmem_wait_ld();
-      if (p_tok < prm.q_row_end) {
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          if (c0 + g * 8 < d) {
-            uint4 w;
-            w.x = pack_f16x2_rn(__uint_as_float(o[g * 8 + 0]) * inv_l, __uint_as_float(o[g * 8 + 1]) * inv_l);
-            w.y = pack_f16x2_rn(__uint_as_float(o[g * 8 + 2]) * inv_l, __uint_as_float(o[g * 8 + 3]) * inv_l);
-            w.z = pack_f16x2_rn(__uint_as_float(o[g * 8 + 4]) * inv_l, __uint_as_float(o[g * 8 + 5]) * inv_l);
-            w.w = pack_f16x2_rn(__uint_as_float(o[g * 8 + 6]) * inv_l, __uint_as_float(o[g * 8 + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(orow + c0 + g * 8) = w;
-          }
-        }
-      }
-    }
-  }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-template <int kPoly16, bool kOnes>
-int launch_q4s(const void* q, const void* k, const void* v, long long q_tok_stride, long long kv_tok_stride,
-               int q_samples_total, int kv_samples_total, const AttnTable& tab, int n_out, int S, int heads, int d,
-               float scale, void* out, int q_row0, int q_nrows, cudaStream_t stream) {
-  constexpr int kBlockN = 128;
-  constexpr int kQBytes = 2 * kBlockM * 128, kStageBytes = 2 * kBlockN * 128;
-  int stages = (227 * 1024 - 1024 - (int)sizeof(AttnCtl4s) - 64 - kQBytes) / kStageBytes;
-  if (stages > kPPStagesMax) stages = kPPStagesMax;
-  const size_t smem_bytes = 1024 + kQBytes + (size_t)stages * kStageBytes + sizeof(AttnCtl4s);
-  CUtensorMap map_q, map_k, map_v;
-  auto make = [&](CUtensorMap* m, const void* base, long long tok_stride, int samples, int box_rows) -> int {
-    const uint64_t dims[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)S, (uint64_t)samples};
-    const uint64_t strides[3] = {(uint64_t)d * 2, (uint64_t)tok_stride * 2, (uint64_t)S * tok_stride * 2};
-    const uint32_t box[4] = {64, 1, (uint32_t)box_rows, 1};
-    CUresult r = encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, box,
-                              CU_TENSOR_MAP_SWIZZLE_128B);
-    if (r != CUDA_SUCCESS) { set_last_error("tf_ext_attn: cuTensorMapEncodeTiled failed: %d", (int)r); return TF_ERR_DRIVER; }
-    return TF_OK;
-  };
-  if (int e = make(&map_q, q, q_tok_stride, q_samples_total, kBlockM)) return e;
-  if (int e = make(&map_k, k, kv_tok_stride, kv_samples_total, kBlockN)) return e;
-  if (int e = make(&map_v, v, kv_tok_stride, kv_samples_total, kBlockN)) return e;
-  AttnParams prm;
-  prm.S = S; prm.heads = heads; prm.d = d; prm.n_out = n_out;
-  prm.q_row0 = q_row0; prm.q_row_end = (q_row0 + q_nrows < S) ? q_row0 + q_nrows : S; prm.out_rows = q_nrows;
-  prm.tiles_m = (prm.q_row_end - q_row0 + 2 * kBlockM - 1) / (2 * kBlockM);
-  prm.handoff = 0;
-  prm.stages = stages;
-  prm.scale_log2 = scale * 1.4426950408889634f;
-  prm.out_tok_stride = (long long)heads * d;
-  auto kern = ext_attn_q4s_kernel<kPoly16, kOnes>;
-  if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes),
-                 "tf_ext_attn smem attribute"))
-    return TF_ERR_CUDA;
-  const long long grid = (long long)n_out * heads * prm.tiles_m;
-  kern<<<(unsigned)grid, 640, smem_bytes, stream>>>(map_q, map_k, map_v, tab, prm, static_cast<__half*>(out));
-  return check_cuda(cudaGetLastError(), "tf_ext_attn launch");
-}
-
-// ================================================================================================
-// Quad-stream kernel for PAIRED samples ("q4d") — PnP q/k injection (reference tokenflow_utils.py:124-130).
-//
-// While t is in the injection schedule the uncond and the cond sample of a keyframe read the SAME q and the
-// SAME k (the source stream's): their score tiles and probabilities are identical, only V differs.  This
-// kernel computes S and P once per pair and multiplies P with [V_uncond | V_cond] in ONE tcgen05.mma per 16
-// keys: the two 64-column V tiles sit next to each other in shared memory, the MN-major B descriptor's
-// leading byte offset steps from one to the other, N = 64 + n_pv (112 at d = 40), and the accumulator holds
-// O_uncond in columns [0, 64) and O_cond in [64, 64 + n_pv).  Q K^T, the exp2 work, the MMA issue slots and the
-// K traffic are halved per output; the algorithmic FLOP count of the call is unchanged (SURVEY.md §8d).
-// Structure: the shared-accumulator quad-stream kernel (two query tiles x two key halves, half-row maxima
-// exchanged per tile), fp16 P over the scores, P V before the next Q K^T.  Needs the ones column (d % 16 != 0).
-// TMEM (512 columns): S_A [0,128)  S_B [128,256)  O_A [256,384)  O_B [384,512).
-// ================================================================================================
-template <int kPoly16>
-__global__ void __launch_bounds__(640, 1)
-ext_attn_q4d_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-                    const __grid_constant__ CUtensorMap map_v, const AttnPairTable tab, const AttnParams prm,
-                    __half* __restrict__ out) {
-  constexpr int kBlockN = 128;
-  constexpr int kQTileBytes = kBlockM * 128;
-  constexpr int kQBytes = 2 * kQTileBytes;
-  constexpr int kTileBytes = kBlockN * 128;
-  constexpr int kStageBytes = 3 * kTileBytes;              // K | V_uncond | V_cond
-  constexpr int kOCol = 256;
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* q_smem = smem;
-  uint8_t* ring = smem + kQBytes;
-  AttnCtl4s* ctl = reinterpret_cast<AttnCtl4s*>(ring + prm.stages * kStageBytes);
-
-  const int S = prm.S, d = prm.d, stages = prm.stages;
-  const int per_sample = prm.heads * prm.tiles_m;
-  const int pair_slot = blockIdx.x / per_sample;
-  const int rem = blockIdx.x - pair_slot * per_sample;
-  const int head = rem / prm.tiles_m;
-  const int m0 = prm.q_row0 + (rem - head * prm.tiles_m) * (2 * kBlockM);
-  const AttnPair pr = tab.p[pair_slot];
-  const int tiles_per_slab = (S + kBlockN - 1) / kBlockN;
-  const int T = pr.n_kv * tiles_per_slab;
-  const int ksteps = (d + 15) / 16;
-  const int n_pv = ((d + 15) / 16) * 16;
-  const int n_acc = 64 + n_pv;                              // accumulator columns: [O_uncond (64) | O_cond (n_pv)]
-
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&map_q);
-    tma_prefetch_desc(&map_k);
-    tma_prefetch_desc(&map_v);
-    mbar_init(&ctl->q_full, 1);
-    for (int i = 0; i < stages; ++i) {
-      mbar_init(&ctl->kv_full[i], 1);
-      mbar_init(&ctl->kv_empty[i], 2);
-      mbar_init(&ctl->v_ready[i], 1);
-    }
-    for (int x = 0; x < 2; ++x) {
-      mbar_init(&ctl->s_full[x], 1);
-      mbar_init(&ctl->p_full[x], 8);
-      mbar_init(&ctl->pv_done[x][0], 1);
-      mbar_init(&ctl->pv_done[x][1], 1);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc(&ctl->tmem_base, 512);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, ctl->tmem_base, 0);
-
-  if (warp < 4) {
-    warpgroup_reg_dec<64>();
-    if (warp == 0) {
-      // ===================== TMA producer =====================
-      if (elect_one()) {
-        mbar_arrive_expect_tx(&ctl->q_full, (uint32_t)kQBytes);
-        tma_load_4d(q_smem, &map_q, &ctl->q_full, 0, head, m0, pr.q_sample);
-        tma_load_4d(q_smem + kQTileBytes, &map_q, &ctl->q_full, 0, head, m0 + kBlockM, pr.q_sample);
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int t = 0; t < T; ++t) {
-          const int slab = t / tiles_per_slab;
-          const int n0 = (t - slab * tiles_per_slab) * kBlockN;
-          mbar_wait(&ctl->kv_empty[stage], phase ^ 1);
-          uint8_t* st = ring + stage * kStageBytes;
-          mbar_arrive_expect_tx(&ctl->kv_full[stage], (uint32_t)kStageBytes);
-          tma_load_4d(st, &map_k, &ctl->kv_full[stage], 0, head, n0, pr.k_sample0 + slab);
-          tma_load_4d(st + kTileBytes, &map_v, &ctl->kv_full[stage], 0, head, n0, pr.v_u0 + slab);
-          tma_load_4d(st + 2 * kTileBytes, &map_v, &ctl->kv_full[stage], 0, head, n0, pr.v_c0 + slab);
-          if (++stage == stages) { stage = 0; phase ^= 1; }
-        }
-      }
-    } else if (warp == 1 || warp == 2) {
-      // ===================== MMA issuers: one warp per query tile =====================
-      const int X = warp - 1;
-      const uint32_t idesc_qk = umma_idesc_f16(128, kBlockN, 0);
-      const uint32_t idesc_pv = umma_idesc_f16(128, (uint32_t)n_acc, 1);
-      constexpr uint32_t hi_kmaj = umma_desc_hi(1024);
-      const uint32_t q_lo = umma_desc_lo(smem_u32(q_smem + X * kQTileBytes), 16);
-      const uint32_t ring_k_lo = umma_desc_lo(smem_u32(ring), 16);
-      // B = [V_uncond | V_cond]: MN-major, the second 64 value columns start one tile (LBO) after the first
-      const uint32_t ring_v_lo = umma_desc_lo(smem_u32(ring + kTileBytes), kTileBytes);
-      constexpr uint32_t kStageStep = kStageBytes >> 4;
-      const uint32_t s_tmem = tmem_base + (uint32_t)(X * kBlockN);
-      const uint32_t o_tmem = tmem_base + kOCol + (uint32_t)(X * 128);
-      auto issue_qk = [&](int st) {
-        const uint32_t k_lo = ring_k_lo + (uint32_t)st * kStageStep;
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks)
-          if (ks < ksteps) tc_mma_ss_lh(s_tmem, q_lo + ks * 2, hi_kmaj, k_lo + ks * 2, hi_kmaj, idesc_qk, ks > 0 ? 1u : 0u);
-        tc_commit(&ctl->s_full[X]);
-      };
-      mbar_wait(&ctl->q_full, 0);
-      if (X == 1) mbar_wait(&ctl->p_full[0], 0);      // tile B starts once tile A's first probabilities exist
-      int qk_stage = 0;
-      uint32_t qk_phase = 0;
-      mbar_wait(&ctl->kv_full[0], 0);
-      tc_fence_after_sync();
-      if (elect_one()) issue_qk(0);
-      __syncwarp();
-      if (++qk_stage == stages) { qk_stage = 0; qk_phase ^= 1; }
-      int stage = 0;
-      uint32_t pv_phase = 0;
-      for (int t = 0; t < T; ++t) {
-        const bool refill = t + 1 < T;
-        const uint32_t par = (uint32_t)(t & 1);
-        if (refill) mbar_wait(&ctl->kv_full[qk_stage], qk_phase);
-        mbar_wait(&ctl->v_ready[stage], pv_phase);
-        const uint32_t v_lo = ring_v_lo + (uint32_t)stage * kStageStep;
-        mbar_wait(&ctl->p_full[X], par);
-        tc_fence_after_sync();
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < 8; ++k)                  // [O_u | O_c] (+)= P_X[:, 16k..16k+15] [V_u | V_c][16k.., :]
-            tc_mma_ts_lh(o_tmem, s_tmem + (k < 4 ? k * 8 : 64 + (k - 4) * 8), v_lo + k * 128, hi_kmaj, idesc_pv,
-                         (t > 0 || k > 0) ? 1u : 0u);
-          tc_commit(&ctl->pv_done[X][par]);
-          tc_commit(&ctl->kv_empty[stage]);
-          if (refill) issue_qk(qk_stage);              // in order after the P V that consumes the P it overwrites
-        }
-        __syncwarp();
-        if (++stage == stages) { stage = 0; pv_phase ^= 1; }
-        if (refill && ++qk_stage == stages) { qk_stage = 0; qk_phase ^= 1; }
-      }
-    } else {
-      // ===================== ones column: V_uncond[:, d] = 1 -> O[:, d] accumulates the (shared) row sums ===========
-      const uint32_t col_byte = (uint32_t)d * 2u;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = 0; t < T; ++t) {
-        mbar_wait(&ctl->kv_full[stage], phase);
-        uint8_t* vt = ring + stage * kStageBytes + kTileBytes;
-#pragma unroll
-        for (int r = (int)lane_id(); r < kBlockN; r += 32) {
-          const uint32_t off = (uint32_t)r * 128u + ((((col_byte >> 4) ^ ((uint32_t)r & 7u))) << 4) + (col_byte & 15u);
-          *reinterpret_cast<__half*>(vt + off) = __float2half_rn(1.0f);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane_id() == 0) mbar_arrive(&ctl->v_ready[stage]);
-        if (++stage == stages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else {
-    warpgroup_reg_inc<104>();
-    // ===================== softmax streams: (tile X, key half H, lane quadrant) =====================
-    const int sid = warp - 4;
-    const int X = sid >> 3;
-    const int H = (sid >> 2) & 1;
-    const int quad = warp & 3;
-    const int row = quad * 32 + (int)lane_id();
-    const int bar_id = 1 + X * 4 + quad;
-    const uint32_t t_lane = (uint32_t)(quad * 32) << 16;
-    const uint32_t s_addr = tmem_base + t_lane + (uint32_t)(X * kBlockN + H * 64);   // own 64 score columns; P at their start
-    const uint32_t o_addr = tmem_base + t_lane + kOCol + (uint32_t)(X * 128);
-    const float sl2 = prm.scale_log2;
-    float m_run = 0.f;
-    int slab_tile = 0;
-    for (int t = 0; t < T; ++t) {
-      const int valid = min(64, S - slab_tile * kBlockN - H * 64);
-      if (++slab_tile == tiles_per_slab) slab_tile = 0;
-      mbar_wait(&ctl->s_full[X], (uint32_t)(t & 1));
-      tc_fence_after_sync();
-      // The tile body exists twice (generic lambda): full tiles never execute the 128 compare/select instructions of
-      // the key mask (written as a plain `if (valid < 64)` the compiler drops the outer test — the inner per-column
-      // tests imply it — and runs the selects on every tile: 128 ALU-pipe instructions per thread and tile).
-      auto tile_body = [&](auto masked_tag) {
-      constexpr bool kMasked = decltype(masked_tag)::value;
-      uint32_t v[2][32];
-      tmem_ld32(s_addr, v[0]);
-      tmem_ld32(s_addr + 32, v[1]);
-      tmem_wait_ld();
-      if constexpr (kMasked) {                     // ragged last key tile of a slab: -inf for the padding keys
-#pragma unroll
-        for (int c = 0; c < 2; ++c)
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (32 * c + i >= valid) v[c][i] = 0xFF800000u;
-      }
-      float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-      for (int c = 0; c < 2; ++c)
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          mx[0] = fmax3(mx[0], __uint_as_float(v[c][i + 0]), __uint_as_float(v[c][i + 1]));
-          mx[1] = fmax3(mx[1], __uint_as_float(v[c][i + 2]), __uint_as_float(v[c][i + 3]));
-          mx[2] = fmax3(mx[2], __uint_as_float(v[c][i + 4]), __uint_as_float(v[c][i + 5]));
-          mx[3] = fmax3(mx[3], __uint_as_float(v[c][i + 6]), __uint_as_float(v[c][i + 7]));
-        }
-      const float mt_half = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-      ctl->xch[t & 1][X][H][row] = mt_half;
-      named_bar_sync(bar_id, 64);
-      const float mt = fmaxf(mt_half, ctl->xch[t & 1][X][1 - H][row]);
-      const float mt_s = fmaxf(mt * sl2, -1.0e30f);
-      if (t == 0) {
-        m_run = mt_s;
-      } else {
-        const bool need = mt_s > m_run + kRescaleThreshold;                    // identical in both warps of the row
-        if (__any_sync(0xffffffffu, need)) {
-          mbar_wait(&ctl->pv_done[X][(t - 1) & 1], (uint32_t)(((t - 1) >> 1) & 1));
-          tc_fence_after_sync();
-          const float m_new = fmaxf(m_run, mt_s);
-          const float alpha = fast_exp2(m_run - m_new);
-          m_run = m_new;
-          for (int c0 = 16 * H; c0 < n_acc; c0 += 32) {                        // alternate 16-column chunks per half
-            uint32_t o[16];
-            tmem_ld16(o_addr + c0, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(o_addr + c0, o);
-          }
-          tmem_wait_st();
-        }
-      }
-      const float neg_m = -m_run;
-#pragma unroll
-      for (int c = 0; c <= 2; ++c) {
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          if (c < 2) {
-            float x0, x1;
-            ffma2(x0, x1, __uint_as_float(v[c][2 * i]), __uint_as_float(v[c][2 * i + 1]), sl2, neg_m);
-            v[c][2 * i] = __float_as_uint(poly_slot(2 * i, kPoly16) ? poly_exp2(x0) : fast_exp2(x0));
-            v[c][2 * i + 1] = __float_as_uint(poly_slot(2 * i + 1, kPoly16) ? poly_exp2(x1) : fast_exp2(x1));
-          }
-          if (c > 0) pk[i] = pack_f16x2_rn(__uint_as_float(v[c - 1][2 * i]), __uint_as_float(v[c - 1][2 * i + 1]));
-        }
-        if (c > 0) tmem_st16(s_addr + 16 * (c - 1), pk);
-      }
-      tmem_wait_st();
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane_id() == 0) mbar_arrive(&ctl->p_full[X]);
-      };
-      if (valid < 64) tile_body(std::true_type{}); else tile_body(std::false_type{});
-    }
-    // ---- final: [O_u | O_c] / L -> fp16, the two halves write alternate 16-column chunks ----
-    mbar_wait(&ctl->pv_done[X][(T - 1) & 1], (uint32_t)(((T - 1) >> 1) & 1));
-    tc_fence_after_sync();
-    uint32_t lsum;
-    tmem_ld1(o_addr + d, lsum);
-    tmem_wait_ld();
-    const float inv_l = 1.0f / __uint_as_float(lsum);
-    const int p_tok = m0 + X * kBlockM + row;
-    for (int c0 = 16 * H; c0 < n_acc; c0 += 32) {
-      uint32_t o[16];
-      tmem_ld16(o_addr + c0, o);
-      tmem_wait_ld();
-      const int smp_out = c0 < 64 ? pr.out_u : pr.out_c;
-      const int col0 = c0 < 64 ? c0 : c0 - 64;
-      __half* orow = out + ((long long)smp_out * prm.out_rows + (p_tok - prm.q_row0)) * prm.out_tok_stride + (long long)head * d;
-      if (p_tok < prm.q_row_end) {
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          if (col0 + g * 8 < d) {
-            uint4 w;
-            w.x = pack_f16x2_rn(__uint_as_float(o[g * 8 + 0]) * inv_l, __uint_as_float(o[g * 8 + 1]) * inv_l);
-            w.y = pack_f16x2_rn(__uint_as_float(o[g * 8 + 2]) * inv_l, __uint_as_float(o[g * 8 + 3]) * inv_l);
-            w.z = pack_f16x2_rn(__uint_as_float(o[g * 8 + 4]) * inv_l, __uint_as_float(o[g * 8 + 5]) * inv_l);
-            w.w = pack_f16x2_rn(__uint_as_float(o[g * 8 + 6]) * inv_l, __uint_as_float(o[g * 8 + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(orow + col0 + g * 8) = w;
-          }
-        }
-      }
-    }
-  }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-template <int kPoly16>
-int launch_q4d(const void* q, const void* k, const void* v, long long q_tok_stride, long long kv_tok_stride,
-               int q_samples_total, int kv_samples_total, const AttnPairTable& tab, int n_pairs, int S, int heads, int d,
-               float scale, void* out, int q_row0, int q_nrows, cudaStream_t stream) {
-  constexpr int kBlockN = 128;
-  constexpr int kQBytes = 2 * kBlockM * 128, kStageBytes = 3 * kBlockN * 128;
-  int stages = (227 * 1024 - 1024 - (int)sizeof(AttnCtl4s) - 64 - kQBytes) / kStageBytes;
-  if (stages > kPPStagesMax) stages = kPPStagesMax;
-  const size_t smem_bytes = 1024 + kQBytes + (size_t)stages * kStageBytes + sizeof(AttnCtl4s);
-  CUtensorMap map_q, map_k, map_v;
-  auto make = [&](CUtensorMap* m, const void* base, long long tok_stride, int samples, int box_rows) -> int {
-    const uint64_t dims[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)S, (uint64_t)samples};
-    const uint64_t strides[3] = {(uint64_t)d * 2, (uint64_t)tok_stride * 2, (uint64_t)S * tok_stride * 2};
-    const uint32_t box[4] = {64, 1, (uint32_t)box_rows, 1};
-    CUresult r = encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, box,
-                              CU_TENSOR_MAP_SWIZZLE_128B);
-    if (r != CUDA_SUCCESS) { set_last_error("tf_ext_attn: cuTensorMapEncodeTiled failed: %d", (int)r); return TF_ERR_DRIVER; }
-    return TF_OK;
-  };
-  if (int e = make(&map_q, q, q_tok_stride, q_samples_total, kBlockM)) return e;
-  if (int e = make(&map_k, k, kv_tok_stride, kv_samples_total, kBlockN)) return e;
-  if (int e = make(&map_v, v, kv_tok_stride, kv_samples_total, kBlockN)) return e;
-  AttnParams prm;
-  prm.S = S; prm.heads = heads; prm.d = d; prm.n_out = n_pairs;
-  prm.q_row0 = q_row0; prm.q_row_end = (q_row0 + q_nrows < S) ? q_row0 + q_nrows : S; prm.out_rows = q_nrows;
-  prm.tiles_m = (prm.q_row_end - q_row0 + 2 * kBlockM - 1) / (2 * kBlockM);
-  prm.handoff = 0;
-  prm.stages = stages;
-  prm.scale_log2 = scale * 1.4426950408889634f;
-  prm.out_tok_stride = (long long)heads * d;
-  auto kern = ext_attn_q4d_kernel<kPoly16>;
-  if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes),
-                 "tf_ext_attn smem attribute"))
-    return TF_ERR_CUDA;
-  const long long grid = (long long)n_pairs * heads * prm.tiles_m;
-  kern<<<(unsigned)grid, 640, smem_bytes, stream>>>(map_q, map_k, map_v, tab, prm, static_cast<__half*>(out));
-  return check_cuda(cudaGetLastError(), "tf_ext_attn (paired) launch");
-}
-
-// ================================================================================================
-// Two-half kernel for head dims 65..128 (SD1.5 middle level: d = 80): one 128-query tile per CTA, every key tile
-// split in two 64-key halves = two softmax streams, 8 softmax warps (two per SM sub-partition).
-//
-// The one-tile kernel at the top of this file ran d = 80 with 4 softmax warps (one per sub-partition, issue-bound:
-// profiles/r02_ext_attn_variants.md) and two tensor-memory passes per tile.  Here each thread keeps its 64 scores in
-// registers (one TMEM read), x*scale - max uses FFMA2, a fraction of the exp2 runs on the FMA pipe, and the two
-// halves own separate accumulators O_L / O_R (P V issued as 4 + 4 sixteen-key steps) merged once at the end.  The
-// score buffer is double-buffered: S[t+1] = Q K_{t+1}^T is issued right after P[t-1] V, so the tensor pipe works on
-// the next scores while the softmax warps are busy with the current ones (the per-tile tensor work, 640 cycles at
-// d = 80, is close to the exp2 work of a tile — neither side waits for the other).
-//   warp 0: TMA   warp 1: MMA issuer   warps 2,3: idle   warps 4-11: softmax (half, quadrant)
-// TMEM (512 columns): S[0] [0,128)  S[1] [128,256)  O_L [256,384)  O_R [384,512); fp16 P_L over S[b] columns
-// [0,32), P_R over [64,96).
-// ================================================================================================
-struct AttnCtlH2 {
-  uint64_t q_full;
-  uint64_t kv_full[8];
-  uint64_t kv_empty[8];
-  uint64_t s_full[2];          // [score buffer]
-  uint64_t p_full[2][2];       // [score buffer][half]
-  uint64_t pv_done[2][2];      // [half][t & 1]
-  uint64_t fin;
-  float2 ml_r[128];
-  uint32_t tmem_base;
-};
-
-template <int kDChunks, int kPoly16>
-__global__ void __launch_bounds__(384, 1)
-ext_attn_h2_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-                   const __grid_constant__ CUtensorMap map_v, const AttnTable tab, const AttnParams prm,
-                   __half* __restrict__ out) {
-  constexpr int kBlockN = 128;
-  constexpr int kQChunkBytes = kBlockM * 128;
-  constexpr int kKVChunkBytes = kBlockN * 128;
-  constexpr int kQBytes = kDChunks * kQChunkBytes;
-  constexpr int kTileBytes = kDChunks * kKVChunkBytes;
-  constexpr int kStageBytes = 2 * kTileBytes;
-  constexpr int kOCol = 256;
-  static_assert(kDChunks <= 2, "two 128-column accumulators");
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* q_smem = smem;
-  uint8_t* ring = smem + kQBytes;
-  AttnCtlH2* ctl = reinterpret_cast<AttnCtlH2*>(ring + prm.stages * kStageBytes);
-
-  const int S = prm.S, d = prm.d, stages = prm.stages;
-  const int per_sample = prm.heads * prm.tiles_m;
-  const int sample_slot = blockIdx.x / per_sample;
-  const int rem = blockIdx.x - sample_slot * per_sample;
-  const int head = rem / prm.tiles_m;
-  const int m0 = prm.q_row0 + (rem - head * prm.tiles_m) * kBlockM;
-  const AttnSample smp = tab.s[sample_slot];
-  const int tiles_per_slab = (S + kBlockN - 1) / kBlockN;
-  const int T = smp.n_kv * tiles_per_slab;
-  const int ksteps = (d + 15) / 16;
-  const int n_pv = ((d + 15) / 16) * 16;
-
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&map_q);
-    tma_prefetch_desc(&map_k);
-    tma_prefetch_desc(&map_v);
-    mbar_init(&ctl->q_full, 1);
-    for (int i = 0; i < stages; ++i) {
-      mbar_init(&ctl->kv_full[i], 1);
-      mbar_init(&ctl->kv_empty[i], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&ctl->s_full[b], 1);
-      for (int hh = 0; hh < 2; ++hh) {
-        mbar_init(&ctl->p_full[b][hh], 4);
-        mbar_init(&ctl->pv_done[hh][b], 1);
-      }
-    }
-    mbar_init(&ctl->fin, 4);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc(&ctl->tmem_base, 512);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, ctl->tmem_base, 0);
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      mbar_arrive_expect_tx(&ctl->q_full, (uint32_t)kQBytes);
-#pragma unroll
-      for (int c = 0; c < kDChunks; ++c)
-        tma_load_4d(q_smem + c * kQChunkBytes, &map_q, &ctl->q_full, c * 64, head, m0, smp.q_sample);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = 0; t < T; ++t) {
-        const int slab = t / tiles_per_slab;
-        const int n0 = (t - slab * tiles_per_slab) * kBlockN;
-        mbar_wait(&ctl->kv_empty[stage], phase ^ 1);
-        uint8_t* st = ring + stage * kStageBytes;
-        mbar_arrive_expect_tx(&ctl->kv_full[stage], (uint32_t)kStageBytes);
-#pragma unroll
-        for (int c = 0; c < kDChunks; ++c) {
-          tma_load_4d(st + c * kKVChunkBytes, &map_k, &ctl->kv_full[stage], c * 64, head, n0, smp.k_sample0 + slab);
-          tma_load_4d(st + kTileBytes + c * kKVChunkBytes, &map_v, &ctl->kv_full[stage], c * 64, head, n0,
-                      smp.v_sample0 + slab);
-        }
-        if (++stage == stages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const uint32_t idesc_qk = umma_idesc_f16(128, kBlockN, 0);
-    const uint32_t idesc_pv = umma_idesc_f16(128, (uint32_t)n_pv, 1);
-    constexpr uint32_t hi_kmaj = umma_desc_hi(1024);
-    const uint32_t q_lo = umma_desc_lo(smem_u32(q_smem), 16);
-    const uint32_t ring_k_lo = umma_desc_lo(smem_u32(ring), 16);
-    const uint32_t ring_v_lo = umma_desc_lo(smem_u32(ring + kTileBytes), kKVChunkBytes);     // LBO: next 64 value columns
-    constexpr uint32_t kStageStep = kStageBytes >> 4;
-    constexpr uint32_t kQChunkStep = kQChunkBytes >> 4, kKChunkStep = kKVChunkBytes >> 4;
-    const uint32_t o_l = tmem_base + kOCol, o_r = tmem_base + kOCol + 128;
-    auto issue_qk = [&](int t, int st) {            // S[t & 1] = Q K_t^T
-      const uint32_t k_lo = ring_k_lo + (uint32_t)st * kStageStep;
-      const uint32_t s_tmem = tmem_base + (uint32_t)((t & 1) * kBlockN);
-#pragma unroll
-      for (int ks = 0; ks < 4 * kDChunks; ++ks)
-        if (ks < ksteps)
-          tc_mma_ss_lh(s_tmem, q_lo + (ks >> 2) * kQChunkStep + (ks & 3) * 2, hi_kmaj,
-                       k_lo + (ks >> 2) * kKChunkStep + (ks & 3) * 2, hi_kmaj, idesc_qk, ks > 0 ? 1u : 0u);
-      tc_commit(&ctl->s_full[t & 1]);
-    };
-    mbar_wait(&ctl->q_full, 0);
-    mbar_wait(&ctl->kv_full[0], 0);
-    tc_fence_after_sync();
-    if (elect_one()) issue_qk(0, 0);
     __syncwarp();
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int t = 0; t < T; ++t) {
-      int nstage = stage + 1;
-      uint32_t nphase = phase;
-      if (nstage == stages) { nstage = 0; nphase ^= 1; }
-      const int b = t & 1;
-      const uint32_t par = (uint32_t)((t >> 1) & 1);
-      if (t + 1 < T) {                              // next score tile first: it overlaps the softmax of this one.  In
-        mbar_wait(&ctl->kv_full[nstage], nphase);   // order after P V of t-1, which read the P this Q K^T overwrites.
-        tc_fence_after_sync();
-        if (elect_one()) issue_qk(t + 1, nstage);
-        __syncwarp();
-      }
-      const uint32_t v_lo = ring_v_lo + (uint32_t)stage * kStageStep;
-      const uint32_t p_tmem = tmem_base + (uint32_t)(b * kBlockN);
-      mbar_wait(&ctl->p_full[b][0], par);
-      tc_fence_after_sync();
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          tc_mma_ts_lh(o_l, p_tmem + k * 8, v_lo + k * 128, hi_kmaj, idesc_pv, (t > 0 || k > 0) ? 1u : 0u);
-        tc_commit(&ctl->pv_done[0][b]);
-      }
-      __syncwarp();
-      mbar_wait(&ctl->p_full[b][1], par);
-      tc_fence_after_sync();
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          tc_mma_ts_lh(o_r, p_tmem + 64 + k * 8, v_lo + (4 + k) * 128, hi_kmaj, idesc_pv, (t > 0 || k > 0) ? 1u : 0u);
-        tc_commit(&ctl->pv_done[1][b]);
-        tc_commit(&ctl->kv_empty[stage]);
-      }
-      __syncwarp();
-      stage = nstage;
-      phase = nphase;
+    if (lane == 0) mbar_arrive(&ctl->empty[st]);
+    // refill the stage of the previous tile (both warpgroups are past it by now, typically)
+    if (threadIdx.x == 0 && t >= 1 && t - 1 + stages < T) {
+      const int pt = t - 1;
+      mbar_wait(&ctl->empty[pt % stages], (uint32_t)(pt / stages) & 1u);
+      load_tile(pt + stages);
     }
-  } else if (warp >= 4) {
-    // ===================== softmax streams: (key half H, lane quadrant) =====================
-    const int H = (warp - 4) >> 2;
-    const int quad = warp & 3;
-    const int row = quad * 32 + (int)lane_id();
-    const uint32_t t_lane = (uint32_t)(quad * 32) << 16;
-    const uint32_t o_addr = tmem_base + t_lane + kOCol + (uint32_t)(H * 128);
-    const float sl2 = prm.scale_log2;
-    float m_run = 0.f;
-    float l_run = 0.f;
-    int slab_tile = 0;
-    for (int t = 0; t < T; ++t) {
-      const int b = t & 1;
-      const uint32_t par = (uint32_t)((t >> 1) & 1);
-      const int valid = min(64, S - slab_tile * kBlockN - H * 64);
-      if (++slab_tile == tiles_per_slab) slab_tile = 0;
-      const uint32_t s_addr = tmem_base + t_lane + (uint32_t)(b * kBlockN + H * 64);
-      mbar_wait(&ctl->s_full[b], par);
-      tc_fence_after_sync();
-      // The tile body exists twice (generic lambda): full tiles never execute the 128 compare/select instructions of
-      // the key mask (written as a plain `if (valid < 64)` the compiler drops the outer test — the inner per-column
-      // tests imply it — and runs the selects on every tile: 128 ALU-pipe instructions per thread and tile).
-      auto tile_body = [&](auto masked_tag) {
-      constexpr bool kMasked = decltype(masked_tag)::value;
-      uint32_t v[2][32];
-      tmem_ld32(s_addr, v[0]);
-      tmem_ld32(s_addr + 32, v[1]);
-      tmem_wait_ld();
-      if constexpr (kMasked) {                     // ragged last key tile of a slab: -inf for the padding keys
+    __syncwarp();
+  }
+
+  // ---- O / l, fp16, rows inside [q_row0, q_row_end) ----
 #pragma unroll
-        for (int c = 0; c < 2; ++c)
+  for (int r = 0; r < 2; ++r) {
+    l_r[r] += __shfl_xor_sync(0xffffffffu, l_r[r], 1);
+    l_r[r] += __shfl_xor_sync(0xffffffffu, l_r[r], 2);
+    l_r[r] = 1.f / l_r[r];
+  }
 #pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (32 * c + i >= valid) v[c][i] = 0xFF800000u;
-      }
-      float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+  for (int v = 0; v < kNV; ++v) {
+    const int out_slab = v == 0 ? it.out_u : it.out_c;
 #pragma unroll
-      for (int c = 0; c < 2; ++c)
+    for (int r = 0; r < 2; ++r) {
+      const int tok = m0 + wg * 64 + wrow + 8 * r;
+      if (tok >= prm.q_row_end) continue;
+      __half* dst = out + ((long long)out_slab * prm.out_rows + (tok - prm.q_row0)) * prm.out_tok_stride + head * d;
 #pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          mx[0] = fmax3(mx[0], __uint_as_float(v[c][i + 0]), __uint_as_float(v[c][i + 1]));
-          mx[1] = fmax3(mx[1], __uint_as_float(v[c][i + 2]), __uint_as_float(v[c][i + 3]));
-          mx[2] = fmax3(mx[2], __uint_as_float(v[c][i + 4]), __uint_as_float(v[c][i + 5]));
-          mx[3] = fmax3(mx[3], __uint_as_float(v[c][i + 6]), __uint_as_float(v[c][i + 7]));
-        }
-      const float mt_s = fmaxf(fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])) * sl2, -1.0e30f);
-      if (t == 0) {
-        m_run = mt_s;
-      } else {
-        const bool need = mt_s > m_run + kRescaleThreshold;
-        if (__any_sync(0xffffffffu, need)) {
-          mbar_wait(&ctl->pv_done[H][(t - 1) & 1], (uint32_t)(((t - 1) >> 1) & 1));
-          tc_fence_after_sync();
-          const float m_new = fmaxf(m_run, mt_s);
-          const float alpha = fast_exp2(m_run - m_new);
-          m_run = m_new;
-          l_run *= alpha;
-          for (int c0 = 0; c0 < n_pv; c0 += 16) {
-            uint32_t o[16];
-            tmem_ld16(o_addr + c0, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(o_addr + c0, o);
-          }
-          tmem_wait_st();
-        }
-      }
-      const float neg_m = -m_run;
-      float ls[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int c = 0; c <= 2; ++c) {
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          if (c < 2) {
-            float x0, x1;
-            ffma2(x0, x1, __uint_as_float(v[c][2 * i]), __uint_as_float(v[c][2 * i + 1]), sl2, neg_m);
-            v[c][2 * i] = __float_as_uint(poly_slot(2 * i, kPoly16) ? poly_exp2(x0) : fast_exp2(x0));
-            v[c][2 * i + 1] = __float_as_uint(poly_slot(2 * i + 1, kPoly16) ? poly_exp2(x1) : fast_exp2(x1));
-          }
-          if (c > 0) {
-            const float p0 = __uint_as_float(v[c - 1][2 * i]), p1 = __uint_as_float(v[c - 1][2 * i + 1]);
-            ls[i & 3] += p0 + p1;
-            pk[i] = pack_f16x2_rn(p0, p1);
-          }
-        }
-        if (c > 0) tmem_st16(s_addr + 16 * (c - 1), pk);
-      }
-      l_run += (ls[0] + ls[1]) + (ls[2] + ls[3]);
-      tmem_wait_st();
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane_id() == 0) mbar_arrive(&ctl->p_full[b][H]);
-      };
-      if (valid < 64) tile_body(std::true_type{}); else tile_body(std::false_type{});
-    }
-    // ---- final merge of the two key halves of a row ----
-    mbar_wait(&ctl->pv_done[H][(T - 1) & 1], (uint32_t)(((T - 1) >> 1) & 1));
-    tc_fence_after_sync();
-    if (H == 1) {
-      ctl->ml_r[row] = make_float2(m_run, l_run);
-      __syncwarp();
-      if (lane_id() == 0) mbar_arrive(&ctl->fin);
-    } else {
-      mbar_wait(&ctl->pv_done[1][(T - 1) & 1], (uint32_t)(((T - 1) >> 1) & 1));
-      mbar_wait(&ctl->fin, 0);
-      tc_fence_after_sync();
-      const float2 mr = ctl->ml_r[row];
-      const float m = fmaxf(m_run, mr.x);
-      const float a_l = fast_exp2(m_run - m), a_r = fast_exp2(mr.x - m);
-      const float inv_l = 1.0f / (a_l * l_run + a_r * mr.y);
-      const float w_l = a_l * inv_l, w_r = a_r * inv_l;
-      const int p_tok = m0 + row;
-      __half* orow = out + ((long long)smp.out_sample * prm.out_rows + (p_tok - prm.q_row0)) * prm.out_tok_stride + (long long)head * d;
-      for (int c0 = 0; c0 < n_pv; c0 += 16) {
-        uint32_t ol[16], orr[16];
-        tmem_ld16(o_addr + c0, ol);
-        tmem_ld16(o_addr + 128 + c0, orr);
-        tmem_wait_ld();
-        if (p_tok < prm.q_row_end) {
-#pragma unroll
-          for (int g = 0; g < 2; ++g) {
-            if (c0 + g * 8 < d) {
-              float f[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e)
-                f[e] = fmaf(w_l, __uint_as_float(ol[g * 8 + e]), w_r * __uint_as_float(orr[g * 8 + e]));
-              uint4 w;
-              w.x = pack_f16x2_rn(f[0], f[1]);
-              w.y = pack_f16x2_rn(f[2], f[3]);
-              w.z = pack_f16x2_rn(f[4], f[5]);
-              w.w = pack_f16x2_rn(f[6], f[7]);
-              *reinterpret_cast<uint4*>(orow + c0 + g * 8) = w;
-            }
-          }
-        }
+      for (int j = 0; j < kO / 4; ++j) {
+        const int c = 8 * j + qcol;
+        if (c < d)
+          *reinterpret_cast<uint32_t*>(dst + c) = pack_f16x2_rn(o[v][4 * j + 2 * r] * l_r[r], o[v][4 * j + 2 * r + 1] * l_r[r]);
       }
     }
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
-template <int kDChunks, int kPoly16>
-int launch_h2(const void* q, const void* k, const void* v, long long q_tok_stride, long long kv_tok_stride,
-              int q_samples_total, int kv_samples_total, const AttnTable& tab, int n_out, int S, int heads, int d,
-              float scale, void* out, int q_row0, int q_nrows, cudaStream_t stream) {
-  constexpr int kBlockN = 128;
-  constexpr int kQBytes = kDChunks * kBlockM * 128;
-  constexpr int kStageBytes = 2 * kDChunks * kBlockN * 128;
-  int stages = (227 * 1024 - 1024 - (int)sizeof(AttnCtlH2) - 64 - kQBytes) / kStageBytes;
-  if (stages > 8) stages = 8;
-  if (stages < 2) { set_last_error("tf_ext_attn: configuration does not fit shared memory"); return TF_ERR_UNSUPPORTED; }
-  const size_t smem_bytes = 1024 + kQBytes + (size_t)stages * kStageBytes + sizeof(AttnCtlH2);
-  CUtensorMap map_q, map_k, map_v;
-  auto make = [&](CUtensorMap* m, const void* base, long long tok_stride, int samples, int box_rows) -> int {
-    const uint64_t dims[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)S, (uint64_t)samples};
-    const uint64_t strides[3] = {(uint64_t)d * 2, (uint64_t)tok_stride * 2, (uint64_t)S * tok_stride * 2};
-    const uint32_t box[4] = {64, 1, (uint32_t)box_rows, 1};
-    CUresult r = encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, box,
-                              CU_TENSOR_MAP_SWIZZLE_128B);
-    if (r != CUDA_SUCCESS) { set_last_error("tf_ext_attn: cuTensorMapEncodeTiled failed: %d", (int)r); return TF_ERR_DRIVER; }
-    return TF_OK;
-  };
-  if (int e = make(&map_q, q, q_tok_stride, q_samples_total, kBlockM)) return e;
-  if (int e = make(&map_k, k, kv_tok_stride, kv_samples_total, kBlockN)) return e;
-  if (int e = make(&map_v, v, kv_tok_stride, kv_samples_total, kBlockN)) return e;
-  AttnParams prm;
-  prm.S = S; prm.heads = heads; prm.d = d; prm.n_out = n_out;
-  prm.q_row0 = q_row0; prm.q_row_end = (q_row0 + q_nrows < S) ? q_row0 + q_nrows : S; prm.out_rows = q_nrows;
-  prm.tiles_m = (prm.q_row_end - q_row0 + kBlockM - 1) / kBlockM;
-  prm.handoff = 0;
-  prm.stages = stages;
-  prm.scale_log2 = scale * 1.4426950408889634f;
-  prm.out_tok_stride = (long long)heads * d;
-  auto kern = ext_attn_h2_kernel<kDChunks, kPoly16>;
-  if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes),
-                 "tf_ext_attn smem attribute"))
-    return TF_ERR_CUDA;
-  const long long grid = (long long)n_out * heads * prm.tiles_m;
-  kern<<<(unsigned)grid, 384, smem_bytes, stream>>>(map_q, map_k, map_v, tab, prm, static_cast<__half*>(out));
-  return check_cuda(cudaGetLastError(), "tf_ext_attn launch");
-}
-
-template <int kDChunks, int kBlockN>
+template <int kDChunks, int kBlockN, int kNPV, class Tab>
 int launch_cfg(const void* q, const void* k, const void* v, long long q_tok_stride, long long kv_tok_stride,
-               int q_samples_total, int kv_samples_total, const AttnTable& tab, int n_out, int S, int heads, int d,
+               int q_samples_total, int kv_samples_total, const Tab& tab, int n_items, int S, int heads, int d,
                float scale, void* out, int q_row0, int q_nrows, cudaStream_t stream) {
+  constexpr int kNV = std::is_same<Tab, AttnPairTable>::value ? 2 : 1;
   constexpr int kQBytes = kDChunks * kBlockM * 128;
-  constexpr int kStageBytes = 2 * kDChunks * kBlockN * 128;
-  int stages = (227 * 1024 - 2048 - kQBytes) / kStageBytes;
-  if (stages > 8) stages = 8;
+  constexpr int kStageBytes = (1 + kNV) * kDChunks * kBlockN * 128;
+  int stages = (kSmemBudget - 2048 - kQBytes) / kStageBytes;
+  if (stages > kMaxStages) stages = kMaxStages;
   if (stages < 2) { set_last_error("tf_ext_attn: configuration does not fit shared memory"); return TF_ERR_UNSUPPORTED; }
   const size_t smem_bytes = 1024 + kQBytes + (size_t)stages * kStageBytes + sizeof(AttnCtl);
 
@@ -2267,20 +309,44 @@ int launch_cfg(const void* q, const void* k, const void* v, long long q_tok_stri
   if (int e = make(&map_v, v, kv_tok_stride, kv_samples_total, kBlockN)) return e;
 
   AttnParams prm;
-  prm.S = S; prm.heads = heads; prm.d = d; prm.n_out = n_out;
+  prm.S = S; prm.heads = heads; prm.d = d;
   prm.q_row0 = q_row0; prm.q_row_end = (q_row0 + q_nrows < S) ? q_row0 + q_nrows : S; prm.out_rows = q_nrows;
   prm.tiles_m = (prm.q_row_end - q_row0 + kBlockM - 1) / kBlockM;
   prm.stages = stages;
   prm.scale_log2 = scale * 1.4426950408889634f;
   prm.out_tok_stride = (long long)heads * d;
 
-  auto kern = ext_attn_kernel<kDChunks, kBlockN>;
+  auto kern = ext_attn_kernel<kDChunks, kBlockN, kNPV, Tab>;
   if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes),
                  "tf_ext_attn smem attribute"))
     return TF_ERR_CUDA;
-  const long long grid = (long long)n_out * heads * prm.tiles_m;
-  kern<<<(unsigned)grid, 192, smem_bytes, stream>>>(map_q, map_k, map_v, tab, prm, static_cast<__half*>(out));
+  const long long grid = (long long)n_items * heads * prm.tiles_m;
+  kern<<<(unsigned)grid, 256, smem_bytes, stream>>>(map_q, map_k, map_v, tab, prm, static_cast<__half*>(out));
   return check_cuda(cudaGetLastError(), "tf_ext_attn launch");
+}
+
+// Head dim -> kernel shape: 64-channel chunks, 128 keys per tile up to d = 128 (64 above, for shared memory),
+// P V width = d rounded up to 16.
+template <class Tab>
+int dispatch(const void* q, const void* k, const void* v, long long q_tok_stride, long long kv_tok_stride,
+             int q_samples_total, int kv_samples_total, const Tab& tab, int n_items, int S, int heads, int d,
+             float scale, void* out, int q_row0, int q_nrows, cudaStream_t stream) {
+  constexpr bool kPair = std::is_same<Tab, AttnPairTable>::value;
+#define TF_CFG(C, N, P)                                                                                          \
+  case P:                                                                                                       \
+    if constexpr (!kPair || P <= 64)                                                                            \
+      return launch_cfg<C, N, P, Tab>(q, k, v, q_tok_stride, kv_tok_stride, q_samples_total, kv_samples_total,  \
+                                      tab, n_items, S, heads, d, scale, out, q_row0, q_nrows, stream);          \
+    break
+  switch ((d + 15) / 16 * 16) {
+    TF_CFG(1, 128, 16); TF_CFG(1, 128, 32); TF_CFG(1, 128, 48); TF_CFG(1, 128, 64);
+    TF_CFG(2, 128, 80); TF_CFG(2, 128, 96); TF_CFG(2, 128, 112); TF_CFG(2, 128, 128);
+    TF_CFG(3, 64, 144); TF_CFG(3, 64, 160); TF_CFG(3, 64, 176); TF_CFG(3, 64, 192);
+    default: break;
+  }
+#undef TF_CFG
+  set_last_error("tf_ext_attn: head dim %d > 192 is not supported", d);
+  return TF_ERR_UNSUPPORTED;
 }
 
 }  // namespace
@@ -2289,135 +355,26 @@ int launch_ext_attn(const void* q, const void* k, const void* v, long long q_tok
                     int q_samples_total, int kv_samples_total, const AttnTable& tab, int n_out, int S, int heads,
                     int d, float scale, void* out, int q_row0, int q_nrows, cudaStream_t stream) {
   if (n_out == 0 || S == 0 || q_nrows <= 0 || q_row0 >= S) return TF_OK;
-  const int rows = (q_row0 + q_nrows < S ? q_row0 + q_nrows : S) - q_row0;      // query rows this launch covers
-  // A/B switches for profiling: TF_EXT_ATTN_MODE=v1 forces the one-query-tile kernel; TF_EXT_ATTN_POLY=<k> evaluates k
-  // of every 16 exp2 on the FMA pipe; TF_EXT_ATTN_ONES=0/1 row sums in registers / by the tensor core.
-  static const char* mode = getenv("TF_EXT_ATTN_MODE");
-  static const char* env_poly = getenv("TF_EXT_ATTN_POLY");
-  static const char* env_ones = getenv("TF_EXT_ATTN_ONES");
-  const bool force_v1 = mode && mode[0] == 'v';
-  if (d <= 64 && rows > 128 && !force_v1) {
-    const bool can_ones = (d % 16) != 0;            // a zero-padded column inside the P V MMA's N exists
-    const bool ones = can_ones && (env_ones ? atoi(env_ones) != 0 : kDefaultOnes);
-    static const char* env_tiles = getenv("TF_EXT_ATTN_TILES");
-    const bool one_tile = env_tiles ? atoi(env_tiles) == 1 : kDefaultOneTile;
-    const bool pp = mode && mode[0] == 'p';         // TF_EXT_ATTN_MODE=pp: the ping-pong kernel (one stream per query tile)
-    const int poly = env_poly ? atoi(env_poly) : (pp ? 0 : (ones ? kDefaultPolyOnes : kDefaultPoly));
-#define TF_PP(P, O)                                                                                              \
-    return launch_pp<128, P, O>(q, k, v, q_tok_stride, kv_tok_stride, q_samples_total, kv_samples_total, tab, n_out, \
-                                S, heads, d, scale, out, q_row0, q_nrows, stream)
-#define TF_Q4(P, O)                                                                                              \
-    do {                                                                                                         \
-      if (one_tile)                                                                                              \
-        return launch_q4<P, O, 1>(q, k, v, q_tok_stride, kv_tok_stride, q_samples_total, kv_samples_total, tab, n_out, S, \
-                                  heads, d, scale, out, q_row0, q_nrows, stream);                              \
-      return launch_q4<P, O, 2>(q, k, v, q_tok_stride, kv_tok_stride, q_samples_total, kv_samples_total, tab, n_out, S,   \
-                                heads, d, scale, out, q_row0, q_nrows, stream);                                \
-    } while (0)
-    if (pp) {
-      if (ones) { if (poly == 0) TF_PP(0, true); TF_PP(4, true); }
-      if (poly == 0) TF_PP(0, false);
-      TF_PP(4, false);
-    }
-    const bool q4s = mode && mode[0] == 'q' && mode[1] == '4' && mode[2] == 's';   // TF_EXT_ATTN_MODE=q4s: shared-accumulator variant
-    if (!q4s) {                                      // default: quad-stream kernel with split accumulators (measured fastest)
-      if (ones) {
-        switch (poly) {
-          case 0: TF_Q4(0, true);
-          case 2: TF_Q4(2, true);
-          case 4: TF_Q4(4, true);
-          default: TF_Q4(3, true);
-        }
-      }
-      switch (poly) {
-        case 0: TF_Q4(0, false);
-        case 3: TF_Q4(3, false);
-        default: TF_Q4(4, false);
-      }
-    }
-#define TF_Q4S(P, O)                                                                                             \
-    return launch_q4s<P, O>(q, k, v, q_tok_stride, kv_tok_stride, q_samples_total, kv_samples_total, tab, n_out, S, \
-                            heads, d, scale, out, q_row0, q_nrows, stream)
-    if (ones) {
-      switch (poly) {
-        case 0: TF_Q4S(0, true);
-        case 4: TF_Q4S(4, true);
-        default: TF_Q4S(2, true);
-      }
-    }
-    if (poly == 0) TF_Q4S(0, false);
-    TF_Q4S(3, false);
-#undef TF_Q4S
-#undef TF_PP
-#undef TF_Q4
-  }
-  if (d <= 64)
-    return launch_cfg<1, 128>(q, k, v, q_tok_stride, kv_tok_stride, q_samples_total, kv_samples_total, tab, n_out,
-                              S, heads, d, scale, out, q_row0, q_nrows, stream);
-  if (d <= 128 && !force_v1) {                   // SD1.5 middle level (d = 80): two-half kernel
-    static const char* env_poly_h2 = getenv("TF_EXT_ATTN_POLY_H2");
-    const int poly = env_poly_h2 ? atoi(env_poly_h2) : kDefaultPolyH2;
-#define TF_H2(P)                                                                                                 \
-    return launch_h2<2, P>(q, k, v, q_tok_stride, kv_tok_stride, q_samples_total, kv_samples_total, tab, n_out, S,  \
-                           heads, d, scale, out, q_row0, q_nrows, stream)
-    switch (poly) {
-      case 0: TF_H2(0);
-      case 2: TF_H2(2);
-      case 4: TF_H2(4);
-      default: TF_H2(3);
-    }
-#undef TF_H2
-  }
-  if (d <= 128)
-    return launch_cfg<2, 128>(q, k, v, q_tok_stride, kv_tok_stride, q_samples_total, kv_samples_total, tab, n_out,
-                              S, heads, d, scale, out, q_row0, q_nrows, stream);
-  if (d <= 192)
-    return launch_cfg<3, 64>(q, k, v, q_tok_stride, kv_tok_stride, q_samples_total, kv_samples_total, tab, n_out,
-                             S, heads, d, scale, out, q_row0, q_nrows, stream);
-  set_last_error("tf_ext_attn: head dim %d > 192 is not supported", d);
-  return TF_ERR_UNSUPPORTED;
+  return dispatch(q, k, v, q_tok_stride, kv_tok_stride, q_samples_total, kv_samples_total, tab, n_out, S, heads, d,
+                  scale, out, q_row0, q_nrows, stream);
 }
 
-// Paired samples (PnP q/k injection): S and P once per pair, P [V_u | V_c] in one MMA.  Returns TF_ERR_UNSUPPORTED for
-// shapes the paired kernel does not cover (the caller then launches the samples separately).
-bool ext_attn_pairs_supported(int rows, int d) {
-  static const char* env = getenv("TF_EXT_ATTN_DEDUP");
-  if (env && atoi(env) == 0) return false;
-  static const char* mode = getenv("TF_EXT_ATTN_MODE");
-  if (mode && (mode[0] == 'v' || mode[0] == 'p')) return false;
-  return d < 64 && (d % 16) != 0 && rows > 128;
+// The paired kernel holds two output accumulators; above d = 64 a pair would cost more registers than the
+// shared score computation saves, so such samples run singly.
+bool ext_attn_pairs_supported(int d) {
+  return d <= 64;
 }
 
 int launch_ext_attn_pairs(const void* q, const void* k, const void* v, long long q_tok_stride, long long kv_tok_stride,
                           int q_samples_total, int kv_samples_total, const AttnPairTable& tab, int n_pairs, int S,
                           int heads, int d, float scale, void* out, int q_row0, int q_nrows, cudaStream_t stream) {
   if (n_pairs == 0 || S == 0 || q_nrows <= 0 || q_row0 >= S) return TF_OK;
-  const int rows = (q_row0 + q_nrows < S ? q_row0 + q_nrows : S) - q_row0;
-  if (!ext_attn_pairs_supported(rows, d)) { set_last_error("tf_ext_attn: paired kernel does not cover S=%d d=%d", S, d); return TF_ERR_UNSUPPORTED; }
-  static const char* env_poly = getenv("TF_EXT_ATTN_POLY_PAIR");
-  const int poly = env_poly ? atoi(env_poly) : kDefaultPolyPair;
-#define TF_Q4D(P)                                                                                                \
-  return launch_q4d<P>(q, k, v, q_tok_stride, kv_tok_stride, q_samples_total, kv_samples_total, tab, n_pairs, S, heads, d, \
-                       scale, out, q_row0, q_nrows, stream)
-  switch (poly) {
-    case 0: TF_Q4D(0);
-    case 2: TF_Q4D(2);
-    case 4: TF_Q4D(4);
-    default: TF_Q4D(3);
+  if (!ext_attn_pairs_supported(d)) {
+    set_last_error("tf_ext_attn: paired kernel does not cover d=%d", d);
+    return TF_ERR_UNSUPPORTED;
   }
-#undef TF_Q4D
+  return dispatch(q, k, v, q_tok_stride, kv_tok_stride, q_samples_total, kv_samples_total, tab, n_pairs, S, heads, d,
+                  scale, out, q_row0, q_nrows, stream);
 }
-
-#ifdef TF_TRACE
-int read_attn_trace(long long* host, int n) {
-  const int total = 3 * kTraceTiles * kTraceEvents;
-  if (n > total) n = total;
-  return check_cuda(cudaMemcpyFromSymbol(host, g_attn_trace, sizeof(long long) * n), "trace read");
-}
-#endif
 
 }  // namespace tf
-
-#ifdef TF_TRACE
-extern "C" int tf_debug_read_attn_trace(long long* host, int n) { return tf::read_attn_trace(host, n); }
-#endif

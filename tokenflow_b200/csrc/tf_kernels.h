@@ -64,7 +64,7 @@ struct AttnPairTable {
 };
 
 
-bool ext_attn_pairs_supported(int rows, int d);
+bool ext_attn_pairs_supported(int d);
 int launch_ext_attn_pairs(const void* q, const void* k, const void* v, long long q_tok_stride, long long kv_tok_stride,
                           int q_samples_total, int kv_samples_total, const AttnPairTable& tab, int n_pairs, int S,
                           int heads, int d, float scale, void* out, int q_row0, int q_nrows, cudaStream_t stream);

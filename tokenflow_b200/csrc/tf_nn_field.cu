@@ -6,30 +6,33 @@
 // GPU path (fp32 normalise -> fp16 operands -> fp32-accumulated GEMM -> *fp16 output* -> argmax),
 // but the [B*S, 2S] similarity matrix (512 MB fp16 per block per batch at the 40-frame SD1.5
 // config, written once and re-read twice by the reference) never exists: it lives 128xN tiles at
-// a time in tensor memory and is consumed by a running (max, first-argmax) epilogue.
+// a time in registers and is consumed by a running (max, first-argmax) epilogue.
 //
-// Kernel shape (one persistent CTA per SM, static round-robin over work items; default kHalves = 1,
-// kBlockN = 256 — see launch_nn_field for the measured choice):
-//   work item   = (frame f, tile of kHalves*128 tokens, keyframe kf)           -> 128*kHalves indices
-//   warp 0      = TMA producer: the item's A tile (tokens x dim, resident for the whole N sweep when
-//                 it fits) and a kStages-deep ring of B tiles (kBlockN keyframe tokens x 64 channels)
-//   warp 1      = tcgen05.mma issuer: D[128 x kBlockN] (+)= A[128 x 16] . B[kBlockN x 16]^T, fp32
-//                 accumulators double-buffered in TMEM (2 x kHalves x kBlockN = 512 columns)
-//   warps 2..   = epilogue, one thread per token row: tcgen05.ld 32 columns -> cvt.rn.f16x2 ->
-//                 packed-half max tree -> (rarely) first-index scan -> running best
-// Operands are K-major with the 128-byte swizzle (TMA writes it, the UMMA descriptor reads it).
+// Kernel shape (one CTA per work item; kBlockN = 128):
+//   work item   = (frame f, tile of 128 tokens, keyframe kf)                     -> 128 indices
+//   warp 8      = TMA producer: the item's A tile (tokens x dim, resident for the whole N sweep
+//                 when it fits in shared memory, else streamed with B) and a ring of B tiles
+//                 (kBlockN keyframe tokens x 64 channels)
+//   warpgroups  = 2, 64 token rows each: wgmma D[64 x kBlockN] (+)= A[64 x 16] . B[kBlockN x 16]^T
+//                 with fp32 accumulators in registers, one 64-channel chunk in flight while the next
+//                 is issued; after each N tile the epilogue rounds to fp16 and keeps a running
+//                 (max, first index) per row and thread, merged across the 4 threads of a row at the end
+// Operands are K-major with the 128-byte swizzle (TMA writes it, the wgmma descriptor reads it).
 //
 // Roofline: tensor-bound, 2*rows*S*dim flops per (frame, keyframe) pair; HBM traffic is only the
 // operands (a few MB, L2 resident) and the int32 indices.
-#include <cstdlib>
+#include <cmath>
 
 #include "tf_common.cuh"
 #include "tf_kernels.h"
+#include "tf_wgmma.cuh"
 
 namespace tf {
 namespace {
 
 constexpr int kChunkK = 64;                 // channels per smem tile row: 64 x fp16 = one 128 B swizzle row
+constexpr int kBlockM = 128;
+constexpr int kBlockN = 128;
 constexpr int kMaxStages = 8;
 constexpr int kSmemBudget = 227 * 1024;
 
@@ -45,222 +48,152 @@ struct SmemCtl {
   uint64_t full[kMaxStages];
   uint64_t empty[kMaxStages];
   uint64_t a_full;
-  uint64_t a_empty;
-  uint64_t tmem_full[2];
-  uint64_t tmem_empty[2];
-  uint32_t tmem_base;
 };
 
-template <int kHalves, int kBlockN, bool kResidentA>
-__global__ void __launch_bounds__(64 + 128 * kHalves, 1)
+template <bool kResidentA>
+__global__ void __launch_bounds__(288, 1)
 nn_field_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_p,
                 const FrameTable tab, const NNItems items, int S, int dim, int stages,
                 int32_t* __restrict__ idx_a, int32_t* __restrict__ idx_b) {
-  constexpr int kBlockM = 128 * kHalves;
   constexpr int kAChunkBytes = kBlockM * 128;         // one 64-channel chunk of the A tile
   constexpr int kBChunkBytes = kBlockN * 128;
   constexpr int kStageBytes = kBChunkBytes + (kResidentA ? 0 : kAChunkBytes);
-  constexpr int kAccCols = kHalves * kBlockN;          // TMEM columns per accumulator buffer
-  constexpr int kEpiWarps = 4 * kHalves;
-  constexpr uint32_t kIdesc = umma_idesc_f16(128, kBlockN, 0);
-  static_assert(2 * kAccCols <= 512, "accumulators exceed tensor memory");
+  constexpr int kAcc = kBlockN / 2;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int nkc = (dim + kChunkK - 1) / kChunkK;
   uint8_t* a_res = smem;                                               // resident A: nkc chunks
-  uint8_t* ring = smem + (kResidentA ? nkc * kAChunkBytes : 0);        // stages x (A chunk?) + B chunk
+  uint8_t* ring = smem + (kResidentA ? nkc * kAChunkBytes : 0);        // stages x (B chunk + A chunk?)
   SmemCtl* ctl = reinterpret_cast<SmemCtl*>(ring + stages * kStageBytes);
 
-  const int warp = threadIdx.x >> 5;
+  // work item -> (frame, first token of the tile, keyframe, output array)
+  int f, m0, kf;
+  int32_t* out;
+  if ((int)blockIdx.x < items.n_a) {
+    f = blockIdx.x / items.tiles_per_frame;
+    m0 = (blockIdx.x - f * items.tiles_per_frame) * kBlockM;
+    kf = tab.kf_a[f];
+    out = idx_a;
+  } else {
+    const int j = blockIdx.x - items.n_a;
+    const int fi = j / items.tiles_per_frame;
+    f = items.b_frames[fi];
+    m0 = (j - fi * items.tiles_per_frame) * kBlockM;
+    kf = tab.kf_b[f];
+    out = idx_b;
+  }
   const int n_tiles = (S + kBlockN - 1) / kBlockN;
-  const int n_items = items.n_a + items.n_b;
+  const int J = n_tiles * nkc;                          // loads: (N tile, channel chunk), chunk fastest
 
-  if (warp == 0 && elect_one()) {
+  auto load = [&](int j) {
+    const int st = j % stages;
+    const int nt = j / nkc, kc = j - nt * nkc;
+    uint8_t* dst = ring + st * kStageBytes;
+    mbar_arrive_expect_tx(&ctl->full[st], (uint32_t)kStageBytes);
+    tma_load_3d(dst, &map_p, &ctl->full[st], kc * kChunkK, nt * kBlockN, kf);
+    if (!kResidentA) tma_load_3d(dst + kBChunkBytes, &map_x, &ctl->full[st], kc * kChunkK, m0, f);
+  };
+
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_x);
     tma_prefetch_desc(&map_p);
     for (int i = 0; i < stages; ++i) {
       mbar_init(&ctl->full[i], 1);
-      mbar_init(&ctl->empty[i], 1);
+      mbar_init(&ctl->empty[i], 8);                     // one arrival per warp
     }
     mbar_init(&ctl->a_full, 1);
-    mbar_init(&ctl->a_empty, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&ctl->tmem_full[i], 1);
-      mbar_init(&ctl->tmem_empty[i], kEpiWarps);
-    }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(&ctl->tmem_base, 512);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = ctl->tmem_base;
-
-  // decode a work item -> (frame, first token of the tile, keyframe, output array)
-  auto decode = [&](int item, int& f, int& m0, int& kf, int32_t*& out) {
-    if (item < items.n_a) {
-      f = item / items.tiles_per_frame;
-      m0 = (item - f * items.tiles_per_frame) * kBlockM;
-      kf = tab.kf_a[f];
-      out = idx_a;
-    } else {
-      const int j = item - items.n_a;
-      const int fi = j / items.tiles_per_frame;
-      f = items.b_frames[fi];
-      m0 = (j - fi * items.tiles_per_frame) * kBlockM;
-      kf = tab.kf_b[f];
-      out = idx_b;
+  if (threadIdx.x >= 256) {
+    // ===================== TMA producer warp =====================
+    if (threadIdx.x == 256) {
+      if (kResidentA) {
+        mbar_arrive_expect_tx(&ctl->a_full, (uint32_t)(nkc * kAChunkBytes));
+        for (int kc = 0; kc < nkc; ++kc) tma_load_3d(a_res + kc * kAChunkBytes, &map_x, &ctl->a_full, kc * kChunkK, m0, f);
+      }
+      for (int j = 0; j < J; ++j) {
+        if (j >= stages) mbar_wait(&ctl->empty[j % stages], (uint32_t)(j / stages - 1) & 1u);
+        load(j);
+      }
     }
+    return;
+  }
+
+  const int wg = threadIdx.x >> 7;
+  const int lane = threadIdx.x & 31;
+  const int qcol = 2 * (lane & 3);
+  const uint32_t ring_addr = smem_u32(ring);
+  const uint32_t a_res_addr = smem_u32(a_res) + wg * 64 * 128;
+  if (kResidentA) {
+    mbar_wait(&ctl->a_full, 0);
+    __syncwarp();
+  }
+
+  // the stage of load j may be refilled (every consumer warp arrives once)
+  auto release = [&](int j) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&ctl->empty[j % stages]);
   };
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t it = 0;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++it) {
-        int f, m0, kf;
-        int32_t* out;
-        decode(item, f, m0, kf, out);
-        if (kResidentA) {
-          mbar_wait(&ctl->a_empty, (it & 1) ^ 1);
-          mbar_arrive_expect_tx(&ctl->a_full, (uint32_t)(nkc * kAChunkBytes));
-          for (int kc = 0; kc < nkc; ++kc)
-            tma_load_3d(a_res + kc * kAChunkBytes, &map_x, &ctl->a_full, kc * kChunkK, m0, f);
-        }
-        for (int nt = 0; nt < n_tiles; ++nt) {
-          for (int kc = 0; kc < nkc; ++kc) {
-            mbar_wait(&ctl->empty[stage], phase ^ 1);
-            uint8_t* st = ring + stage * kStageBytes;
-            mbar_arrive_expect_tx(&ctl->full[stage], (uint32_t)kStageBytes);
-            if (!kResidentA) tma_load_3d(st + kBChunkBytes, &map_x, &ctl->full[stage], kc * kChunkK, m0, f);
-            tma_load_3d(st, &map_p, &ctl->full[stage], kc * kChunkK, nt * kBlockN, kf);
-            if (++stage == stages) { stage = 0; phase ^= 1; }
-          }
-        }
+  float best[2] = {-INFINITY, -INFINITY};
+  int best_idx[2] = {0, 0};
+  int j = 0;
+  for (int nt = 0; nt < n_tiles; ++nt) {
+    float acc[kAcc];
+    for (int kc = 0; kc < nkc; ++kc, ++j) {
+      const int st = j % stages;
+      mbar_wait(&ctl->full[st], (uint32_t)(j / stages) & 1u);
+      __syncwarp();
+      const uint32_t b_addr = ring_addr + st * kStageBytes;
+      const uint32_t a_addr = kResidentA ? a_res_addr + kc * kAChunkBytes : b_addr + kBChunkBytes + wg * 64 * 128;
+      wgmma_fence();
+#pragma unroll
+      for (int k4 = 0; k4 < kChunkK / 16; ++k4)
+        wgmma_ss<kBlockN>(acc, wgmma_desc(a_addr + k4 * 32, 16, 1024), wgmma_desc(b_addr + k4 * 32, 16, 1024),
+                          (kc > 0 || k4 > 0) ? 1u : 0u);
+      wgmma_commit();
+      if (kc > 0) {                                    // the previous chunk's MMAs are done: its stage is free
+        wgmma_wait<1>();
+        release(j - 1);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: one thread, descriptors advanced by 32-bit adds =====================
-    if (lane_id() == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t it = 0;
-      uint32_t tile_ctr = 0;                       // accumulator tiles issued so far (buffer = ctr & 1)
-      constexpr uint32_t hi = umma_desc_hi(1024);
-      const uint32_t ring_lo = umma_desc_lo(smem_u32(ring), 16);
-      const uint32_t a_res_lo = umma_desc_lo(smem_u32(a_res), 16);
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++it) {
-        if (kResidentA) {
-          mbar_wait(&ctl->a_full, it & 1);
-          tc_fence_after_sync();
-        }
-        for (int nt = 0; nt < n_tiles; ++nt, ++tile_ctr) {
-          const uint32_t acc = tile_ctr & 1;
-          mbar_wait(&ctl->tmem_empty[acc], ((tile_ctr >> 1) & 1) ^ 1);
-          tc_fence_after_sync();
-          const uint32_t d_tmem = tmem_base + acc * kAccCols;
-          for (int kc = 0; kc < nkc; ++kc) {
-            mbar_wait(&ctl->full[stage], phase);
-            tc_fence_after_sync();
-            const uint32_t b_lo = ring_lo + (uint32_t)stage * (kStageBytes >> 4);
-            const uint32_t a_lo = kResidentA ? a_res_lo + (uint32_t)kc * (kAChunkBytes >> 4) : b_lo + (kBChunkBytes >> 4);
+    wgmma_wait<0>();
+    reg_fence(acc);
+    release(j - 1);
+
+    // epilogue: fp16-rounded similarities, strictly greater keeps the earlier index
+    const int n0 = nt * kBlockN;
 #pragma unroll
-            for (int h = 0; h < kHalves; ++h) {
+    for (int jb = 0; jb < kBlockN / 8; ++jb) {
 #pragma unroll
-              for (int k4 = 0; k4 < kChunkK / 16; ++k4)
-                tc_mma_ss_lh(d_tmem + h * kBlockN, a_lo + h * ((128 * 128) >> 4) + k4 * 2, hi, b_lo + k4 * 2, hi, kIdesc,
-                             (kc > 0 || k4 > 0) ? 1u : 0u);
-            }
-            tc_commit(&ctl->empty[stage]);                 // smem stage reusable once these MMAs retire
-            if (kc == nkc - 1) tc_commit(&ctl->tmem_full[acc]);
-            if (++stage == stages) { stage = 0; phase ^= 1; }
-          }
-        }
-        if (kResidentA) tc_commit(&ctl->a_empty);           // A tile free once the item's MMAs retire
+      for (int e = 0; e < 4; ++e) {
+        const int r = e >> 1;
+        const int c = n0 + 8 * jb + qcol + (e & 1);
+        const float h = __half2float(__float2half_rn(acc[4 * jb + e]));
+        if (c < S && h > best[r]) { best[r] = h; best_idx[r] = c; }
       }
-    }
-  } else {
-    // ===================== epilogue: running first-argmax over fp16-rounded similarities ==========
-    const int ew = warp - 2;
-    const int quad = warp & 3;                    // TMEM lane quadrant this warp may access
-    const int half = ew >> 2;
-    const int row_in_tile = half * 128 + quad * 32 + (int)lane_id();
-    const uint32_t t_lane = (uint32_t)(quad * 32) << 16;
-    uint32_t tile_ctr = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      int f, m0, kf;
-      int32_t* out;
-      decode(item, f, m0, kf, out);
-      __half best = __ushort_as_half((unsigned short)0xFC00);     // -inf
-      int best_idx = 0;
-      for (int nt = 0; nt < n_tiles; ++nt, ++tile_ctr) {
-        const uint32_t acc = tile_ctr & 1;
-        mbar_wait(&ctl->tmem_full[acc], (tile_ctr >> 1) & 1);
-        tc_fence_after_sync();
-        const uint32_t t_addr = tmem_base + t_lane + acc * kAccCols + half * kBlockN;
-        const int n0 = nt * kBlockN;
-#pragma unroll 1
-        for (int c0 = 0; c0 < kBlockN; c0 += 32) {
-          if (n0 + c0 >= S) break;                                   // whole chunk beyond the keyframe
-          uint32_t v[32];
-          tmem_ld32(t_addr + c0, v);
-          tmem_wait_ld();
-          uint32_t h2[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) h2[i] = pack_f16x2_rn(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1]));
-          const int valid = S - (n0 + c0);                           // columns of this chunk inside the keyframe
-          if (valid < 32) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              if (2 * i >= valid) h2[i] = (h2[i] & 0xFFFF0000u) | 0xFC00u;
-              if (2 * i + 1 >= valid) h2[i] = (h2[i] & 0x0000FFFFu) | 0xFC000000u;
-            }
-          }
-          __half2 m8[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            m8[i] = __hmax2(*reinterpret_cast<__half2*>(&h2[2 * i]), *reinterpret_cast<__half2*>(&h2[2 * i + 1]));
-#pragma unroll
-          for (int i = 0; i < 4; ++i) m8[i] = __hmax2(m8[i], m8[i + 4]);
-          m8[0] = __hmax2(__hmax2(m8[0], m8[1]), __hmax2(m8[2], m8[3]));
-          const __half cm = __hmax(__low2half(m8[0]), __high2half(m8[0]));
-          if (__hgt(cm, best)) {                                     // strictly greater: earlier index keeps ties
-            const float cmf = __half2float(cm);
-            uint32_t eq = 0;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float2 p = __half22float2(*reinterpret_cast<__half2*>(&h2[i]));
-              eq |= (p.x == cmf ? 1u : 0u) << (2 * i);
-              eq |= (p.y == cmf ? 1u : 0u) << (2 * i + 1);
-            }
-            best = cm;
-            best_idx = n0 + c0 + (__ffs(eq) - 1);
-          }
-        }
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane_id() == 0) mbar_arrive(&ctl->tmem_empty[acc]);
-      }
-      const int p = m0 + row_in_tile;
-      if (p < S) out[(long long)f * S + p] = best_idx;
     }
   }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
+  // merge the four threads of each row: larger value wins, equal values keep the smaller index
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+#pragma unroll
+    for (int off = 1; off <= 2; off <<= 1) {
+      const float ob = __shfl_xor_sync(0xffffffffu, best[r], off);
+      const int oi = __shfl_xor_sync(0xffffffffu, best_idx[r], off);
+      if (ob > best[r] || (ob == best[r] && oi < best_idx[r])) { best[r] = ob; best_idx[r] = oi; }
+    }
+    const int p = m0 + wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2) + 8 * r;
+    if ((lane & 3) == 0 && p < S) out[(long long)f * S + p] = best_idx[r];
   }
 }
 
-template <int kHalves, int kBlockN, bool kResidentA>
+template <bool kResidentA>
 int launch_cfg(const void* x_unit, const void* piv_unit, const FrameTable& tab, const NNItems& items, int F, int S,
                int dim, int K, int32_t* idx_a, int32_t* idx_b, cudaStream_t stream) {
-  constexpr int kBlockM = 128 * kHalves;
   const int nkc = (dim + kChunkK - 1) / kChunkK;
   const int a_bytes = kResidentA ? nkc * kBlockM * 128 : 0;
   const int stage_bytes = kBlockN * 128 + (kResidentA ? 0 : kBlockM * 128);
@@ -289,38 +222,22 @@ int launch_cfg(const void* x_unit, const void* piv_unit, const FrameTable& tab, 
                               CU_TENSOR_MAP_SWIZZLE_128B);
     if (r != CUDA_SUCCESS) { set_last_error("tf_nn_field: cuTensorMapEncodeTiled(pivots) failed: %d", (int)r); return TF_ERR_DRIVER; }
   }
-  auto kern = nn_field_kernel<kHalves, kBlockN, kResidentA>;
+  auto kern = nn_field_kernel<kResidentA>;
   if (check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes),
                  "tf_nn_field smem attribute"))
     return TF_ERR_CUDA;
   const int n_items = items.n_a + items.n_b;
-  int grid = sm_count();
-  if (grid > n_items) grid = n_items;
-  kern<<<grid, 64 + 128 * kHalves, smem_bytes, stream>>>(map_x, map_p, tab, items, S, dim, stages, idx_a, idx_b);
+  kern<<<n_items, 288, smem_bytes, stream>>>(map_x, map_p, tab, items, S, dim, stages, idx_a, idx_b);
   return check_cuda(cudaGetLastError(), "tf_nn_field launch");
 }
 
 }  // namespace
 
-int g_nn_field_force_cfg = -1;   // test hook: 0 = <2,128,resident>, 1 = <1,256,resident>, 2 = <1,256,streamed>
-
 int launch_nn_field(const void* x_unit, const void* piv_unit, const FrameTable& tab, int F, int S, int dim, int K,
                     int32_t* idx_a, int32_t* idx_b, cudaStream_t stream) {
   if (F == 0 || S == 0) return TF_OK;
-  int cfg = g_nn_field_force_cfg;
-  static const char* env_cfg = getenv("TF_NN_FIELD_CFG");           // A/B switch for profiling
-  if (cfg < 0 && env_cfg) {
-    cfg = env_cfg[0] - '0';
-    if (cfg == 0 && dim > 320) cfg = 1;          // a forced configuration only applies where it fits
-    if (cfg == 1 && dim > 640) cfg = 2;
-  }
-  // Default: 128-token tiles with N = 256 MMAs.  Measured at the C2 top level (profiles/r01_kbench.json):
-  // <1,256> 1157 TFLOP/s vs <2,128> 959 — a tcgen05.mma costs ~90-100 cycles to issue whatever its shape,
-  // so the 64-cycle N = 128 MMAs of the 256-token configuration leave the tensor pipe a third idle.
-  if (cfg < 0) cfg = dim <= 640 ? 1 : 2;
-  const int block_m = (cfg == 0) ? 256 : 128;
   NNItems items;
-  items.tiles_per_frame = (S + block_m - 1) / block_m;
+  items.tiles_per_frame = (S + kBlockM - 1) / kBlockM;
   items.n_a = F * items.tiles_per_frame;
   items.n_b_frames = 0;
   for (int f = 0; f < F; ++f)
@@ -330,11 +247,10 @@ int launch_nn_field(const void* x_unit, const void* piv_unit, const FrameTable& 
     set_last_error("tf_nn_field: idx_b is NULL but some frame has a second keyframe");
     return TF_ERR_INVALID_ARGUMENT;
   }
-  switch (cfg) {
-    case 0: return launch_cfg<2, 128, true>(x_unit, piv_unit, tab, items, F, S, dim, K, idx_a, idx_b, stream);
-    case 1: return launch_cfg<1, 256, true>(x_unit, piv_unit, tab, items, F, S, dim, K, idx_a, idx_b, stream);
-    default: return launch_cfg<1, 256, false>(x_unit, piv_unit, tab, items, F, S, dim, K, idx_a, idx_b, stream);
-  }
+  // The token tile stays in shared memory for the whole keyframe sweep while at least four B stages fit
+  // beside it (dim <= 640: every SD level but the 1280-channel one); above that A streams with B.
+  if (dim <= 640) return launch_cfg<true>(x_unit, piv_unit, tab, items, F, S, dim, K, idx_a, idx_b, stream);
+  return launch_cfg<false>(x_unit, piv_unit, tab, items, F, S, dim, K, idx_a, idx_b, stream);
 }
 
 }  // namespace tf

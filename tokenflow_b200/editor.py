@@ -373,9 +373,9 @@ class TokenFlowEditor(nn.Module):
         return out
 
     def _step_compute(self, *a):
-        # Off unless asked for: on one GPU the concurrent chains slow each other down (3.32 vs 3.50 frames/s at C2), and
-        # with real NCCL ranks the 8-GPU run of this schedule did not finish (profiles/README.md) — only its
-        # single-process forms are verified (tests/test_gpu_round2.py).
+        # Off unless asked for: on one GPU the concurrent chains slow each other down, and with real NCCL ranks this
+        # schedule has not been run to completion — only its single-process forms are verified
+        # (tests/test_gpu_round2.py).
         dual = bool(self.config.get("dual_stream", False))
         if dual and self.device.type == "cuda":
             return self._dual_compute(*a)

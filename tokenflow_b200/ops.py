@@ -1,7 +1,7 @@
 """ctypes binding of libtokenflow_b200.so (include/tokenflow_b200.h) and the op layer the hooks call.
 
 `CudaOps` is the product and the only op implementation in this package: every method enqueues a
-hand-written sm_100a kernel on the current CUDA stream through the C ABI.  There is no CPU or
+hand-written sm_90a kernel on the current CUDA stream through the C ABI.  There is no CPU or
 PyTorch fallback — constructing `CudaOps` without the built library or without a CUDA device
 raises, loudly.  (Tests substitute an oracle-backed op object through
 `tokenflow_utils._install_ops_for_testing`; that object lives under `oracle/`, not here.)
@@ -125,18 +125,18 @@ def _f32(vals: Sequence[float]):
 
 
 class CudaOps:
-    """The hot-path operators, each one C-ABI call = one sm_100a kernel launch on the current stream."""
+    """The hot-path operators, each one C-ABI call = one sm_90a kernel launch on the current stream."""
 
-    name = "cuda-sm100a"
+    name = "cuda-sm90a"
 
     def __init__(self):
         self.lib = load_library()
         if not torch.cuda.is_available():
             raise TokenflowB200Error(
-                "tokenflow_b200 needs a CUDA device (sm_100a / B200); there is no CPU path.")
+                "tokenflow_b200 needs a CUDA device (sm_90a / H100); there is no CPU path.")
         major, minor = torch.cuda.get_device_capability()
-        if major != 10:
-            raise TokenflowB200Error(f"tokenflow_b200 kernels are compiled for sm_100a only (got sm_{major}{minor})")
+        if (major, minor) != (9, 0):
+            raise TokenflowB200Error(f"tokenflow_b200 kernels are compiled for sm_90a only (got sm_{major}{minor})")
 
     # -- helpers ---------------------------------------------------------------------------
     def _check(self, status: int, what: str):

@@ -3,14 +3,14 @@
 Same public names, signatures and module-state contract as omerbt/TokenFlow's tokenflow_utils.py
 (consumed by `from tokenflow_utils import *` in run_tokenflow_pnp.py:16 / run_tokenflow_sdedit.py:15),
 so the reference drivers run unchanged — but the three hot operations underneath are hand-written
-sm_100a CUDA kernels reached through the C ABI in include/tokenflow_b200.h:
+sm_90a CUDA kernels reached through the C ABI in include/tokenflow_b200.h:
 
     extended attention      attn1 closure        -> tf_ext_attn_fwd      (reference :114-199, :224-281)
     NN field                TokenFlowBlock       -> tf_unit_rows + tf_nn_field   (:329-348, util.py:61-69)
     propagation             TokenFlowBlock       -> tf_propagate         (:361-397)
 
 There is no PyTorch/CPU fallback: the first hot-path call constructs `ops.CudaOps`, which raises if
-the library or a B200 is missing.
+the library or an H100 is missing.
 
 Differences from the reference that do not change results:
   * per-pass host work is O(#blocks): module lists are discovered once per model instead of walking
@@ -49,7 +49,7 @@ def _ops():
     global _OPS
     if _OPS is None:
         from .ops import CudaOps
-        _OPS = CudaOps()            # raises without the .so or without a B200: no fallback
+        _OPS = CudaOps()            # raises without the .so or without an H100: no fallback
     return _OPS
 
 
@@ -524,7 +524,7 @@ def make_tokenflow_attention_block(block_class: Type[torch.nn.Module]) -> Type[t
             if getattr(self, "use_ada_layer_norm", False) or getattr(self, "use_ada_layer_norm_zero", False):
                 raise NotImplementedError(
                     "tokenflow_b200: AdaLayerNorm transformer blocks are not part of any Stable-Diffusion "
-                    "UNet and are not supported by the B200 hot path")
+                    "UNet and are not supported by the H100 hot path")
             cross_attention_kwargs = cross_attention_kwargs if cross_attention_kwargs is not None else {}
             n_piv = getattr(self, "_tf_fused", 0)
             if n_piv:

@@ -1,6 +1,4 @@
 """Extended-attention micro-benchmark + accuracy check for one shape (CUDA events, L2 flushed).
-The kernel variant is chosen by the TF_EXT_ATTN_* environment variables (read once per process), so
-tools/attn_variants.sh runs this script once per variant.
 Usage: python tools/attn_bench.py [--S 4096 --dim 320 --heads 8 --n 5 --inject 0] [--tag name]"""
 import argparse
 import json
@@ -69,8 +67,7 @@ def main():
     flops = 4.0 * n * S * S * dim * (2 * n + 1)
     med = ts[len(ts) // 2]
     rec = {"tag": args.tag, "S": S, "d": d, "n": n, "inject": args.inject, "ms": round(med, 4), "best_ms": round(ts[0], 4),
-           "tflops": round(flops / med / 1e9, 1), "max_err": max(errs),
-           "env": {k_: v_ for k_, v_ in os.environ.items() if k_.startswith("TF_EXT_ATTN")}}
+           "tflops": round(flops / med / 1e9, 1), "max_err": max(errs)}
     print(json.dumps(rec), flush=True)
 
 
