@@ -56,6 +56,16 @@ def test_argument_validation_needs_no_gpu(lib):
     assert lib.tf_nn_field(None, None, kf, None, 0, 16, 32, 3, None, None, None) == 0
 
 
+@pytest.mark.parametrize("inject", [0, 1])
+def test_ext_attn_head_dim_over_192_is_rejected_before_any_cuda_call(lib, inject):
+    """No attention variant is compiled above d = 192: the head-dim dispatch fails on the host.  The pointers
+    are host memory, never dereferenced (and no CUDA device is needed)."""
+    buf = (ctypes.c_uint8 * 4096)()
+    p = (ctypes.addressof(buf) + 15) & ~15
+    st = lib.tf_ext_attn_fwd(p, p, p, 200, 2, 16, 1, 200, 200 ** -0.5, inject, p, None)
+    assert st == 3 and b"head dim 200" in lib.tf_last_error()         # TF_ERR_UNSUPPORTED
+
+
 def test_library_is_sm90a_and_uses_wgmma():
     """The shipped cubin is sm_90a and the hot kernels really use wgmma / TMA / mbarrier."""
     import shutil

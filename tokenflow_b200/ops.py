@@ -288,7 +288,8 @@ class CudaOps:
     def nn_field(self, x_unit: torch.Tensor, piv_unit: torch.Tensor, kf_a: Sequence[int],
                  kf_b: Sequence[int]) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
         """x_unit [F,S,dim], piv_unit [K,S,dim] fp16 unit rows → int32 idx_a, idx_b [F,S]
-        (reference tokenflow_utils.py:335-343)."""
+        (reference tokenflow_utils.py:335-343).  The idx_b rows of frames with kf_b < 0 are left unwritten
+        (idx_b is None when no frame has a second keyframe)."""
         F_, S, dim = x_unit.shape
         K = piv_unit.shape[0]
         assert x_unit.dtype == torch.float16 and piv_unit.dtype == torch.float16
@@ -364,7 +365,8 @@ class CudaOps:
         """General form (sharded pivotal pass): `table[j] = (q slab, first k slab, first v slab, number of
         consecutive key slabs)` for output sample j.  q [Q,S,dim], k/v [KV,S,dim] fp16 (column slices of packed
         buffers are read in place) → [len(table), nrows, dim]: only the query tokens [row0, row0 + nrows) are
-        computed (default: all S; row0 a multiple of 128).  Rows past S stay unwritten."""
+        computed (default: all S; row0 a multiple of 128).  When row0 + nrows > S, the output rows of tokens
+        past S (rows S - row0 onwards) are left unwritten."""
         _, S, dim = q.shape
         d = dim // heads
         nrows = S if nrows is None else int(nrows)
