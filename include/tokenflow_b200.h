@@ -132,6 +132,31 @@ int tf_ext_attn_fwd_rows(const void* q, int q_slabs, int64_t q_tok_stride, const
 int tf_cfg_ddim(const void* eps_uncond, const void* eps_cond, const void* x, const float* coef, float guidance,
                 int64_t n, void* out, tf_stream_t stream);
 
+/* ---- UNet body (not part of the reference's hook surface: the Stable-Diffusion UNet it runs) ---- */
+
+/* Channels-last GroupNorm fused with the time-embedding add before it and the SiLU after it:
+ *   out[n,p,c] = [SiLU]( GroupNorm_groups( x[n,p,c] [+ bias[n,c]] ) * gamma[c] + beta[c] )
+ * with the eager fp16 rounding sequence: x + bias rounded to fp16; mean, rstd = rsqrtf(var + fp16(eps)) rounded to
+ * fp16 as ATen stores them; y = fp16(fmaf(rstd*gamma, x, beta - mean*rstd*gamma)) in fp32; SiLU of the fp16 y as
+ * y / (1 + expf(-y)).  Statistics in fp64 over fp32 partials of shifted values;
+ * deterministic (no atomics, fixed reduction order).  Two kernel launches.
+ *   x, out       device [n, hw, c] fp16 dense NHWC (a channels_last [n, c, h, w] tensor), hw = h*w
+ *   bias         device [n, c] fp16 or NULL; row pitch `bias_stride` elements (0 = one row for every sample)
+ *   gamma, beta  device [c] fp16 (the GroupNorm's weight / bias)
+ *   silu         != 0: apply SiLU
+ *   workspace    device, >= tf_group_norm_nhwc_workspace(n, hw, c, groups) bytes, 16-byte aligned, uninitialised
+ * c % 8 == 0 and groups | c (else TF_ERR_INVALID_ARGUMENT); 8 <= c / groups and c <= 4096 (else unsupported). */
+int64_t tf_group_norm_nhwc_workspace(int64_t n, int64_t hw, int c, int groups); /* bytes, or -1 for a bad shape */
+int tf_group_norm_nhwc(const void* x, const void* bias, int64_t bias_stride, const void* gamma, const void* beta,
+                       int64_t n, int64_t hw, int c, int groups, float eps, int silu, void* workspace,
+                       int64_t workspace_bytes, void* out, tf_stream_t stream);
+
+/* GEGLU gate of the transformer blocks' feed-forward: out = fp16(xh * fp16(gelu(gate))), gelu in ATen's erf form
+ * (x/2 * (1 + erff(x / sqrt(2)))), so the result equals the eager `F.linear(x, w_x, b_x) * F.gelu(F.linear(x, w_g,
+ * b_g))` bit for bit given the same GEMM outputs.
+ *   xh, gate, out  device [n] fp16 contiguous */
+int tf_geglu(const void* xh, const void* gate, int64_t n, void* out, tf_stream_t stream);
+
 /* ---- multi-GPU: all-gather of keyframe tensors along the pivotal-sample axis (SURVEY.md §8e) ----
  * NCCL (all-gather over NVLink 5 / NVSwitch) bound at run time; one communicator per process/GPU.
  * Rendezvous: rank 0 calls tf_comm_unique_id and ships the TF_COMM_ID_BYTES to the other ranks by any

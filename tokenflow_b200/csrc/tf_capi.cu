@@ -90,6 +90,20 @@ static int fill_table(FrameTable& tab, const int32_t* kf_a, const int32_t* kf_b,
   return TF_OK;
 }
 
+static int check_group_norm_shape(int64_t n, int64_t hw, int c, int groups) {
+  if (n < 0 || hw < 0 || c <= 0 || (c & 7) || groups <= 0 || c % groups) {
+    set_last_error("tf_group_norm_nhwc: bad shape n=%lld hw=%lld c=%d groups=%d (c %% 8 == 0 and groups | c required)",
+                   (long long)n, (long long)hw, c, groups);
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  if (c / groups < 8 || c > kGnMaxChannels) {
+    set_last_error("tf_group_norm_nhwc: c=%d groups=%d not supported (8 <= c / groups, c <= %d)", c, groups,
+                   kGnMaxChannels);
+    return TF_ERR_UNSUPPORTED;
+  }
+  return TF_OK;
+}
+
 }  // namespace tf
 
 using namespace tf;
@@ -171,6 +185,48 @@ int tf_cfg_ddim(const void* eps_uncond, const void* eps_cond, const void* x, con
     return TF_ERR_INVALID_ARGUMENT;
   }
   int e = launch_cfg_ddim(eps_uncond, eps_cond, x, coef, guidance, n, out, static_cast<cudaStream_t>(stream));
+  if (!e) g_launches += 1;
+  return e;
+}
+
+int64_t tf_group_norm_nhwc_workspace(int64_t n, int64_t hw, int c, int groups) {
+  if (check_group_norm_shape(n, hw, c, groups)) return -1;
+  return (int64_t)group_norm_nhwc_workspace(n, hw, c, groups);
+}
+
+int tf_group_norm_nhwc(const void* x, const void* bias, int64_t bias_stride, const void* gamma, const void* beta,
+                       int64_t n, int64_t hw, int c, int groups, float eps, int silu, void* workspace,
+                       int64_t workspace_bytes, void* out, tf_stream_t stream) {
+  if (int e = check_group_norm_shape(n, hw, c, groups)) return e;
+  if (bias && (bias_stride < 0 || (bias_stride & 7) || (bias_stride > 0 && bias_stride < c))) {
+    set_last_error("tf_group_norm_nhwc: bias row stride %lld (0, or >= c and a multiple of 8)", (long long)bias_stride);
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  if (n == 0 || hw == 0) return TF_OK;
+  const long long need = group_norm_nhwc_workspace(n, hw, c, groups);
+  if (workspace_bytes < need) {
+    set_last_error("tf_group_norm_nhwc: workspace of %lld bytes, %lld needed", (long long)workspace_bytes, need);
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  if (!x || !gamma || !beta || !workspace || !out || !aligned16(x) || !aligned16(out) || !aligned16(workspace) ||
+      (bias && !aligned16(bias))) {
+    set_last_error("tf_group_norm_nhwc: NULL or misaligned pointer");
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  int e = launch_group_norm_nhwc(x, bias, bias_stride, gamma, beta, n, hw, c, groups, eps, silu, workspace, out,
+                                 static_cast<cudaStream_t>(stream));
+  if (!e) g_launches += 2 * ((n + 65534) / 65535);
+  return e;
+}
+
+int tf_geglu(const void* xh, const void* gate, int64_t n, void* out, tf_stream_t stream) {
+  if (n < 0) { set_last_error("tf_geglu: n=%lld", (long long)n); return TF_ERR_INVALID_ARGUMENT; }
+  if (n == 0) return TF_OK;
+  if (!xh || !gate || !out || !aligned16(xh) || !aligned16(gate) || !aligned16(out)) {
+    set_last_error("tf_geglu: NULL or misaligned pointer");
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  int e = launch_geglu(xh, gate, n, out, static_cast<cudaStream_t>(stream));
   if (!e) g_launches += 1;
   return e;
 }

@@ -29,6 +29,14 @@ int launch_layernorm_rows(const void* x_f16, long long rows, int dim, long long 
 int launch_cfg_ddim(const void* eps_uncond, const void* eps_cond, const void* x, const float* coef_dev, float guidance,
                     long long n, void* out, cudaStream_t stream);
 
+// Channels-last GroupNorm (tf_body.cu): 8 <= C / groups, C % 8 == 0, C <= kGnMaxChannels.
+constexpr int kGnMaxChannels = 4096;
+long long group_norm_nhwc_workspace(long long n, long long hw, int c, int groups);
+int launch_group_norm_nhwc(const void* x, const void* bias, long long bias_stride, const void* gamma, const void* beta,
+                           long long n, long long hw, int c, int groups, float eps, int silu, void* workspace,
+                           void* out, cudaStream_t stream);
+int launch_geglu(const void* xh, const void* gate, long long n, void* out, cudaStream_t stream);
+
 int launch_propagate(const void* A, const int32_t* idx_a, const int32_t* idx_b, const FrameTable& tab, int F,
                      int S, int dim, int K, const void* residual, void* out, int out_is_f32, long long F_total,
                      cudaStream_t stream);

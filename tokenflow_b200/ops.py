@@ -59,6 +59,12 @@ _SIGNATURES = {
                                              ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, _c_i32p,
                                              _c_i32p, _c_i32p, _c_i32p, _c_i32p, ctypes.c_int, ctypes.c_int,
                                              ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]),
+    "tf_group_norm_nhwc_workspace": (ctypes.c_int64, [ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int]),
+    "tf_group_norm_nhwc": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
+                                          ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int,
+                                          ctypes.c_float, ctypes.c_int, ctypes.c_void_p, ctypes.c_int64,
+                                          ctypes.c_void_p, ctypes.c_void_p]),
+    "tf_geglu": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
 }
 
 
@@ -384,6 +390,79 @@ class CudaOps:
             _i32([t[2] for t in table]), _i32([t[3] for t in table]), S, heads, d, float(scale), int(row0), nrows,
             out.data_ptr(), self._stream()), "tf_ext_attn_fwd_rows"))
         return out
+
+    # -- UNet body ----------------------------------------------------------------------------
+    @staticmethod
+    def group_norm_nhwc_supported(x: torch.Tensor, norm: torch.nn.GroupNorm) -> bool:
+        """Shapes tf_group_norm_nhwc covers: CUDA fp16 channels_last [N, C, H, W] with C % 8 == 0, C <= 4096, at least
+        8 channels per group and fp16 affine parameters."""
+        if not (x.is_cuda and x.dtype == torch.float16 and x.dim() == 4
+                and x.is_contiguous(memory_format=torch.channels_last)):
+            return False
+        c, g = x.shape[1], norm.num_groups
+        w, b = norm.weight, norm.bias
+        return (c % 8 == 0 and c <= 4096 and c % g == 0 and c // g >= 8 and w is not None and b is not None
+                and w.dtype == b.dtype == torch.float16 and w.is_contiguous() and b.is_contiguous())
+
+    def group_norm_nhwc(self, x: torch.Tensor, norm: torch.nn.GroupNorm, bias: Optional[torch.Tensor] = None,
+                        silu: bool = False) -> torch.Tensor:
+        """[SiLU](GroupNorm(x [+ bias[:, :, None, None]])) of a channels_last fp16 [N, C, H, W] tensor, channels_last
+        out, with the eager fp16 rounding sequence.  `bias` is fp16 [N, C] or [1, C] (the resnet's time-embedding
+        projection).  Two launches; the statistics workspace comes from the caching allocator on this stream."""
+        n, c, h, w = x.shape
+        if bias is not None:
+            assert bias.dtype == torch.float16 and bias.dim() == 2 and bias.shape[1] == c and bias.shape[0] in (1, n)
+            if bias.stride(1) != 1 or bias.stride(0) % 8 or bias.data_ptr() % 16:
+                bias = bias.contiguous()
+            bias_stride = 0 if bias.shape[0] == 1 else bias.stride(0)
+        ws_bytes = int(self.lib.tf_group_norm_nhwc_workspace(n, h * w, c, norm.num_groups))
+        if ws_bytes < 0:
+            self._check(3, "tf_group_norm_nhwc_workspace")
+        ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=x.device)
+        out = torch.empty_like(x, memory_format=torch.channels_last)
+        work = 3.0 * x.numel() * 2 + (n * c * 2 if bias is not None else 0)
+        self._timed("tf_group_norm", work, lambda: self._check(self.lib.tf_group_norm_nhwc(
+            x.data_ptr(), bias.data_ptr() if bias is not None else None, bias_stride if bias is not None else 0,
+            norm.weight.data_ptr(), norm.bias.data_ptr(), n, h * w, c, norm.num_groups, float(norm.eps), int(bool(silu)),
+            ws.data_ptr(), ws.numel(), out.data_ptr(), self._stream()), "tf_group_norm_nhwc"))
+        return out
+
+    def geglu(self, xh: torch.Tensor, gate: torch.Tensor) -> torch.Tensor:
+        """xh * gelu(gate) of two fp16 tensors of one shape (the GEGLU GEMM outputs), bit-equal to the eager product."""
+        assert xh.dtype == gate.dtype == torch.float16 and xh.shape == gate.shape
+        xh, gate = (t if t.is_contiguous() and t.data_ptr() % 16 == 0 else t.contiguous() for t in (xh, gate))
+        out = torch.empty_like(xh)
+        n = xh.numel()
+        self._timed("tf_geglu", 3.0 * n * 2, lambda: self._check(
+            self.lib.tf_geglu(xh.data_ptr(), gate.data_ptr(), n, out.data_ptr(), self._stream()), "tf_geglu"))
+        return out
+
+
+_DEFAULT_OPS = None
+
+
+def default_ops() -> CudaOps:
+    """The process-wide CudaOps (built on first use; raises without the library or an sm_90 device)."""
+    global _DEFAULT_OPS
+    if _DEFAULT_OPS is None:
+        _DEFAULT_OPS = CudaOps()
+    return _DEFAULT_OPS
+
+
+_BODY_OPS = False           # not looked up yet
+
+
+def body_ops() -> Optional[CudaOps]:
+    """The CudaOps the UNet body's fused GroupNorm / GEGLU run on — the same object as the hook layer's, so its
+    per-launch timing covers them — or None when the library or an sm_90 device is missing (the body then runs its
+    ATen ops: CPU runs, fp32 models)."""
+    global _BODY_OPS
+    if _BODY_OPS is False:
+        try:
+            _BODY_OPS = default_ops()
+        except TokenflowB200Error:
+            _BODY_OPS = None
+    return _BODY_OPS
 
 
 class Communicator:

@@ -3,7 +3,12 @@ TokenFlow hooks patch.
 
 `diffusers` is not installed here and there is no network, so the L1 "third-party model runtime"
 (SURVEY.md §1, Appendix B) is restated as a small local module tree.  It is plumbing, not the
-product: every conv / linear / cross-attention here is a stock PyTorch (cuDNN / cuBLAS) call.
+product: every conv / linear / cross-attention here is a stock PyTorch (cuDNN / cuBLAS) call.  Two
+elementwise stages run on the library's kernels when the body runs fp16 channels_last on an H100
+(`norm_act`, `GEGLU`): GroupNorm with the time-embedding add before it and the SiLU after it
+(tf_group_norm_nhwc: ATen has no channels_last GroupNorm and would copy to NCHW and back around every
+norm), and the GEGLU gate (tf_geglu).  Both keep the eager fp16 rounding sequence; anything else (CPU,
+NCHW, fp32, channel counts the kernel does not cover) runs the ATen ops.
 The hooks discover modules *by class name* (reference util.py:46-58) and by the hard-coded SD
 topology (reference tokenflow_utils.py:20-40, 208-214), so the names and nesting below follow the
 mid-2023 diffusers layout:
@@ -66,6 +71,21 @@ class GroupNorm(nn.GroupNorm):
             with torch.autocast("cuda", enabled=False):
                 return F.group_norm(x, self.num_groups, self.weight, self.bias, self.eps)
         return super().forward(x)
+
+
+def norm_act(norm: nn.GroupNorm, x: torch.Tensor, bias: Optional[torch.Tensor] = None,
+             silu: bool = True) -> torch.Tensor:
+    """[SiLU](norm(x [+ bias[:, :, None, None]])): one tf_group_norm_nhwc call (two launches, three passes over x)
+    for CUDA fp16 channels_last input, else the eager ATen sequence (fp16 add, GroupNorm, SiLU)."""
+    from .ops import CudaOps, body_ops
+    if CudaOps.group_norm_nhwc_supported(x, norm) and (bias is None or bias.dtype == torch.float16):
+        ops = body_ops()
+        if ops is not None:
+            return ops.group_norm_nhwc(x, norm, bias, silu)
+    if bias is not None:
+        x = x + bias[:, :, None, None]
+    x = norm(x)
+    return F.silu(x) if silu else x
 
 
 class BodyLayerNorm(nn.LayerNorm):
@@ -136,7 +156,13 @@ class GEGLU(nn.Module):
         # product run vectorised (chunking one fused output leaves strided views and the slow path)
         w_x, w_g = self.proj.weight.chunk(2, dim=0)
         b_x, b_g = self.proj.bias.chunk(2, dim=0)
-        return F.linear(x, w_x, b_x) * F.gelu(F.linear(x, w_g, b_g))
+        xh, g = F.linear(x, w_x, b_x), F.linear(x, w_g, b_g)
+        if xh.is_cuda and xh.dtype == g.dtype == torch.float16:
+            from .ops import body_ops
+            ops = body_ops()
+            if ops is not None:
+                return ops.geglu(xh, g)             # one pass: gelu(g) is never written
+        return xh * F.gelu(g)
 
 
 class FeedForward(nn.Module):
@@ -192,7 +218,7 @@ class Transformer2DModel(nn.Module):
     def forward(self, hidden_states, encoder_hidden_states=None):
         b, c, hh, ww = hidden_states.shape
         residual = hidden_states
-        x = self.norm(hidden_states)
+        x = norm_act(self.norm, hidden_states, silu=False)
         if self.use_linear_projection:
             x = x.permute(0, 2, 3, 1).reshape(b, hh * ww, c)
             x = self.proj_in(x)
@@ -233,13 +259,13 @@ class ResnetBlock2D(nn.Module):
         self.conv_shortcut = nn.Conv2d(in_channels, out_channels, 1) if in_channels != out_channels else None
 
     def forward(self, input_tensor, temb):
-        h = self.conv1(self.nonlinearity(self.norm1(input_tensor)))
-        if temb is not None:
-            h = h + self.time_emb_proj(self.nonlinearity(temb))[:, :, None, None]
-        h = self.conv2(self.dropout(self.nonlinearity(self.norm2(h))))
+        h = self.conv1(norm_act(self.norm1, input_tensor))
+        t = self.time_emb_proj(self.nonlinearity(temb)) if temb is not None else None
+        h = self.conv2(self.dropout(norm_act(self.norm2, h, bias=t)))       # temb add + norm2 + SiLU
         if self.conv_shortcut is not None:
             input_tensor = self.conv_shortcut(input_tensor)
-        return (input_tensor + h) / self.output_scale_factor
+        out = input_tensor + h
+        return out if self.output_scale_factor == 1.0 else out / self.output_scale_factor
 
 
 class Downsample2D(nn.Module):
@@ -426,7 +452,7 @@ class UNet2DConditionModel(nn.Module):
         x = self.mid_block(x, emb, encoder_hidden_states)
         for blk in self.up_blocks:
             x = blk(x, skips, emb, encoder_hidden_states)
-        x = self.conv_out(self.conv_act(self.conv_norm_out(x)))
+        x = self.conv_out(norm_act(self.conv_norm_out, x))          # conv_norm_out + conv_act (SiLU)
         return UNetOutput(sample=x)
 
 

@@ -29,6 +29,7 @@ from typing import List, Optional, Sequence, Type
 
 import torch
 
+from .sd_unet import norm_act
 from .util import isinstance_str, batch_cosine_sim  # noqa: F401  (re-exported like the reference)
 
 __all__ = [
@@ -48,8 +49,8 @@ _OPS = None
 def _ops():
     global _OPS
     if _OPS is None:
-        from .ops import CudaOps
-        _OPS = CudaOps()            # raises without the .so or without an H100: no fallback
+        from .ops import default_ops
+        _OPS = default_ops()        # raises without the .so or without an H100: no fallback
     return _OPS
 
 
@@ -321,7 +322,7 @@ def register_conv_injection(model, injection_schedule):
     def make_forward(res):
         def forward(input_tensor, temb):
             skip = input_tensor
-            h = res.nonlinearity(res.norm1(input_tensor))
+            h = norm_act(res.norm1, input_tensor)
             resample = res.upsample if res.upsample is not None else res.downsample
             if resample is not None:
                 if res.upsample is not None and h.shape[0] >= 64:
@@ -329,14 +330,16 @@ def register_conv_injection(model, injection_schedule):
                 skip, h = resample(skip), resample(h)
             h = res.conv1(h)
             if temb is not None:
-                temb = res.time_emb_proj(res.nonlinearity(temb))[:, :, None, None]
-                if res.time_embedding_norm == "default":
-                    h = h + temb
-            h = res.norm2(h)
-            if temb is not None and res.time_embedding_norm == "scale_shift":
-                scale, shift = torch.chunk(temb, 2, dim=1)
-                h = h * (1 + scale) + shift
-            h = res.conv2(res.dropout(res.nonlinearity(h)))
+                temb = res.time_emb_proj(res.nonlinearity(temb))
+            if res.time_embedding_norm == "default":    # temb add + norm2 + SiLU (one fused kernel on the GPU)
+                h = norm_act(res.norm2, h, bias=temb)
+            else:
+                h = res.norm2(h)
+                if temb is not None and res.time_embedding_norm == "scale_shift":
+                    scale, shift = torch.chunk(temb[:, :, None, None], 2, dim=1)
+                    h = h * (1 + scale) + shift
+                h = res.nonlinearity(h)
+            h = res.conv2(res.dropout(h))
             if _in_schedule(res):
                 def inject_thirds(part):
                     n = part.shape[0] // 3
@@ -361,7 +364,8 @@ def register_conv_injection(model, injection_schedule):
                     h = inject_sharded(h, shard)
             if res.conv_shortcut is not None:
                 skip = res.conv_shortcut(skip)
-            return (skip + h) / res.output_scale_factor
+            out = skip + h
+            return out if res.output_scale_factor == 1.0 else out / res.output_scale_factor
         return forward
 
     conv_module = model.unet.up_blocks[1].resnets[1]
