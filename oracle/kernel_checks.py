@@ -17,6 +17,14 @@ scale-free.  The fixed north-star bound max|got - ref| < 1e-3 (BASELINE.json) st
 kernel's own fp16 operands (dot products accumulated in fp64, rounded to fp16, first index on ties), up to
 rows inside a 1-ulp fp16 tie class, whose winner depends on the GEMM's fp32 accumulation order.  Such
 rows are bounded and counted.
+
+`check_group_norm` compares a tf_group_norm_nhwc output with the eager ATen sequence it replaces and with
+an fp64 evaluation.  ATen stores the group mean and rstd in fp16, so those bounds cannot see a statistics
+error below about one fp16 ulp of the mean or rstd.  `check_group_norm_workspace` closes that gap: it reads
+the kernel's per-chunk partial sums (the caller's workspace, `[N, G, stats_chunks]` of (Σd, Σd²)) and
+compares every entry with an fp64 evaluation to 2^-16 of the chunk's Σ|d| and Σd².  Each fp32 inner sum
+of the kernel runs over at most 32 values (about 2^-19 of their Σ|d| in the worst case); a dropped pixel
+moves a chunk's sums by about 1 / stats_px >= 2^-12 of them.
 """
 from __future__ import annotations
 
@@ -24,6 +32,7 @@ import math
 from typing import Optional, Sequence
 
 import torch
+import torch.nn.functional as F
 
 ATTN_REL_ULP = 2.0 ** -10       # fp16 rounding (2^-11 relative) of P and of the output, with a 2x margin
 ATTN_ABS_FLOOR = 2.0 ** -24
@@ -200,3 +209,200 @@ def check_nn_field(idx_a: torch.Tensor, idx_b: Optional[torch.Tensor], x_unit: t
                                       f"outside the fp16 tie class")
     assert ties <= max(2, int(max_tie_frac * total)), f"{ties}/{total} rows differ from the oracle"
     return {"ties": ties, "total": total}
+
+
+# ------------------------------------------------------------------------------------------------
+# GroupNorm (tf_group_norm_nhwc)
+# ------------------------------------------------------------------------------------------------
+GN_MAX_THREADS = 512            # tf_body.cu kGnMaxThreads
+GN_STATS_CHUNK_BYTES = 64 << 10  # kGnStatsChunkBytes
+GN_APPLY_CHUNK_BYTES = 128 << 10  # kGnApplyChunkBytes
+GN_WS_REL_TOL = 2.0 ** -16       # observed on one H100 80GB HBM3 (400 W): at most 7.6e-8 (Σd) and 2.6e-7 (Σd²) over
+                                 # the 222 shapes of tests/test_gpu_body_kernels.py, 4.9e-8 / 6.5e-8 at the real UNet
+                                 # sites; a dropped pixel moves a chunk by >= 2^-12
+
+
+def gn_layout(hw: int, c: int) -> dict:
+    """tf_body.cu `gn_layout`: one thread per 8-channel column, `rows` pixel rows per CTA, and the pixel chunk of a
+    statistics / apply CTA (a multiple of `rows` of about 64 / 128 KB of input)."""
+    cols = c // 8
+    rows = max(1, GN_MAX_THREADS // cols)
+
+    def chunk(nbytes):
+        px = nbytes // (2 * c)
+        px = -(-px // rows) * rows
+        return max(px, rows)
+
+    stats_px, apply_px = chunk(GN_STATS_CHUNK_BYTES), chunk(GN_APPLY_CHUNK_BYTES)
+    return {"cols": cols, "rows": rows, "threads": -(-cols * rows // 32) * 32, "stats_px": stats_px,
+            "apply_px": apply_px, "stats_chunks": -(-hw // stats_px), "apply_chunks": -(-hw // apply_px)}
+
+
+def ulp16(v: torch.Tensor) -> torch.Tensor:
+    """fp16 spacing at |v| (fp32 tensor of magnitudes): 2^(e - 11) for v = m * 2^e, m in [0.5, 1); 2^-24 below."""
+    _, e = torch.frexp(v.abs())
+    return torch.clamp(torch.ldexp(torch.ones_like(v), e - 11), min=2.0 ** -24)
+
+
+def _add_bias(x, bias):
+    return x if bias is None else x + bias[:, :, None, None]      # the fp16 add, as the eager path rounds it
+
+
+def group_norm_aten(x, norm, bias, silu):
+    """The eager sequence tf_group_norm_nhwc replaces: fp16 add, ATen GroupNorm, SiLU."""
+    y = F.group_norm(_add_bias(x, bias), norm.num_groups, norm.weight, norm.bias, norm.eps)
+    return F.silu(y) if silu else y
+
+
+def group_norm_fp64(x, norm, bias, silu):
+    x = _add_bias(x, bias)
+    n = x.shape[0]
+    xd = x.double().reshape(n, norm.num_groups, -1)
+    mean = xd.mean(-1, keepdim=True)
+    var = ((xd - mean) ** 2).mean(-1, keepdim=True)
+    y = ((xd - mean) / torch.sqrt(var + norm.eps)).reshape(x.shape)
+    y = y * norm.weight.double()[None, :, None, None] + norm.bias.double()[None, :, None, None]
+    return y * torch.sigmoid(y) if silu else y
+
+
+def group_norm_stat_flip_bound(x, norm, bias, silu):
+    """How far the output moves when ATen's fp16 mean or rstd (RowwiseMomentsCUDAKernel<Half> stores both in the input
+    dtype) is one fp16 ulp away: a statistic computed slightly differently can land on the other side of an fp16
+    rounding boundary, and then every output element of that group moves by up to
+    |rstd * gamma| * ulp(mean) + |x - mean| * |gamma| * ulp(rstd); after SiLU, 1.1 (its largest slope) times that plus
+    one ulp of the fp16 pre-activation."""
+    x = _add_bias(x, bias)
+    n, c, h, w = x.shape
+    G = norm.num_groups
+    _, mean, rstd = torch.ops.aten.native_group_norm(x.contiguous(), norm.weight, norm.bias, n, c, h * w, G, norm.eps)
+    mean = mean.float().view(n, G, 1).expand(n, G, c // G).reshape(n, c, 1, 1)
+    rstd = rstd.float().view(n, G, 1).expand(n, G, c // G).reshape(n, c, 1, 1)
+    gamma = norm.weight.float().abs()[None, :, None, None]
+    bound = rstd * gamma * ulp16(mean) + (x.float() - mean).abs() * gamma * ulp16(rstd)
+    if not silu:
+        return bound
+    # SiLU maps a one-ulp difference of its fp16 input y to up to 1.1 ulp(y), more than ulp(silu(y)) for y < 0
+    y = F.group_norm(x, G, norm.weight, norm.bias, norm.eps).float()
+    return 1.1 * (bound + ulp16(y))
+
+
+def aten_misrounded_groups(x, norm, bias) -> torch.Tensor:
+    """[N, G] bool: groups whose ATen fp16 mean or rstd differs from the fp64 statistic rounded to fp16 (ATen's fp32
+    Welford lands on the wrong side of an fp16 rounding boundary)."""
+    x = _add_bias(x, bias)
+    n, c, h, w = x.shape
+    G = norm.num_groups
+    _, mean, rstd = torch.ops.aten.native_group_norm(x.contiguous(), norm.weight, norm.bias, n, c, h * w, G, norm.eps)
+    xd = x.double().reshape(n, G, -1)
+    m = xd.mean(-1)
+    var = ((xd - m[..., None]) ** 2).mean(-1)
+    r = 1.0 / torch.sqrt(var + float(torch.tensor(norm.eps).half()))
+    return (mean.view(n, G) != m.half()) | (rstd.view(n, G) != r.half())
+
+
+def check_group_norm(got: torch.Tensor, x: torch.Tensor, norm, bias: Optional[torch.Tensor], silu: bool,
+                     tag: str = "", exempt_aten_misrounded: bool = False) -> dict:
+    """Assert that `got` is `[SiLU](GroupNorm(x [+ bias[:, :, None, None]]))` as tf_group_norm_nhwc computes it.
+
+    x [N, C, H, W] fp16 (any H, W), bias fp16 [N, C] / [1, C] or None.  At least 99.9 % of the elements are within
+    1 fp16 ulp of ATen; every element is within 1 ulp plus what a one-ulp change of ATen's fp16 mean / rstd explains
+    (`group_norm_stat_flip_bound`); the error against fp64 is no worse than ATen's by more than the same amount.
+    The 99.9 % rule is statistical: with few groups (tiny images, one group) or with statistics ATen's fp32 Welford
+    rounds badly, a single group whose ATen fp16 statistic is misrounded (`aten_misrounded_groups`) exceeds 0.1 % on
+    its own.  `exempt_aten_misrounded` leaves those groups out of the fraction; they still meet the other two bounds.
+    Returns the bit-equal and within-1-ulp fractions."""
+    assert got.dtype == torch.float16 and tuple(got.shape) == tuple(x.shape), (got.dtype, tuple(got.shape))
+    want = group_norm_aten(x, norm, bias, silu)
+    g32, w32 = got.float(), want.float()
+    ulp = ulp16(torch.maximum(g32.abs(), w32.abs()))
+    diff = (g32 - w32).abs()
+    counted = torch.ones_like(diff, dtype=torch.bool)
+    exempt = 0
+    if exempt_aten_misrounded:
+        n, c = x.shape[:2]
+        G = norm.num_groups
+        bad = aten_misrounded_groups(x, norm, bias)
+        exempt = int(bad.sum())
+        counted = ~bad.view(n, G, 1).expand(n, G, c // G).reshape(n, c, 1, 1).expand_as(diff)
+    within = (diff <= ulp)[counted].float().mean().item() if counted.any() else 1.0
+    stats = {"bit_equal": (got == want).float().mean().item(), "within_1ulp": within,
+             "within_1ulp_all": (diff <= ulp).float().mean().item(), "max_ulps": (diff / ulp).max().item(),
+             "exempt_groups": exempt}
+    print(f"{tag}: bit-equal {stats['bit_equal']:.5f}, within 1 ulp {stats['within_1ulp']:.5f} "
+          f"({stats['within_1ulp_all']:.5f} with every group), max |diff| / ulp {stats['max_ulps']:.2f}, "
+          f"groups with misrounded ATen statistics left out {exempt}")
+    assert stats["within_1ulp"] >= 0.999, f"{tag}: only {stats['within_1ulp']:.5f} of the elements within 1 ulp of ATen"
+    flip = group_norm_stat_flip_bound(x, norm, bias, silu)
+    assert (diff <= ulp + flip).all(), f"{tag}: {(diff > ulp + flip).sum().item()} elements off by more than 1 ulp " \
+                                       "plus a one-ulp change of the fp16 statistics"
+    ref = group_norm_fp64(x, norm, bias, silu)
+    err_got = (g32.double() - ref).abs()
+    err_aten = (w32.double() - ref).abs()
+    ulp3 = ulp16(torch.maximum(torch.maximum(g32.abs(), w32.abs()), ref.float().abs())).double()
+    assert (err_got <= err_aten + ulp3 + flip.double()).all(), f"{tag}: less accurate than ATen"
+    return stats
+
+
+def group_norm_partials(x: torch.Tensor, bias: Optional[torch.Tensor], groups: int, stats_px: int):
+    """fp64 (Σd, Σd², Σ|d|), each [N, G, chunks], of d = fp16(x + bias) - shift over the pixel chunks
+    [k * stats_px, min((k + 1) * stats_px, hw)); the shift is the group's element at pixel 0, channel g * cpg."""
+    xv = _add_bias(x, bias)
+    n, c, h, w = xv.shape
+    hw, cpg = h * w, c // groups
+    chunks = -(-hw // stats_px)
+    xd = xv.permute(0, 2, 3, 1).reshape(n, hw, groups, cpg).double()
+    d = xd - xd[:, :1, :, :1]
+    d = torch.cat([d, d.new_zeros(n, chunks * stats_px - hw, groups, cpg)], dim=1).view(n, chunks, stats_px, groups, cpg)
+    sums = [d.sum((2, 4)), (d * d).sum((2, 4)), d.abs().sum((2, 4))]
+    return tuple(s.permute(0, 2, 1).contiguous() for s in sums)
+
+
+def check_group_norm_workspace(ws: torch.Tensor, x: torch.Tensor, bias: Optional[torch.Tensor], groups: int, hw: int,
+                               c: int, tol: float = GN_WS_REL_TOL, tag: str = "") -> dict:
+    """Assert that the statistics workspace a tf_group_norm_nhwc call left behind holds the exact partial sums.
+
+    ws: the workspace bytes (uint8, exactly what `tf_group_norm_nhwc_workspace` asked for), read as
+    [N, G, stats_chunks] of double2 (Σd, Σd²).  Every entry must match `group_norm_partials` to `tol` of the chunk's
+    Σ|d| (first sum) and Σd² (second sum).  Returns the largest error of each sum relative to its scale."""
+    n = x.shape[0]
+    L = gn_layout(hw, c)
+    assert tuple(x.shape[1:2]) == (c,) and x.shape[2] * x.shape[3] == hw, (tuple(x.shape), c, hw)
+    assert ws.dtype == torch.uint8 and ws.numel() == n * groups * L["stats_chunks"] * 16, \
+        f"{tag}: workspace of {ws.numel()} bytes, layout [N={n}, G={groups}, chunks={L['stats_chunks']}] x 16"
+    got = ws.view(torch.float64).view(n, groups, L["stats_chunks"], 2).to(x.device)
+    s1, s2, sabs = group_norm_partials(x, bias, groups, L["stats_px"])
+    e1, e2 = (got[..., 0] - s1).abs(), (got[..., 1] - s2).abs()
+    ok1, ok2 = e1 <= tol * sabs, e2 <= tol * s2
+    stats = {"rel1": (e1 / sabs.clamp_min(1e-300)).max().item(), "rel2": (e2 / s2.clamp_min(1e-300)).max().item()}
+    for ok, name, ref in ((ok1, "sum d", s1), (ok2, "sum d^2", s2)):
+        if not ok.all():
+            i, g, k = (int(v) for v in (~ok).nonzero()[0])
+            j = 0 if name == "sum d" else 1
+            raise AssertionError(f"{tag}: {int((~ok).sum())} workspace entries off in {name}; first at sample {i} "
+                                 f"group {g} chunk {k}: {got[i, g, k, j].item():.17g} vs fp64 {ref[i, g, k].item():.17g}")
+    return stats
+
+
+def guarded_group_norm(lib, x: torch.Tensor, norm, bias: Optional[torch.Tensor], silu: bool, guard: int = 256):
+    """tf_group_norm_nhwc straight through the C ABI into a NaN-filled buffer with guard bands, with a workspace of
+    exactly the size `tf_group_norm_nhwc_workspace` asks for.  Asserts that every output element was written and
+    nothing outside.  Returns (out as a channels_last [N, C, H, W] view, workspace bytes)."""
+    n, c, h, w = x.shape
+    assert x.is_contiguous(memory_format=torch.channels_last)
+    numel = x.numel()
+    buf = torch.full((numel + 2 * guard,), float("nan"), dtype=torch.float16, device=x.device)
+    out = buf[guard:guard + numel]
+    ws = torch.empty(lib.tf_group_norm_nhwc_workspace(n, h * w, c, norm.num_groups), dtype=torch.uint8,
+                     device=x.device)
+    if bias is not None:
+        assert bias.stride(1) == 1
+        bias_stride = 0 if bias.shape[0] == 1 else bias.stride(0)
+    st = lib.tf_group_norm_nhwc(x.data_ptr(), bias.data_ptr() if bias is not None else None,
+                                bias_stride if bias is not None else 0, norm.weight.data_ptr(), norm.bias.data_ptr(),
+                                n, h * w, c, norm.num_groups, float(norm.eps), int(silu), ws.data_ptr(), ws.numel(),
+                                out.data_ptr(), torch.cuda.current_stream().cuda_stream)
+    assert st == 0, lib.tf_last_error()
+    torch.cuda.synchronize()
+    assert torch.isnan(buf[:guard]).all() and torch.isnan(buf[guard + numel:]).all(), "write outside the output"
+    assert not torch.isnan(out).any(), "output element left unwritten"
+    return out.view(n, h, w, c).permute(0, 3, 1, 2), ws

@@ -308,9 +308,12 @@ def test_block_sd15_top_level_shape_vs_reference_gpu_path(inject):
 # ------------------------------------------------------------------------------------------------
 # the CUDA-graphed fused step == the eager fused step, bit for bit, over all three injection variants
 # ------------------------------------------------------------------------------------------------
-def _editor(mode, steps, graph, n_frames=8, batch=2, latent=16, seed=1, strict=False):
+def _editor(mode, steps, graph, n_frames=8, batch=2, latent=16, seed=1, strict=False, kind="tiny",
+            channels_last=False):
     tfu._install_ops_for_testing(None)
-    unet = sd_unet.build_unet("tiny", seed=seed, device="cuda", dtype=torch.float16)
+    unet = sd_unet.build_unet(kind, seed=seed, device="cuda", dtype=torch.float16, init_on_device=kind != "tiny")
+    if channels_last:
+        unet = unet.to(memory_format=torch.channels_last)
     cfg = {"n_frames": n_frames, "batch_size": batch, "n_timesteps": steps, "guidance_scale": 7.5, "mode": mode,
            "pnp_attn_t": 0.5, "pnp_f_t": 0.8, "start": 0.9, "fused_pass": True, "cuda_graph": graph, "keyframe_seed": seed}
     x, text, pnp, src = synthetic_inputs(n_frames, latent, unet.config.cross_attention_dim, steps, seed=seed,
@@ -320,11 +323,16 @@ def _editor(mode, steps, graph, n_frames=8, batch=2, latent=16, seed=1, strict=F
     return ed, x
 
 
-@pytest.mark.parametrize("mode,steps", [("pnp", 5), ("sdedit", 10)])
-def test_cuda_graph_step_identical_to_eager(mode, steps):
-    ed_e, x = _editor(mode, steps, graph=False)
+@pytest.mark.parametrize("mode,steps,kind", [pytest.param("pnp", 5, "tiny", id="pnp-5"),
+                                             pytest.param("sdedit", 10, "tiny", id="sdedit-10"),
+                                             pytest.param("pnp", 5, "sd15", id="pnp-5-sd15-channels_last")])
+def test_cuda_graph_step_identical_to_eager(mode, steps, kind):
+    """The SD1.5 case runs the native body (channels_last: every GroupNorm site on tf_group_norm_nhwc with its
+    workspace from the graph pool, every GEGLU on tf_geglu) inside the captured step."""
+    kw = {} if kind == "tiny" else dict(kind=kind, latent=64, batch=4, channels_last=True)
+    ed_e, x = _editor(mode, steps, graph=False, **kw)
     want = ed_e.sample_loop(x.clone())
-    ed_g, x = _editor(mode, steps, graph=True)
+    ed_g, x = _editor(mode, steps, graph=True, **kw)
     got = ed_g.sample_loop(x.clone())
     assert ed_g.keyframe_log == ed_e.keyframe_log
     if mode == "pnp":
@@ -332,7 +340,7 @@ def test_cuda_graph_step_identical_to_eager(mode, steps):
     assert all(e["replays"] >= 1 for e in ed_g._graphs.values())
     assert torch.equal(got, want), (got.float() - want.float()).abs().max().item()
     # per-launch event nodes of the graphs are readable when timing was on at capture
-    ed_t, x = _editor(mode, steps, graph=True)             # (re-creates the global op object: enable timing after it)
+    ed_t, x = _editor(mode, steps, graph=True, **kw)       # (re-creates the global op object: enable timing after it)
     ops_ = tfu._ops()
     ops_.enable_timing(True)
     try:
@@ -343,6 +351,9 @@ def test_cuda_graph_step_identical_to_eager(mode, steps):
         ops_.enable_timing(False)
     assert kt["tf_ext_attn"]["launches"] == 16 and kt["tf_ext_attn"]["ms"] > 0
     assert ed_t.graph_launches_per_step() >= 16 * 4
+    if kind != "tiny":
+        assert kt["tf_group_norm"]["launches"] == 61 and kt["tf_geglu"]["launches"] == 16, \
+            {k: v["launches"] for k, v in kt.items()}
 
 
 @pytest.mark.parametrize("graph", [False, True])

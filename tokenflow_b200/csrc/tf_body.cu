@@ -17,10 +17,12 @@
 // Rounding follows the eager ATen sequence:  x + bias is rounded to fp16 (the eager add is an fp16 tensor op);
 // mean and rstd = rsqrtf(var_f32 + fp16(eps)) are rounded to fp16 (ATen's RowwiseMomentsCUDAKernel<Half> stores them
 // in the input dtype), a = rstd * gamma, b = -a * mean + beta (ComputeFusedParamsCUDAKernel), y = fp16(fmaf(a, x, b));
-// SiLU of the fp16 y as y / (1 + expf(-y)), rounded.  The statistics are at least as accurate
-// as ATen's fp32 Welford: each value is taken relative to a per-(sample, group) shift (the group's first element,
-// so the sums do not cancel when |mean| >> std), summed in fp32 over the (<= 4) pixels x 8 channels of
-// one load batch of a thread, then in fp64.
+// SiLU of the fp16 y as y / (1 + expf(-y)), rounded.  Each value is taken relative to a per-(sample, group) shift
+// (the group's first element, so the sums do not cancel when |mean| >> std), summed in fp32 over the (<= 4) pixels
+// x 8 channels of one load batch of a thread, then in fp64.  That matches or beats ATen's fp32 Welford while the
+// shift is a typical element of its group.  When the shift is far from the group mean (an outlier of ~1000 in a
+// group of unit spread), var = E[d^2] - mean(d)^2 cancels, the fp32 inner sums of d^2 carry that error, and rstd
+// rounds to the other fp16 neighbour more often than ATen's does (tests/test_gpu_body_kernels.py, outlier_shift).
 //
 // GEGLU.  out = fp16(float(xh) * float(fp16(gelu_erf(float(g))))) — the eager `F.linear(..) * F.gelu(F.linear(..))`
 // with ATen's erf form of gelu, one read of each GEMM output and one write instead of writing and re-reading gelu(g).
