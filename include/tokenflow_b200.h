@@ -132,6 +132,15 @@ int tf_ext_attn_fwd_rows(const void* q, int q_slabs, int64_t q_tok_stride, const
 int tf_cfg_ddim(const void* eps_uncond, const void* eps_cond, const void* x, const float* coef, float guidance,
                 int64_t n, void* out, tf_stream_t stream);
 
+/* Guidance-free DDIM update of the inversion stage (preprocess.py:217-225 inversion, :251-260 reconstruction),
+ * the DDIM half of tf_cfg_ddim with the same fp16 rounding sequence:
+ *     out = h( h(s3 * h( h(x - h(s1 * eps)) * inv_s2 )) + h(s4 * eps) )
+ *   eps, x, out   device [n] fp16 contiguous; out == x (in place) is allowed
+ *   coef   device [4] fp32 (s1, inv_s2, s3, s4): inversion (sigma_prev, 1/mu_prev, mu, sigma), reconstruction
+ *          (sigma, 1/mu, mu_prev, sigma_prev) — in device memory so one captured graph serves every timestep and
+ *          both directions */
+int tf_ddim(const void* eps, const void* x, const float* coef, int64_t n, void* out, tf_stream_t stream);
+
 /* ---- UNet body (not part of the reference's hook surface: the Stable-Diffusion UNet it runs) ---- */
 
 /* Channels-last GroupNorm fused with the time-embedding add before it and the SiLU after it:

@@ -189,6 +189,18 @@ int tf_cfg_ddim(const void* eps_uncond, const void* eps_cond, const void* x, con
   return e;
 }
 
+int tf_ddim(const void* eps, const void* x, const float* coef, int64_t n, void* out, tf_stream_t stream) {
+  if (n < 0) { set_last_error("tf_ddim: n=%lld", (long long)n); return TF_ERR_INVALID_ARGUMENT; }
+  if (n == 0) return TF_OK;
+  if (!eps || !x || !coef || !out || !aligned16(eps) || !aligned16(x) || !aligned16(out)) {
+    set_last_error("tf_ddim: NULL or misaligned pointer");
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  int e = launch_ddim(eps, x, coef, n, out, static_cast<cudaStream_t>(stream));
+  if (!e) g_launches += 1;
+  return e;
+}
+
 int64_t tf_group_norm_nhwc_workspace(int64_t n, int64_t hw, int c, int groups) {
   if (check_group_norm_shape(n, hw, c, groups)) return -1;
   return (int64_t)group_norm_nhwc_workspace(n, hw, c, groups);

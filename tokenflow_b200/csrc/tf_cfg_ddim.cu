@@ -14,6 +14,10 @@
 // 4-float buffer before the replay).
 //
 // HBM-bound and tiny (3 reads + 1 write of the latents, 0.65 MB each at C2): 8 halves per thread.
+//
+// tf_ddim is the same DDIM update without the guidance (the inversion stage's two directions), with the
+// coefficients of the direction it runs: inversion s1 = sigma_prev, inv_s2 = 1/mu_prev, s3 = mu, s4 = sigma;
+// reconstruction s1 = sigma, inv_s2 = 1/mu, s3 = mu_prev, s4 = sigma_prev.
 #include "tf_common.cuh"
 #include "tf_kernels.h"
 
@@ -22,15 +26,20 @@ namespace {
 
 __device__ __forceinline__ float rh(float x) { return __half2float(__float2half_rn(x)); }
 
+// The DDIM half of the step, shared by both kernels so the rounding sequence lives in one place:
+// out = h(h(s3 * h(h(x - h(s1 * e)) * inv_s2)) + h(s4 * e)).
+__device__ __forceinline__ float ddim_one(float e, float xv, float s1, float inv_s2, float s3, float s4) {
+  const float p = rh(rh(xv - rh(s1 * e)) * inv_s2);
+  return rh(rh(s3 * p) + rh(s4 * e));
+}
+
 __global__ void __launch_bounds__(256)
 cfg_ddim_kernel(const __half* __restrict__ eu, const __half* __restrict__ ec, const __half* __restrict__ x,
                 const float* __restrict__ coef, float g, long long n_vec, long long n, __half* __restrict__ out) {
   const float s1 = coef[0], inv_s2 = coef[1], s3 = coef[2], s4 = coef[3];
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   auto one = [&](float u, float c, float xv) -> float {
-    const float e = rh(u + rh(g * rh(c - u)));
-    const float p = rh(rh(xv - rh(s1 * e)) * inv_s2);
-    return rh(rh(s3 * p) + rh(s4 * e));
+    return ddim_one(rh(u + rh(g * rh(c - u))), xv, s1, inv_s2, s3, s4);
   };
   if (i < n_vec) {
     const uint4 ru = reinterpret_cast<const uint4*>(eu)[i];
@@ -54,7 +63,45 @@ cfg_ddim_kernel(const __half* __restrict__ eu, const __half* __restrict__ ec, co
   }
 }
 
+// Guidance-free DDIM update (both directions of the inversion stage, reference preprocess.py:217-225 and
+// :251-260): one read of eps and x, one write.  `out` may alias `x`: every element is read before it is
+// written by the same thread.
+__global__ void __launch_bounds__(256)
+ddim_kernel(const __half* __restrict__ eps, const __half* x, const float* __restrict__ coef, long long n_vec,
+            long long n, __half* out) {
+  const float s1 = coef[0], inv_s2 = coef[1], s3 = coef[2], s4 = coef[3];
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_vec) {
+    const uint4 re = reinterpret_cast<const uint4*>(eps)[i];
+    const uint4 rx = reinterpret_cast<const uint4*>(x)[i];
+    const __half2* he = reinterpret_cast<const __half2*>(&re);
+    const __half2* hx = reinterpret_cast<const __half2*>(&rx);
+    uint4 w;
+    __half2* ho = reinterpret_cast<__half2*>(&w);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float2 ev = __half22float2(he[e]), xv = __half22float2(hx[e]);
+      ho[e] = __floats2half2_rn(ddim_one(ev.x, xv.x, s1, inv_s2, s3, s4), ddim_one(ev.y, xv.y, s1, inv_s2, s3, s4));
+    }
+    reinterpret_cast<uint4*>(out)[i] = w;
+  }
+  if (i == 0) {                                   // tail (n not a multiple of 8)
+    for (long long j = n_vec * 8; j < n; ++j)
+      out[j] = __float2half_rn(ddim_one(__half2float(eps[j]), __half2float(x[j]), s1, inv_s2, s3, s4));
+  }
+}
+
 }  // namespace
+
+int launch_ddim(const void* eps, const void* x, const float* coef_dev, long long n, void* out, cudaStream_t stream) {
+  if (n == 0) return TF_OK;
+  const long long n_vec = n / 8;
+  const long long threads = n_vec > 0 ? n_vec : 1;
+  const unsigned blocks = (unsigned)((threads + 255) / 256);
+  ddim_kernel<<<blocks, 256, 0, stream>>>(static_cast<const __half*>(eps), static_cast<const __half*>(x), coef_dev,
+                                          n_vec, n, static_cast<__half*>(out));
+  return check_cuda(cudaGetLastError(), "tf_ddim launch");
+}
 
 int launch_cfg_ddim(const void* eps_uncond, const void* eps_cond, const void* x, const float* coef_dev, float guidance,
                     long long n, void* out, cudaStream_t stream) {

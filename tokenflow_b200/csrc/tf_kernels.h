@@ -28,6 +28,7 @@ int launch_layernorm_rows(const void* x_f16, long long rows, int dim, long long 
 
 int launch_cfg_ddim(const void* eps_uncond, const void* eps_cond, const void* x, const float* coef_dev, float guidance,
                     long long n, void* out, cudaStream_t stream);
+int launch_ddim(const void* eps, const void* x, const float* coef_dev, long long n, void* out, cudaStream_t stream);
 
 // Channels-last GroupNorm (tf_body.cu): 8 <= C / groups, C % 8 == 0, C <= kGnMaxChannels.
 constexpr int kGnMaxChannels = 4096;

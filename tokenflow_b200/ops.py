@@ -37,6 +37,8 @@ _SIGNATURES = {
                                          ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_void_p]),
     "tf_cfg_ddim": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float,
                                    ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
+    "tf_ddim": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
+                               ctypes.c_void_p]),
     "tf_comm_nccl_version": (ctypes.c_int, []),
     "tf_comm_unique_id": (ctypes.c_int, [ctypes.c_void_p]),
     "tf_comm_init": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_void_p)]),
@@ -289,6 +291,21 @@ class CudaOps:
         self._timed("tf_cfg_ddim", n * 8.0, lambda: self._check(
             self.lib.tf_cfg_ddim(eu.data_ptr(), ec.data_ptr(), xx.data_ptr(), coef.data_ptr(), float(guidance), n,
                                  out.data_ptr(), self._stream()), "tf_cfg_ddim"))
+        return out
+
+    def ddim(self, eps: torch.Tensor, x: torch.Tensor, coef: torch.Tensor,
+             out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Guidance-free DDIM update of the inversion stage (reference preprocess.py:217-225 / :251-260);
+        `coef` = device fp32 [4] (s1, inv_s2, s3, s4), see include/tokenflow_b200.h.  `out` may be `x` (in place)."""
+        assert eps.dtype == x.dtype == torch.float16 and coef.dtype == torch.float32 and coef.is_cuda
+        assert eps.shape == x.shape
+        e = eps if eps.is_contiguous() else eps.contiguous()
+        if out is None:
+            out = torch.empty_like(x, memory_format=torch.contiguous_format)
+        assert out.shape == x.shape and out.dtype == torch.float16 and out.is_contiguous() and x.is_contiguous()
+        n = x.numel()
+        self._timed("tf_ddim", n * 6.0, lambda: self._check(
+            self.lib.tf_ddim(e.data_ptr(), x.data_ptr(), coef.data_ptr(), n, out.data_ptr(), self._stream()), "tf_ddim"))
         return out
 
     def nn_field(self, x_unit: torch.Tensor, piv_unit: torch.Tensor, kf_a: Sequence[int],

@@ -1,19 +1,69 @@
 """The stage in front of the edit: DDIM inversion of the encoded frames and the on-disk hand-off the drivers read
 (reference preprocess.py:198-230 `ddim_inversion`, :232-261 `ddim_sample`, :227-229 / :313-314 the files).
 
-SURVEY.md §8 f-4: this is not part of the hot path — plain UNet forwards, no TokenFlow operator — and the parts of the
-reference's preprocess script that need Stable-Diffusion weights (VAE encode / decode, CLIP text encoder, the depth /
-ControlNet variants) stay out of scope.  What is here is the latent-space arithmetic and the file format, so that a
-latents directory can be produced for, and read back by, `TokenFlowEditor` / the reference drivers
-(`tokenflow_utils.load_source_latents_t`): frames are independent in this stage, so with several ranks each rank
-inverts its own contiguous share and the saved tensors are all-gathered.
+The parts of the reference's preprocess script that need Stable-Diffusion weights (VAE encode / decode, CLIP text
+encoder, the depth / ControlNet variants) stay out of scope.  What is here is the latent-space arithmetic and the file
+format, so that a latents directory can be produced for, and read back by, `TokenFlowEditor` / the reference drivers
+(`tokenflow_utils.load_source_latents_t`), or handed to the editor in memory (`saved_latents`).  Frames are
+independent in this stage, so with several ranks each rank inverts its own contiguous share and the saved tensors are
+all-gathered.
+
+Two paths compute the same steps:
+  * CPU / fp32 UNet: the eager loop below, step by step as the reference writes it;
+  * CUDA fp16 UNet: one CUDA graph of a step over the rank's share (the UNet calls in batches of `batch_size`, then the
+    DDIM update `tf_ddim` in place), replayed for every step of both directions.  The step's timestep and its four
+    DDIM coefficients are read from device buffers the host refreshes per replay; saved timesteps are device-to-device
+    copies into one resident buffer, all-gathered once at the end.
 """
 from __future__ import annotations
 
 import os
-from typing import Iterable, Optional
+from typing import Dict, Iterable, List, Optional, Tuple
 
 import torch
+
+# Which attn1 the graphed path runs: the module's own SDPA forward (False) or the native per-sample attention of
+# `tokenflow_utils.register_native_self_attention`, installed for the duration of the call (True).  SDPA stays: on an
+# H100 80GB HBM3 at a 400 W power limit the native route made the C2 inversion step slower, 132.2 ms against 124.2 ms
+# (tools/invert_bench.py, README.md).  A test seam for that script and the GPU tests, which time and check both
+# routes; not a user option.
+_NATIVE_ATTN1 = False
+
+
+def inversion_coef_tables(scheduler) -> Tuple[torch.Tensor, torch.Tensor]:
+    """fp32 [steps, 4] coefficient rows (s1, inv_s2, s3, s4) of `tf_ddim` for every step of the inversion (ascending
+    timesteps) and of the reconstruction (descending), from `scheduler.timesteps` of the grid that is set.
+
+    The values are the ones the reference's expressions produce (preprocess.py:211-224, :245-259): its alphas are 0-dim
+    fp32 tensors, so `1 - a` and `a ** 0.5` are fp32 operations, and ATen divides the fp16 latents by the 0-dim
+    `mu` as a multiply by the fp32 reciprocal 1 / mu.  `final_alpha_cumprod` stands in for the missing neighbour at
+    both ends of the grid.
+    inversion step i (t = ts_up[i], prev = ts_up[i - 1]):     sigma_prev, 1 / mu_prev, mu, sigma
+    reconstruction step i (t = ts_dn[i], prev = ts_dn[i + 1]): sigma, 1 / mu, mu_prev, sigma_prev"""
+    a = scheduler.alphas_cumprod.cpu()
+    final = scheduler.final_alpha_cumprod.cpu()
+    ts_dn = [int(t) for t in scheduler.timesteps.tolist()]
+    ts_up = ts_dn[::-1]
+    # 0-dim CPU tensor arithmetic, one step at a time, exactly as the reference evaluates it (the CPU's fp32 sqrt is
+    # ATen's, which need not be the correctly rounded one)
+    mu_sigma = lambda alpha: (alpha ** 0.5, (1 - alpha) ** 0.5)
+    inv, rec = [], []
+    for i, t in enumerate(ts_up):
+        mu, sigma = mu_sigma(a[t])
+        mu_p, sigma_p = mu_sigma(a[ts_up[i - 1]] if i > 0 else final)
+        inv.append(torch.stack([sigma_p, 1 / mu_p, mu, sigma]))
+    for i, t in enumerate(ts_dn):
+        mu, sigma = mu_sigma(a[t])
+        mu_p, sigma_p = mu_sigma(a[ts_dn[i + 1]] if i < len(ts_dn) - 1 else final)
+        rec.append(torch.stack([sigma, 1 / mu, mu_p, sigma_p]))
+    return torch.stack(inv), torch.stack(rec)
+
+
+def saved_timesteps(ts_up: List[int], timesteps_to_save: Optional[Iterable[int]]) -> List[int]:
+    """The timesteps of an inversion over `ts_up` whose latents are saved (reference preprocess.py:227-229): those in
+    `timesteps_to_save` (default: all), and the last one."""
+    keep = set(int(t) for t in timesteps_to_save) if timesteps_to_save is not None else set(ts_up)
+    return [t for i, t in enumerate(ts_up) if t in keep or i == len(ts_up) - 1]
 
 
 class LatentInverter:
@@ -24,6 +74,23 @@ class LatentInverter:
         self.device = next(unet.parameters()).device
         self.scheduler.set_timesteps(n_timesteps, device=self.device)
         self.world_size, self.rank, self.group = world_size, rank, group
+        self.comm = None                      # ops.Communicator (C-ABI NCCL all-gather), see attach_communicator
+        self._saved: Dict[int, torch.Tensor] = {}
+        self._graphs = {}                     # (share shape, batch size, cond shape, attn1 route) -> captured step
+        self._graph_pool = None
+        self._tables = None
+        self._use_graph = True                # test seam: False runs the same device path eagerly
+
+    def attach_communicator(self, comm):
+        """Route the final all-gather of the graphed path through the C ABI (tf_allgather) instead of
+        torch.distributed."""
+        self.comm = comm
+
+    def saved_latents(self) -> Dict[int, torch.Tensor]:
+        """{t: [N, 4, h, w]} of the last `ddim_inversion` on the CUDA fp16 path — the tensors it writes as
+        `noisy_latents_<t>.pt`, kept in memory so that `TokenFlowEditor(..., source_latents=
+        inv.saved_latents().__getitem__)` needs no disk round trip."""
+        return self._saved
 
     # -- the two DDIM directions -------------------------------------------------------------------------------
     def _alphas(self, t: int, t_prev: Optional[int]):
@@ -57,6 +124,8 @@ class LatentInverter:
         """Reference preprocess.py:198-230.  latent_frames [N,4,h,w] (clean, VAE-encoded) → the latents at the noisiest
         timestep; `noisy_latents_<t>.pt` is written for every t in `timesteps_to_save` (default: all) and for the
         last one."""
+        if self._graphed_path():
+            return self._device_inversion(cond, latent_frames, save_path, batch_size, save_latents, timesteps_to_save)
         ts = [int(t) for t in reversed(self.scheduler.timesteps.tolist())]                 # ascending noise level
         keep = set(int(t) for t in timesteps_to_save) if timesteps_to_save is not None else set(ts)
         n = latent_frames.shape[0]
@@ -81,6 +150,8 @@ class LatentInverter:
     def ddim_sample(self, x: torch.Tensor, cond: torch.Tensor, batch_size: int) -> torch.Tensor:
         """Reference preprocess.py:232-261: deterministic DDIM reconstruction from the inverted latents (the
         `inverted.mp4` check of the reference, in latent space)."""
+        if self._graphed_path():
+            return self._device_sample(x, cond, batch_size)
         ts = [int(t) for t in self.scheduler.timesteps.tolist()]
         n = x.shape[0]
         lo, hi = self._local(n)
@@ -93,6 +164,147 @@ class LatentInverter:
                 pred_x0 = (xb - sigma * eps) / mu
                 x[b:b + batch_size] = mu_prev * pred_x0 + sigma_prev * eps
         return self._gathered(x, n)
+
+    # -- CUDA fp16: graph-replayed steps ------------------------------------------------------------------------
+    def _graphed_path(self) -> bool:
+        p = next(self.unet.parameters())
+        return p.is_cuda and p.dtype == torch.float16
+
+    def _device_tables(self):
+        """(inversion coefficients, reconstruction coefficients, ascending timesteps, descending timesteps) on the
+        device, for the grid that is set."""
+        ts_dn = [int(t) for t in self.scheduler.timesteps.tolist()]
+        if self._tables is None or self._tables[0] != ts_dn:
+            inv, rec = inversion_coef_tables(self.scheduler)
+            dev = lambda v: v.to(self.device)
+            self._tables = (ts_dn, dev(inv), dev(rec), dev(torch.tensor(ts_dn[::-1])), dev(torch.tensor(ts_dn)))
+        return self._tables[1:]
+
+    def _step_runner(self, share: int, shape, batch_size: int, cond: torch.Tensor):
+        """Static buffers and the step over a share of `share` frames: the UNet over the share in batches of
+        `batch_size`, then `tf_ddim` in place.  Captured once per share shape and replayed; `_use_graph = False` runs
+        the same function eagerly."""
+        from . import tokenflow_utils as tfu
+        ops = tfu._ops()                      # the library is required: raises without it or without an H100
+        bs = max(1, min(batch_size, share))
+        key = (share, tuple(shape), bs, tuple(cond.shape[1:]), _NATIVE_ATTN1, self._use_graph)
+        entry = self._graphs.get(key)
+        if entry is not None:
+            entry["cond"].copy_(cond.expand(bs, -1, -1))
+            return entry
+        dev = self.device
+        st = {"x": torch.zeros((share,) + tuple(shape), dtype=torch.float16, device=dev),
+              "t": torch.zeros((), dtype=torch.int64, device=dev),
+              "coef": torch.zeros(4, dtype=torch.float32, device=dev),
+              "cond": cond.to(dev, torch.float16).repeat(bs, 1, 1)}
+
+        def step():
+            x = st["x"]
+            outs = []
+            for b in range(0, share, bs):
+                xb = x[b:b + bs]
+                out = self.unet(xb, st["t"], encoder_hidden_states=st["cond"][:xb.shape[0]])
+                outs.append(out["sample"] if isinstance(out, dict) else out.sample)
+            eps = outs[0] if len(outs) == 1 else torch.cat(outs)
+            ops.ddim(eps, x, st["coef"], out=x)
+
+        entry = {"st": st, "cond": st["cond"], "step": step, "graph": None}
+        if self._use_graph and share > 0:
+            # warm-up on a side stream (cuDNN autotuning, lazy initialisation, allocator growth), then one capture
+            # into the inverter's private pool.  Both run on the zeroed buffers, before the real latents arrive.
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                for _ in range(2):
+                    step()
+            torch.cuda.current_stream().wait_stream(side)
+            torch.cuda.synchronize()
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph, pool=self._graph_pool, capture_error_mode="thread_local"):
+                step()
+            if self._graph_pool is None:
+                self._graph_pool = graph.pool()
+            entry["graph"] = graph
+        self._graphs[key] = entry
+        return entry
+
+    def _run_steps(self, x_share: torch.Tensor, cond, batch_size: int, coef: torch.Tensor, ts: torch.Tensor,
+                   save_slots: Optional[Dict[int, int]] = None, saved: Optional[torch.Tensor] = None):
+        """All steps of one direction over this rank's share: per step, refresh the timestep and the coefficient row,
+        replay, and copy the latents of a saved step into its slot of `saved`.  Returns the share's final latents."""
+        from . import tokenflow_utils as tfu
+        share = x_share.shape[0]
+        if share == 0:
+            return x_share
+        native = _NATIVE_ATTN1
+        if native:
+            tfu.register_native_self_attention(self.unet)
+        try:
+            entry = self._step_runner(share, x_share.shape[1:], batch_size, cond)
+            st = entry["st"]
+            st["x"].copy_(x_share)
+            for i in range(coef.shape[0]):
+                st["t"].copy_(ts[i])
+                st["coef"].copy_(coef[i])
+                if entry["graph"] is not None:
+                    entry["graph"].replay()
+                else:
+                    entry["step"]()
+                if save_slots is not None and i in save_slots:
+                    saved[save_slots[i], :share].copy_(st["x"])
+            return st["x"].clone()
+        finally:
+            if native:
+                tfu.remove_native_self_attention(self.unet)
+
+    def _all_gather(self, t: torch.Tensor) -> torch.Tensor:
+        if self.world_size == 1:
+            return t
+        if self.comm is not None:
+            return self.comm.all_gather(t.contiguous())
+        import torch.distributed as dist
+        out = torch.empty((self.world_size * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
+        dist.all_gather_into_tensor(out, t.contiguous(), group=self.group)
+        return out
+
+    def _share(self, frames: torch.Tensor) -> Tuple[torch.Tensor, int]:
+        n = frames.shape[0]
+        lo, hi = self._local(n)
+        return frames[lo:hi].to(self.device, torch.float16), -(-n // self.world_size)
+
+    @torch.no_grad()
+    def _device_inversion(self, cond, latent_frames, save_path, batch_size, save_latents, timesteps_to_save):
+        inv_coef, _, ts_up_dev, _ = self._device_tables()
+        ts_up = [int(t) for t in reversed(self.scheduler.timesteps.tolist())]
+        plan = saved_timesteps(ts_up, timesteps_to_save)
+        slots = {ts_up.index(t): k for k, t in enumerate(plan)}
+        n = latent_frames.shape[0]
+        x_share, per = self._share(latent_frames)
+        saved = torch.zeros((len(plan), per) + tuple(latent_frames.shape[1:]), dtype=torch.float16, device=self.device)
+        self._run_steps(x_share, cond, batch_size, inv_coef, ts_up_dev, slots, saved)
+        # one collective after the last step: [G * n_saved, per, ...] -> per saved timestep, the N frames in order
+        full = self._all_gather(saved).view((self.world_size, len(plan), per) + tuple(latent_frames.shape[1:]))
+        self._saved = {t: full[:, k].reshape((self.world_size * per,) + tuple(latent_frames.shape[1:]))[:n].clone()
+                       for k, t in enumerate(plan)}
+        del full, saved
+        if save_latents and save_path is not None and self.rank == 0:
+            os.makedirs(os.path.join(save_path, "latents"), exist_ok=True)
+            for t, v in self._saved.items():
+                torch.save(v, os.path.join(save_path, "latents", f"noisy_latents_{t}.pt"))
+        return self._saved[plan[-1]].clone()
+
+    @torch.no_grad()
+    def _device_sample(self, x, cond, batch_size):
+        _, rec_coef, _, ts_dn_dev = self._device_tables()
+        n = x.shape[0]
+        x_share, per = self._share(x)
+        out = self._run_steps(x_share, cond, batch_size, rec_coef, ts_dn_dev)
+        if self.world_size == 1:
+            return out
+        pad = per - out.shape[0]
+        if pad:
+            out = torch.cat([out, out.new_zeros((pad,) + tuple(out.shape[1:]))])
+        return self._all_gather(out)[:n]
 
 
 def write_inversion_prompt(save_path: str, prompt: str) -> None:

@@ -37,7 +37,7 @@ __all__ = [
     "PivotalShard", "set_strict_dtype", "register_dual_stream",
     "register_time", "load_source_latents_t",
     "register_conv_injection", "register_extended_attention_pnp", "register_extended_attention",
-    "make_tokenflow_attention_block", "set_tokenflow", "isinstance_str", "batch_cosine_sim",
+    "register_native_self_attention", "remove_native_self_attention", "make_tokenflow_attention_block", "set_tokenflow", "isinstance_str", "batch_cosine_sim",
 ]
 
 # --------------------------------------------------------------------------------------------
@@ -495,6 +495,63 @@ def register_extended_attention(model):
     """Reference :216-294 (SDEdit flavour: no injection)."""
     for module in _transformer_blocks(model.unet):
         module.attn1.forward = _sa_forward(module.attn1, pnp=False)
+
+
+# --------------------------------------------------------------------------------------------
+# plain self-attention (the inversion stage's UNet, preprocess.py:222 / :256)
+# --------------------------------------------------------------------------------------------
+_SELF_TABLES = {}
+
+
+def _self_table(n: int):
+    """Every sample attends to its own S keys: table entry (j, j, j, 1)."""
+    tab = _SELF_TABLES.get(n)
+    if tab is None:
+        tab = _SELF_TABLES[n] = [(j, j, j, 1) for j in range(n)]
+    return tab
+
+
+def _plain_sa_forward(attn, fallback):
+    """Per-sample self-attention on tf_ext_attn: q/k/v as one GEMM on the concatenated weight, the kernel reads them in
+    place by token stride, then to_out.  Other inputs (CPU, fp32, biased projections, cross-attention, a mask) go to
+    `fallback`, the forward the module had before."""
+    to_out = attn.to_out[0] if type(attn.to_out) is torch.nn.modules.container.ModuleList else attn.to_out
+
+    def forward(x, encoder_hidden_states=None, attention_mask=None):
+        if (encoder_hidden_states is not None or attention_mask is not None or not x.is_cuda
+                or x.dtype != torch.float16 or any(getattr(attn, n).bias is not None for n in ("to_q", "to_k", "to_v"))
+                or not (torch.is_autocast_enabled() or attn.to_q.weight.dtype == torch.float16)):
+            return fallback(x, encoder_hidden_states=encoder_hidden_states, attention_mask=attention_mask)
+        dim = attn.to_q.weight.shape[0]
+        qkv = torch.nn.functional.linear(x, _fused_weight(attn, ("to_q", "to_k", "to_v"), torch.float16))
+        q, k, v = qkv[..., :dim], qkv[..., dim:2 * dim], qkv[..., 2 * dim:]
+        out = _ops().ext_attn_table(q, k, v, _self_table(x.shape[0]), attn.heads, attn.scale)
+        return to_out(out)
+
+    return forward
+
+
+def register_native_self_attention(unet):
+    """Install the native per-sample self-attention on every transformer block's attn1 (attn2 stays as it is).
+    `remove_native_self_attention` restores the forward each attn1 had before."""
+    for module in _transformer_blocks(unet):
+        attn = module.attn1
+        if "_tf_plain_prev" in attn.__dict__:
+            continue
+        attn._tf_plain_prev = attn.__dict__.get("forward")
+        attn.forward = _plain_sa_forward(attn, attn.forward)
+
+
+def remove_native_self_attention(unet):
+    for module in _transformer_blocks(unet):
+        attn = module.attn1
+        if "_tf_plain_prev" not in attn.__dict__:
+            continue
+        prev = attn.__dict__.pop("_tf_plain_prev")
+        if prev is None:
+            attn.__dict__.pop("forward", None)
+        else:
+            attn.forward = prev
 
 
 # --------------------------------------------------------------------------------------------
