@@ -160,11 +160,36 @@ int tf_group_norm_nhwc(const void* x, const void* bias, int64_t bias_stride, con
                        int64_t n, int64_t hw, int c, int groups, float eps, int silu, void* workspace,
                        int64_t workspace_bytes, void* out, tf_stream_t stream);
 
+/* The same GroupNorm [+ SiLU] at exactly 4 channels per group and without the bias add: the VAE's 128-channel levels
+ * with 32 groups (every 16-byte vector of 8 channels spans two groups).  Same rounding sequence, same determinism,
+ * and the same workspace format, [n, groups, stats_chunks] of (sum d, sum d^2) in fp64.
+ *   x, out       device [n, hw, c] fp16 dense NHWC;  gamma, beta  device [c] fp16
+ *   workspace    device, >= tf_group_norm_nhwc_g4_workspace(n, hw, c, groups) bytes, 16-byte aligned, uninitialised
+ * c % 8 == 0 and c == 4 * groups (else TF_ERR_INVALID_ARGUMENT); c <= 4096 (else unsupported). */
+int64_t tf_group_norm_nhwc_g4_workspace(int64_t n, int64_t hw, int c, int groups); /* bytes, or -1 for a bad shape */
+int tf_group_norm_nhwc_g4(const void* x, const void* gamma, const void* beta, int64_t n, int64_t hw, int c, int groups,
+                          float eps, int silu, void* workspace, int64_t workspace_bytes, void* out, tf_stream_t stream);
+
 /* GEGLU gate of the transformer blocks' feed-forward: out = fp16(xh * fp16(gelu(gate))), gelu in ATen's erf form
  * (x/2 * (1 + erff(x / sqrt(2)))), so the result equals the eager `F.linear(x, w_x, b_x) * F.gelu(F.linear(x, w_g,
  * b_g))` bit for bit given the same GEMM outputs.
  *   xh, gate, out  device [n] fp16 contiguous */
 int tf_geglu(const void* xh, const void* gate, int64_t n, void* out, tf_stream_t stream);
+
+/* ---- pixels in and out of the VAE (the reference's frame loading and saving around encode / decode) ---- */
+
+/* Encoder input from uint8 RGB frames: out = fp16(fp16(2 * fp16(v / 255)) - 1), the value of `2 * imgs - 1` on
+ * `T.ToTensor()(frame).to(torch.float16)` (fp32 true quotient, rounded to fp16, then the fp16 multiply and subtract)
+ * bit for bit.
+ *   frames_u8   device [n_px, 3] uint8 ([N, H, W, 3] frames, n_px = N*H*W), 16-byte aligned
+ *   out_f16     device [n_px, 3] fp16: a channels_last [N, 3, H, W] tensor, 16-byte aligned */
+int tf_frames_to_nhwc(const void* frames_u8, int64_t n_px, void* out_f16, tf_stream_t stream);
+
+/* uint8 frames from the decoder output: ((x / 2 + 0.5).clamp(0, 1) * 255).to(uint8) with every op rounded to fp16 and
+ * truncation at the end, bit for bit; a NaN gives 0, +-Inf give 255 / 0.
+ *   x_f16       device [n_px, 3] fp16 (a channels_last [N, 3, H, W] tensor), 16-byte aligned
+ *   frames_u8   device [n_px, 3] uint8 ([N, H, W, 3]), 16-byte aligned */
+int tf_nhwc_to_frames(const void* x_f16, int64_t n_px, void* frames_u8, tf_stream_t stream);
 
 /* ---- multi-GPU: all-gather of keyframe tensors along the pivotal-sample axis (SURVEY.md §8e) ----
  * NCCL (all-gather over NVLink 5 / NVSwitch) bound at run time; one communicator per process/GPU.

@@ -24,6 +24,11 @@
 // group of unit spread), var = E[d^2] - mean(d)^2 cancels, the fp32 inner sums of d^2 carry that error, and rstd
 // rounds to the other fp16 neighbour more often than ATen's does (tests/test_gpu_body_kernels.py, outlier_shift).
 //
+// tf_group_norm_nhwc_g4 runs the same two kernels at exactly 4 channels per group (the VAE's 128-channel levels with
+// 32 groups), without the bias: a thread's 8-channel column then always spans two groups, the (lo, hi) pair of sums
+// the kernels already carry for columns that straddle a group boundary.  It is compiled for that constant and gets a
+// larger apply chunk (gn_layout_g4).
+//
 // GEGLU.  out = fp16(float(xh) * float(fp16(gelu_erf(float(g))))) — the eager `F.linear(..) * F.gelu(F.linear(..))`
 // with ATen's erf form of gelu, one read of each GEMM output and one write instead of writing and re-reading gelu(g).
 #include "tf_common.cuh"
@@ -61,6 +66,23 @@ GnLayout gn_layout(long long hw, int c) {
   return L;
 }
 
+// The 4-channel-group sites are the VAE's full-resolution levels (512^2 x 128 channels: 64 MB a sample).  Their
+// statistics chunks are gn_layout's, so the workspace has the same [N, G, stats_chunks] format, but every apply CTA
+// reduces all G x stats_chunks partials of its sample first: 512 KB at 512^2, four times a 128 KB apply chunk.  So
+// an apply CTA takes at least 1/64 of the sample (1 MB there): the partials it reads, L2 hits, stay at half its input.
+constexpr int kGnG4ApplyChunksPerSample = 64;
+
+GnLayout gn_layout_g4(long long hw, int c) {
+  GnLayout L = gn_layout(hw, c);
+  long long px = (hw + kGnG4ApplyChunksPerSample - 1) / kGnG4ApplyChunksPerSample;
+  px = (px + L.rows - 1) / L.rows * L.rows;
+  if (px > L.apply_px) {
+    L.apply_px = px;
+    L.apply_chunks = (int)((hw + px - 1) / px);
+  }
+  return L;
+}
+
 __device__ __forceinline__ void unpack8(const uint4& raw, float (&v)[8]) {
   const __half2* h = reinterpret_cast<const __half2*>(&raw);
 #pragma unroll
@@ -81,10 +103,12 @@ __device__ __forceinline__ float group_shift(const __half* xn, const __half* bia
   return kBias ? round_h(v + __half2float(bias_n[c])) : v;
 }
 
-template <bool kBias>
+// kCpg: channels per group when known at compile time (4: the VAE's full-resolution sites), 0 = the runtime `cpg_rt`.
+template <bool kBias, int kCpg>
 __global__ void __launch_bounds__(kGnMaxThreads, 2)
 gn_stats_kernel(const __half* __restrict__ x, const __half* __restrict__ bias, long long bias_stride, long long hw,
-                int C, int cpg, int G, int rows, long long chunk_px, int chunks, double2* __restrict__ ws) {
+                int C, int cpg_rt, int G, int rows, long long chunk_px, int chunks, double2* __restrict__ ws) {
+  const int cpg = kCpg ? kCpg : cpg_rt;
   extern __shared__ double2 part[];                 // [threads][2]: the (<= 2) groups a thread's 8 channels touch
   const int cols = C >> 3;
   const int tid = threadIdx.x;
@@ -158,12 +182,13 @@ gn_stats_kernel(const __half* __restrict__ x, const __half* __restrict__ bias, l
   }
 }
 
-template <bool kBias, bool kSilu>
+template <bool kBias, bool kSilu, int kCpg>
 __global__ void __launch_bounds__(kGnMaxThreads, 2)
 gn_apply_kernel(const __half* __restrict__ x, const __half* __restrict__ bias, long long bias_stride,
                 const __half* __restrict__ gamma, const __half* __restrict__ beta, float eps, long long hw, int C,
-                int cpg, int G, int rows, long long chunk_px, const double2* __restrict__ ws, int stats_chunks,
+                int cpg_rt, int G, int rows, long long chunk_px, const double2* __restrict__ ws, int stats_chunks,
                 __half* __restrict__ out) {
+  const int cpg = kCpg ? kCpg : cpg_rt;
   extern __shared__ float smem[];                   // a[C], b[C], mean[G], rstd[G]
   float* sa = smem;
   float* sb = sa + C;
@@ -287,42 +312,66 @@ long long group_norm_nhwc_workspace(long long n, long long hw, int c, int groups
   return n * groups * (long long)gn_layout(hw, c).stats_chunks * (long long)sizeof(double2);
 }
 
-int launch_group_norm_nhwc(const void* x, const void* bias, long long bias_stride, const void* gamma, const void* beta,
-                           long long n, long long hw, int c, int groups, float eps, int silu, void* workspace,
-                           void* out, cudaStream_t stream) {
-  const GnLayout L = gn_layout(hw, c);
+namespace {
+
+// Both entry points: the same two kernels, the statistics layout of gn_layout (so the workspace has one format), and
+// an apply layout of the caller's choice.  kCpg = 4 has no bias path (no 4-channel-group site adds one).
+template <int kCpg>
+int launch_gn(const GnLayout& L, const __half* xp, const __half* bp, long long bias_stride, const __half* gp,
+              const __half* btp, long long n, long long hw, int c, int groups, float eps, int silu, double2* ws,
+              __half* op, cudaStream_t stream, const char* stats_what, const char* apply_what) {
   const int cpg = c / groups;
   const size_t stats_smem = (size_t)L.threads * 2 * sizeof(double2);
-  const size_t apply_smem = (2 * (size_t)c + 2 * (size_t)groups) * sizeof(float);   // <= 36 KB at C = 4096
-  const __half* xp = static_cast<const __half*>(x);
-  const __half* bp = static_cast<const __half*>(bias);
-  const __half* gp = static_cast<const __half*>(gamma);
-  const __half* btp = static_cast<const __half*>(beta);
-  __half* op = static_cast<__half*>(out);
-  double2* ws = static_cast<double2*>(workspace);
+  const size_t apply_smem = (2 * (size_t)c + 2 * (size_t)groups) * sizeof(float);   // <= 40 KB at C = 4096, G = 1024
   for (long long n0 = 0; n0 < n; n0 += 65535) {     // grid.y is the sample
     const unsigned ny = (unsigned)(n - n0 < 65535 ? n - n0 : 65535);
     const long long off = n0 * hw * c;
     const __half* bn = bp ? bp + n0 * bias_stride : nullptr;
     double2* wsn = ws + n0 * groups * (long long)L.stats_chunks;
     const dim3 gs((unsigned)L.stats_chunks, ny), ga((unsigned)L.apply_chunks, ny);
-    if (bn)
-      gn_stats_kernel<true><<<gs, L.threads, stats_smem, stream>>>(xp + off, bn, bias_stride, hw, c, cpg, groups, L.rows,
-                                                                   L.stats_px, L.stats_chunks, wsn);
-    else
-      gn_stats_kernel<false><<<gs, L.threads, stats_smem, stream>>>(xp + off, nullptr, 0, hw, c, cpg, groups, L.rows,
-                                                                    L.stats_px, L.stats_chunks, wsn);
-    if (int e = check_cuda(cudaGetLastError(), "tf_group_norm_nhwc statistics launch")) return e;
+#define TF_GN_STATS(B)                                                                                             \
+  gn_stats_kernel<B, kCpg><<<gs, L.threads, stats_smem, stream>>>(xp + off, bn, bias_stride, hw, c, cpg, groups,     \
+                                                                  L.rows, L.stats_px, L.stats_chunks, wsn)
 #define TF_GN_APPLY(B, S)                                                                                          \
-  gn_apply_kernel<B, S><<<ga, L.threads, apply_smem, stream>>>(xp + off, bn, bias_stride, gp, btp, eps, hw, c, cpg,   \
-                                                               groups, L.rows, L.apply_px, wsn, L.stats_chunks,     \
-                                                               op + off)
-    if (bn) { if (silu) TF_GN_APPLY(true, true); else TF_GN_APPLY(true, false); }
-    else { if (silu) TF_GN_APPLY(false, true); else TF_GN_APPLY(false, false); }
+  gn_apply_kernel<B, S, kCpg><<<ga, L.threads, apply_smem, stream>>>(xp + off, bn, bias_stride, gp, btp, eps, hw, c,  \
+                                                                     cpg, groups, L.rows, L.apply_px, wsn,          \
+                                                                     L.stats_chunks, op + off)
+    if constexpr (kCpg == 0) {
+      if (bn) TF_GN_STATS(true); else TF_GN_STATS(false);
+    } else {
+      TF_GN_STATS(false);
+    }
+    if (int e = check_cuda(cudaGetLastError(), stats_what)) return e;
+    if constexpr (kCpg == 0) {
+      if (bn) { if (silu) TF_GN_APPLY(true, true); else TF_GN_APPLY(true, false); }
+      else { if (silu) TF_GN_APPLY(false, true); else TF_GN_APPLY(false, false); }
+    } else {
+      if (silu) TF_GN_APPLY(false, true); else TF_GN_APPLY(false, false);
+    }
+#undef TF_GN_STATS
 #undef TF_GN_APPLY
-    if (int e = check_cuda(cudaGetLastError(), "tf_group_norm_nhwc apply launch")) return e;
+    if (int e = check_cuda(cudaGetLastError(), apply_what)) return e;
   }
   return TF_OK;
+}
+
+}  // namespace
+
+int launch_group_norm_nhwc(const void* x, const void* bias, long long bias_stride, const void* gamma, const void* beta,
+                           long long n, long long hw, int c, int groups, float eps, int silu, void* workspace,
+                           void* out, cudaStream_t stream) {
+  return launch_gn<0>(gn_layout(hw, c), static_cast<const __half*>(x), static_cast<const __half*>(bias), bias_stride,
+                      static_cast<const __half*>(gamma), static_cast<const __half*>(beta), n, hw, c, groups, eps, silu,
+                      static_cast<double2*>(workspace), static_cast<__half*>(out), stream,
+                      "tf_group_norm_nhwc statistics launch", "tf_group_norm_nhwc apply launch");
+}
+
+int launch_group_norm_nhwc_g4(const void* x, const void* gamma, const void* beta, long long n, long long hw, int c,
+                              float eps, int silu, void* workspace, void* out, cudaStream_t stream) {
+  return launch_gn<4>(gn_layout_g4(hw, c), static_cast<const __half*>(x), nullptr, 0, static_cast<const __half*>(gamma),
+                      static_cast<const __half*>(beta), n, hw, c, c / 4, eps, silu, static_cast<double2*>(workspace),
+                      static_cast<__half*>(out), stream, "tf_group_norm_nhwc_g4 statistics launch",
+                      "tf_group_norm_nhwc_g4 apply launch");
 }
 
 int launch_geglu(const void* xh, const void* gate, long long n, void* out, cudaStream_t stream) {

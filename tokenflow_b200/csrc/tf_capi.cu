@@ -104,6 +104,19 @@ static int check_group_norm_shape(int64_t n, int64_t hw, int c, int groups) {
   return TF_OK;
 }
 
+static int check_group_norm_g4_shape(int64_t n, int64_t hw, int c, int groups) {
+  if (n < 0 || hw < 0 || c <= 0 || (c & 7) || groups <= 0 || c != 4 * groups) {
+    set_last_error("tf_group_norm_nhwc_g4: bad shape n=%lld hw=%lld c=%d groups=%d (c %% 8 == 0 and c / groups == 4 "
+                   "required)", (long long)n, (long long)hw, c, groups);
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  if (c > kGnMaxChannels) {
+    set_last_error("tf_group_norm_nhwc_g4: c=%d not supported (c <= %d)", c, kGnMaxChannels);
+    return TF_ERR_UNSUPPORTED;
+  }
+  return TF_OK;
+}
+
 }  // namespace tf
 
 using namespace tf;
@@ -228,6 +241,54 @@ int tf_group_norm_nhwc(const void* x, const void* bias, int64_t bias_stride, con
   int e = launch_group_norm_nhwc(x, bias, bias_stride, gamma, beta, n, hw, c, groups, eps, silu, workspace, out,
                                  static_cast<cudaStream_t>(stream));
   if (!e) g_launches += 2 * ((n + 65534) / 65535);
+  return e;
+}
+
+int64_t tf_group_norm_nhwc_g4_workspace(int64_t n, int64_t hw, int c, int groups) {
+  if (check_group_norm_g4_shape(n, hw, c, groups)) return -1;
+  return (int64_t)group_norm_nhwc_workspace(n, hw, c, groups);
+}
+
+int tf_group_norm_nhwc_g4(const void* x, const void* gamma, const void* beta, int64_t n, int64_t hw, int c, int groups,
+                          float eps, int silu, void* workspace, int64_t workspace_bytes, void* out, tf_stream_t stream) {
+  if (int e = check_group_norm_g4_shape(n, hw, c, groups)) return e;
+  if (n == 0 || hw == 0) return TF_OK;
+  const long long need = group_norm_nhwc_workspace(n, hw, c, groups);
+  if (workspace_bytes < need) {
+    set_last_error("tf_group_norm_nhwc_g4: workspace of %lld bytes, %lld needed", (long long)workspace_bytes, need);
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  if (!x || !gamma || !beta || !workspace || !out || !aligned16(x) || !aligned16(out) || !aligned16(workspace)) {
+    set_last_error("tf_group_norm_nhwc_g4: NULL or misaligned pointer");
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  int e = launch_group_norm_nhwc_g4(x, gamma, beta, n, hw, c, eps, silu, workspace, out,
+                                    static_cast<cudaStream_t>(stream));
+  if (!e) g_launches += 2 * ((n + 65534) / 65535);
+  return e;
+}
+
+int tf_frames_to_nhwc(const void* frames_u8, int64_t n_px, void* out_f16, tf_stream_t stream) {
+  if (n_px < 0 || n_px > INT64_MAX / 3) { set_last_error("tf_frames_to_nhwc: n_px=%lld", (long long)n_px); return TF_ERR_INVALID_ARGUMENT; }
+  if (n_px == 0) return TF_OK;
+  if (!frames_u8 || !out_f16 || !aligned16(frames_u8) || !aligned16(out_f16)) {
+    set_last_error("tf_frames_to_nhwc: NULL or misaligned pointer");
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  int e = launch_frames_to_nhwc(frames_u8, 3 * n_px, out_f16, static_cast<cudaStream_t>(stream));
+  if (!e) g_launches += 1;
+  return e;
+}
+
+int tf_nhwc_to_frames(const void* x_f16, int64_t n_px, void* frames_u8, tf_stream_t stream) {
+  if (n_px < 0 || n_px > INT64_MAX / 3) { set_last_error("tf_nhwc_to_frames: n_px=%lld", (long long)n_px); return TF_ERR_INVALID_ARGUMENT; }
+  if (n_px == 0) return TF_OK;
+  if (!x_f16 || !frames_u8 || !aligned16(x_f16) || !aligned16(frames_u8)) {
+    set_last_error("tf_nhwc_to_frames: NULL or misaligned pointer");
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  int e = launch_nhwc_to_frames(x_f16, 3 * n_px, frames_u8, static_cast<cudaStream_t>(stream));
+  if (!e) g_launches += 1;
   return e;
 }
 

@@ -36,7 +36,14 @@ long long group_norm_nhwc_workspace(long long n, long long hw, int c, int groups
 int launch_group_norm_nhwc(const void* x, const void* bias, long long bias_stride, const void* gamma, const void* beta,
                            long long n, long long hw, int c, int groups, float eps, int silu, void* workspace,
                            void* out, cudaStream_t stream);
+// The same kernels at exactly 4 channels per group, no bias (the VAE's 128-channel levels).
+int launch_group_norm_nhwc_g4(const void* x, const void* gamma, const void* beta, long long n, long long hw, int c,
+                              float eps, int silu, void* workspace, void* out, cudaStream_t stream);
 int launch_geglu(const void* xh, const void* gate, long long n, void* out, cudaStream_t stream);
+
+// Pixel conversions around the VAE (tf_pixels.cu); n = elements (pixels x 3).
+int launch_frames_to_nhwc(const void* frames, long long n, void* out, cudaStream_t stream);
+int launch_nhwc_to_frames(const void* x, long long n, void* frames, cudaStream_t stream);
 
 int launch_propagate(const void* A, const int32_t* idx_a, const int32_t* idx_b, const FrameTable& tab, int F,
                      int S, int dim, int K, const void* residual, void* out, int out_is_f32, long long F_total,

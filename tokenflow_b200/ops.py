@@ -66,6 +66,12 @@ _SIGNATURES = {
                                           ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int,
                                           ctypes.c_float, ctypes.c_int, ctypes.c_void_p, ctypes.c_int64,
                                           ctypes.c_void_p, ctypes.c_void_p]),
+    "tf_group_norm_nhwc_g4_workspace": (ctypes.c_int64, [ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int]),
+    "tf_group_norm_nhwc_g4": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64,
+                                             ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_int,
+                                             ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
+    "tf_frames_to_nhwc": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
+    "tf_nhwc_to_frames": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
     "tf_geglu": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
 }
 
@@ -410,16 +416,27 @@ class CudaOps:
 
     # -- UNet body ----------------------------------------------------------------------------
     @staticmethod
-    def group_norm_nhwc_supported(x: torch.Tensor, norm: torch.nn.GroupNorm) -> bool:
-        """Shapes tf_group_norm_nhwc covers: CUDA fp16 channels_last [N, C, H, W] with C % 8 == 0, C <= 4096, at least
-        8 channels per group and fp16 affine parameters."""
+    def _group_norm_nhwc_operands(x: torch.Tensor, norm: torch.nn.GroupNorm) -> bool:
+        """CUDA fp16 channels_last [N, C, H, W] with C % 8 == 0, C <= 4096, groups dividing C and fp16 affine
+        parameters: what both GroupNorm entry points need besides their channels per group."""
         if not (x.is_cuda and x.dtype == torch.float16 and x.dim() == 4
                 and x.is_contiguous(memory_format=torch.channels_last)):
             return False
         c, g = x.shape[1], norm.num_groups
         w, b = norm.weight, norm.bias
-        return (c % 8 == 0 and c <= 4096 and c % g == 0 and c // g >= 8 and w is not None and b is not None
+        return (c % 8 == 0 and c <= 4096 and c % g == 0 and w is not None and b is not None
                 and w.dtype == b.dtype == torch.float16 and w.is_contiguous() and b.is_contiguous())
+
+    @staticmethod
+    def group_norm_nhwc_supported(x: torch.Tensor, norm: torch.nn.GroupNorm) -> bool:
+        """Shapes tf_group_norm_nhwc covers: CUDA fp16 channels_last [N, C, H, W] with C % 8 == 0, C <= 4096, at least
+        8 channels per group and fp16 affine parameters."""
+        return CudaOps._group_norm_nhwc_operands(x, norm) and x.shape[1] // norm.num_groups >= 8
+
+    @staticmethod
+    def group_norm_nhwc_g4_supported(x: torch.Tensor, norm: torch.nn.GroupNorm) -> bool:
+        """Shapes tf_group_norm_nhwc_g4 covers: the same operands with exactly 4 channels per group."""
+        return CudaOps._group_norm_nhwc_operands(x, norm) and x.shape[1] == 4 * norm.num_groups
 
     def group_norm_nhwc(self, x: torch.Tensor, norm: torch.nn.GroupNorm, bias: Optional[torch.Tensor] = None,
                         silu: bool = False) -> torch.Tensor:
@@ -442,6 +459,45 @@ class CudaOps:
             x.data_ptr(), bias.data_ptr() if bias is not None else None, bias_stride if bias is not None else 0,
             norm.weight.data_ptr(), norm.bias.data_ptr(), n, h * w, c, norm.num_groups, float(norm.eps), int(bool(silu)),
             ws.data_ptr(), ws.numel(), out.data_ptr(), self._stream()), "tf_group_norm_nhwc"))
+        return out
+
+    def group_norm_nhwc_g4(self, x: torch.Tensor, norm: torch.nn.GroupNorm, silu: bool = False) -> torch.Tensor:
+        """[SiLU](GroupNorm(x)) of a channels_last fp16 [N, C, H, W] tensor with 4 channels per group (no bias add),
+        channels_last out, with the eager fp16 rounding sequence; the statistics workspace comes from the caching
+        allocator on this stream."""
+        n, c, h, w = x.shape
+        ws_bytes = int(self.lib.tf_group_norm_nhwc_g4_workspace(n, h * w, c, norm.num_groups))
+        if ws_bytes < 0:
+            self._check(1, "tf_group_norm_nhwc_g4_workspace")
+        ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=x.device)
+        out = torch.empty_like(x, memory_format=torch.channels_last)
+        self._timed("tf_group_norm_g4", 3.0 * x.numel() * 2, lambda: self._check(self.lib.tf_group_norm_nhwc_g4(
+            x.data_ptr(), norm.weight.data_ptr(), norm.bias.data_ptr(), n, h * w, c, norm.num_groups, float(norm.eps),
+            int(bool(silu)), ws.data_ptr(), ws.numel(), out.data_ptr(), self._stream()), "tf_group_norm_nhwc_g4"))
+        return out
+
+    def frames_to_nhwc(self, frames: torch.Tensor) -> torch.Tensor:
+        """uint8 RGB frames [N, H, W, 3] (CUDA) -> the encoder input 2 * ToTensor(frames) - 1 as a channels_last fp16
+        [N, 3, H, W] tensor, bit-equal to the reference's host conversion followed by the fp16 ops."""
+        assert frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[-1] == 3 and frames.is_cuda
+        if not frames.is_contiguous() or frames.data_ptr() % 16:
+            frames = frames.contiguous()
+        n, h, w, _ = frames.shape
+        out = torch.empty((n, 3, h, w), dtype=torch.float16, device=frames.device, memory_format=torch.channels_last)
+        self._timed("tf_frames_to_nhwc", 3.0 * n * h * w, lambda: self._check(self.lib.tf_frames_to_nhwc(
+            frames.data_ptr(), n * h * w, out.data_ptr(), self._stream()), "tf_frames_to_nhwc"))
+        return out
+
+    def nhwc_to_frames(self, x: torch.Tensor) -> torch.Tensor:
+        """fp16 decoder output [N, 3, H, W] -> uint8 frames [N, H, W, 3], bit-equal to
+        `((x / 2 + 0.5).clamp(0, 1) * 255).to(torch.uint8)` in fp16 (NaN -> 0)."""
+        assert x.dtype == torch.float16 and x.dim() == 4 and x.shape[1] == 3 and x.is_cuda
+        if not x.is_contiguous(memory_format=torch.channels_last) or x.data_ptr() % 16:
+            x = x.contiguous(memory_format=torch.channels_last)
+        n, _, h, w = x.shape
+        out = torch.empty((n, h, w, 3), dtype=torch.uint8, device=x.device)
+        self._timed("tf_nhwc_to_frames", 3.0 * n * h * w, lambda: self._check(self.lib.tf_nhwc_to_frames(
+            x.data_ptr(), n * h * w, out.data_ptr(), self._stream()), "tf_nhwc_to_frames"))
         return out
 
     def geglu(self, xh: torch.Tensor, gate: torch.Tensor) -> torch.Tensor:

@@ -1,12 +1,17 @@
 """The stage in front of the edit: DDIM inversion of the encoded frames and the on-disk hand-off the drivers read
 (reference preprocess.py:198-230 `ddim_inversion`, :232-261 `ddim_sample`, :227-229 / :313-314 the files).
 
-The parts of the reference's preprocess script that need Stable-Diffusion weights (VAE encode / decode, CLIP text
-encoder, the depth / ControlNet variants) stay out of scope.  What is here is the latent-space arithmetic and the file
-format, so that a latents directory can be produced for, and read back by, `TokenFlowEditor` / the reference drivers
-(`tokenflow_utils.load_source_latents_t`), or handed to the editor in memory (`saved_latents`).  Frames are
-independent in this stage, so with several ranks each rank inverts its own contiguous share and the saved tensors are
-all-gathered.
+The VAE stage around it is here too (`encode_imgs`, `decode_latents`, reference preprocess.py:163-182 and
+run_tokenflow_pnp.py:145-163, on `vae.AutoencoderKL`), and the edit's starting noise (`ddim_eps`, run_tokenflow_pnp.py:
+186-193), so that one process goes from uint8 frames to edited uint8 frames without the disk:
+
+    encode_imgs -> LatentInverter.ddim_inversion -> saved_latents() -> ddim_eps -> scheduler.add_noise ->
+    TokenFlowEditor.sample_loop -> decode_latents
+
+The CLIP text encoder and the depth / ControlNet variants stay out of scope.  The latents directory is still written
+in the reference's format, so it can be read back by `TokenFlowEditor` / the reference drivers
+(`tokenflow_utils.load_source_latents_t`).  Frames are independent in this stage, so with several ranks each rank
+inverts its own contiguous share and the saved tensors are all-gathered.
 
 Two paths compute the same steps:
   * CPU / fp32 UNet: the eager loop below, step by step as the reference writes it;
@@ -305,6 +310,75 @@ class LatentInverter:
         if pad:
             out = torch.cat([out, out.new_zeros((pad,) + tuple(out.shape[1:]))])
         return self._all_gather(out)[:n]
+
+
+def _native_vae(vae) -> bool:
+    p = next(vae.parameters())
+    return p.is_cuda and p.dtype == torch.float16
+
+
+@torch.no_grad()
+def encode_imgs(vae, frames_u8: torch.Tensor, batch_size: int = 10, deterministic: bool = True,
+                generator: Optional[torch.Generator] = None) -> torch.Tensor:
+    """uint8 RGB frames [N, H, W, 3] -> scaled latents [N, 4, H/8, W/8] in the VAE's dtype (reference
+    preprocess.py:174-182, run_tokenflow_pnp.py:145-153): `2 * ToTensor(frames).to(dtype) - 1`, encoded in batches of
+    `batch_size`, the posterior mean (or a sample) times 0.18215.
+
+    A CUDA fp16 VAE gets the uint8 frames on the device and `tf_frames_to_nhwc` computes the encoder input there, bit
+    for bit the reference's host conversion, in the channels_last layout (NCHW when the VAE's weights are NCHW).
+    Otherwise the conversion is the reference's: an fp32 quotient on the host, then the dtype's ops."""
+    from .vae import SCALING_FACTOR
+    assert frames_u8.dtype == torch.uint8 and frames_u8.dim() == 4 and frames_u8.shape[-1] == 3
+    p = next(vae.parameters())
+    if _native_vae(vae):
+        from . import ops as tf_ops
+        imgs = tf_ops.default_ops().frames_to_nhwc(frames_u8.to(p.device))
+        if not vae.encoder.conv_in.weight.is_contiguous(memory_format=torch.channels_last):
+            imgs = imgs.contiguous()
+    else:
+        imgs = frames_u8.cpu().permute(0, 3, 1, 2).contiguous().float().div(255).to(p.dtype).to(p.device)
+        imgs = 2 * imgs - 1
+    latents = []
+    for i in range(0, len(imgs), batch_size):
+        posterior = vae.encode(imgs[i:i + batch_size]).latent_dist
+        latent = posterior.mean if deterministic else posterior.sample(generator)
+        latents.append(latent * SCALING_FACTOR)
+    return torch.cat(latents).contiguous()
+
+
+@torch.no_grad()
+def decode_latents(vae, latents: torch.Tensor, batch_size: int = 10) -> torch.Tensor:
+    """Scaled latents [N, 4, h, w] -> uint8 RGB frames [N, 8h, 8w, 3] on the latents' device (reference
+    preprocess.py:163-172, run_tokenflow_pnp.py:156-163 and the uint8 conversion of util.save_video / ToPILImage):
+    `latents / 0.18215` decoded in batches of `batch_size`, then `((img / 2 + 0.5).clamp(0, 1) * 255).to(uint8)`.
+    A CUDA fp16 VAE runs that conversion as `tf_nhwc_to_frames`, bit for bit, reading the decoder's channels_last
+    output in place."""
+    from .vae import SCALING_FACTOR
+    native = _native_vae(vae)
+    if native:
+        from . import ops as tf_ops
+        ops = tf_ops.default_ops()
+    frames = []
+    for b in range(0, latents.shape[0], batch_size):
+        imgs = vae.decode(1 / SCALING_FACTOR * latents[b:b + batch_size]).sample
+        if native:
+            frames.append(ops.nhwc_to_frames(imgs))
+        else:
+            frames.append(((imgs / 2 + 0.5).clamp(0, 1) * 255).to(torch.uint8).permute(0, 2, 3, 1))
+    return torch.cat(frames).contiguous()
+
+
+def ddim_eps(latents: torch.Tensor, saved: Dict[int, torch.Tensor], scheduler) -> torch.Tensor:
+    """The noise that takes the clean latents to the noisiest inverted ones (reference run_tokenflow_pnp.py:186-193):
+    `saved` is {t: latents} as `LatentInverter.saved_latents()` returns it (the reference globs the
+    noisy_latents_<t>.pt files and takes the largest t), and eps = (x_T - mu_T * x_0) / sigma_T with the scheduler's
+    0-dim fp32 alphas, in fp16."""
+    noisest = max(int(t) for t in saved)
+    noisy = saved[noisest].to(latents.device)
+    alpha_prod_T = scheduler.alphas_cumprod[noisest]
+    mu_T, sigma_T = alpha_prod_T ** 0.5, (1 - alpha_prod_T) ** 0.5
+    eps = (noisy - mu_T * latents) / sigma_T
+    return eps.to(torch.float16)
 
 
 def write_inversion_prompt(save_path: str, prompt: str) -> None:

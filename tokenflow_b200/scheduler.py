@@ -43,5 +43,9 @@ class DDIMScheduler:
         return {"prev_sample": prev}
 
     def add_noise(self, original: torch.Tensor, noise: torch.Tensor, timestep):
-        a = float(self.alphas_cumprod[int(timestep)])
-        return (a ** 0.5 * original + (1 - a) ** 0.5 * noise).to(original.dtype)
+        """diffusers' arithmetic (the edit's start, reference run_tokenflow_pnp.py:257): the alpha is taken in the
+        samples' dtype, and its square roots are tensor ops in that dtype."""
+        alphas = self.alphas_cumprod.to(device=original.device, dtype=original.dtype)
+        t = torch.as_tensor(timestep).to(original.device)
+        a = alphas[t].flatten().view((-1,) + (1,) * (original.dim() - 1))
+        return a ** 0.5 * original + (1 - a) ** 0.5 * noise

@@ -44,10 +44,14 @@ def seed_everything(seed: int):
 
 def save_video(raw_frames: torch.Tensor, save_path: str, fps: int = 10):
     """Reference util.py:88-96 writes h264 through torchvision.io.write_video, which torchvision
-    0.26 no longer ships; frames ([N,3,H,W] in [0,1]) are written with OpenCV instead."""
+    0.26 no longer ships; frames ([N,3,H,W] in [0,1], or uint8 [N,H,W,3] as `preprocess.decode_latents`
+    returns them) are written with OpenCV instead."""
     import cv2
 
-    frames = (raw_frames * 255).to(torch.uint8).cpu().permute(0, 2, 3, 1).numpy()
+    if raw_frames.dtype == torch.uint8:
+        frames = raw_frames.cpu().numpy()
+    else:
+        frames = (raw_frames * 255).to(torch.uint8).cpu().permute(0, 2, 3, 1).numpy()
     h, w = frames.shape[1:3]
     writer = cv2.VideoWriter(save_path, cv2.VideoWriter_fourcc(*"mp4v"), fps, (w, h))
     try:
