@@ -25,6 +25,21 @@ the kernel's per-chunk partial sums (the caller's workspace, `[N, G, stats_chunk
 compares every entry with an fp64 evaluation to 2^-16 of the chunk's Σ|d| and Σd².  Each fp32 inner sum
 of the kernel runs over at most 32 values (about 2^-19 of their Σ|d| in the worst case); a dropped pixel
 moves a chunk's sums by about 1 / stats_px >= 2^-12 of them.
+
+`check_unit_rows` pins tf_unit_rows bit for bit.  The kernel's arithmetic is exact enough to state: the squared
+norm is summed in fp64 (about 2^-50 relative, far below the fp32 rounding of its square root), so
+nrm = fp32(sqrt(Σx²)); the quotient is the IEEE fp32 x / nrm (Markstein's reciprocal-and-one-correction
+sequence, `div_by`), and fp64 division of two fp32 numbers rounded to fp32 is that quotient, since
+53 >= 2 * 24 + 2 bits make the double rounding innocuous.  The output is fp16 of the quotient.  A mismatch
+is exempt only where the kernel's quotient could lawfully be 1 fp32 ulp away and that ulp decides the fp16
+rounding: exactly 1 fp16 ulp off, with the exact fp32 quotient within 1 fp32 ulp of an fp16 midpoint.  Such
+elements are counted; at most `max_exempt` (default one in 2^20) may occur.
+
+`check_layernorm_rows` checks tf_layernorm_rows / tf_layernorm_unit_rows against LayerNorm and unit rows
+evaluated in fp64 (`layernorm_fp64`), with an interval rule: every fp16 output must be the fp16 rounding of
+some value within δ of the fp64 result, δ coming from a first-order error analysis of the kernel's fp32
+pipeline (`layernorm_deltas`).  A correct kernel uses a small fraction of δ; a wrong variance divisor, eps
+or affine parameter, a dropped vector or a row written to the wrong place moves outputs by many δ.
 """
 from __future__ import annotations
 
@@ -406,3 +421,294 @@ def guarded_group_norm(lib, x: torch.Tensor, norm, bias: Optional[torch.Tensor],
     assert torch.isnan(buf[:guard]).all() and torch.isnan(buf[guard + numel:]).all(), "write outside the output"
     assert not torch.isnan(out).any(), "output element left unwritten"
     return out.view(n, h, w, c).permute(0, 3, 1, 2), ws
+
+
+# ------------------------------------------------------------------------------------------------
+# norm1 and unit rows (tf_unit_rows, tf_layernorm_rows, tf_layernorm_unit_rows)
+# ------------------------------------------------------------------------------------------------
+LN_SLOT_CHANNELS = 256          # tf_unit_rows.cu: one register slot of a row = 32 lanes x 8 channels
+LN_MAX_DIM = 1280               # kLnMaxVecPerLane = 5 slots
+U32 = 2.0 ** -24                # unit roundoff of fp32 (half an ulp, relative)
+RSQRTF_ULPS = 2                 # rsqrtf: maximum error 2 ulp (CUDA C++ Programming Guide, single-precision functions)
+UNIT_MAX_EXEMPT_FRAC = 2.0 ** -20
+
+
+def _ord16(t: torch.Tensor) -> torch.Tensor:
+    """fp16 values as integers in value order (+0 and -0 both 0; adjacent finite values differ by 1)."""
+    b = t.contiguous().view(torch.int16).int()
+    return torch.where(b < 0, -(b & 0x7FFF), b)
+
+
+def _from_ord16(o: torch.Tensor) -> torch.Tensor:
+    b = torch.where(o < 0, (-o) | 0x8000, o)
+    return b.to(torch.int32).to(torch.int16).view(torch.float16)        # two's-complement wrap keeps the bits
+
+
+def _ulp32(a: torch.Tensor) -> torch.Tensor:
+    """fp32 spacing at |a| (fp64 tensor): 2^(e - 24) for |a| in [2^(e-1), 2^e); 2^-149 below the normal range."""
+    _, e = torch.frexp(a.abs())
+    return torch.clamp(torch.ldexp(torch.ones_like(a), e - 24), min=2.0 ** -149)
+
+
+def unit_rows_exact(x: torch.Tensor):
+    """tf_unit_rows' arithmetic, stated exactly: (fp16 output, fp32 quotient) of x [..., dim] fp32 / fp16."""
+    dim = x.shape[-1]
+    xd = x.reshape(-1, dim).double()
+    nrm = torch.sqrt((xd * xd).sum(-1, keepdim=True)).float()
+    q = (xd / nrm.double()).float()
+    return q.half().view(x.shape), q.view(x.shape)
+
+
+def _near_fp16_midpoint(q: torch.Tensor) -> torch.Tensor:
+    """True where the fp32 value q lies within 1 fp32 ulp of a midpoint between two adjacent fp16 values."""
+    a = q.double().abs()
+    h = q.abs().half()
+    o = _ord16(h)
+    up, dn = _from_ord16(o + 1).double(), _from_ord16((o - 1).clamp_min(0)).double()
+    hd = h.double()
+    dist = torch.minimum((a - (hd + up) / 2).abs(), (a - (hd + dn) / 2).abs())
+    return dist <= _ulp32(a)
+
+
+def check_unit_rows(got: torch.Tensor, x: torch.Tensor, tag: str = "", max_exempt: Optional[int] = None) -> dict:
+    """Assert that `got` is tf_unit_rows(x): equal to `unit_rows_exact(x)` element for element (±0 alike, NaN exactly
+    where the reference is NaN), up to Markstein-case elements (see the module docstring), which are counted, printed
+    and capped at `max_exempt` (default numel * 2^-20).  Returns {"exempt", "elements"}."""
+    assert got.dtype == torch.float16 and tuple(got.shape) == tuple(x.shape), (got.dtype, tuple(got.shape))
+    want, q = unit_rows_exact(x.detach())
+    g = got.detach().to(want.device)
+    nan_w, nan_g = torch.isnan(want), torch.isnan(g)
+    assert torch.equal(nan_w, nan_g), (f"{tag}: {int((nan_g & ~nan_w).sum())} NaN outputs where the reference is "
+                                       f"finite, {int((nan_w & ~nan_g).sum())} finite where it is NaN")
+    fin = ~nan_w
+    assert torch.isfinite(g[fin]).all(), f"{tag}: infinite output"
+    d = (_ord16(g) - _ord16(want)).abs()
+    d = torch.where(fin, d, torch.zeros_like(d))
+    exempt = (d == 1) & _near_fp16_midpoint(q) & fin
+    bad = (d != 0) & ~exempt
+    n_ex = int(exempt.sum())
+    if bad.any():
+        dim = x.shape[-1]
+        i = int(bad.flatten().nonzero()[0])
+        raise AssertionError(
+            f"{tag}: {int(bad.sum())} of {g.numel()} unit-row elements differ from fp16(x / fp32(||x||)); first at row "
+            f"{i // dim} channel {i % dim}: got {g.flatten()[i].item():.8g}, want {want.flatten()[i].item():.8g} "
+            f"(fp32 quotient {q.flatten()[i].item():.10g}, {int(d.flatten()[i])} fp16 ulps)")
+    cap = int(g.numel() * UNIT_MAX_EXEMPT_FRAC) if max_exempt is None else max_exempt
+    print(f"{tag}: unit rows equal to the exact quotient; Markstein-case elements {n_ex} of {g.numel()}")
+    assert n_ex <= cap, f"{tag}: {n_ex} elements 1 fp16 ulp off next to a midpoint (at most {cap})"
+    return {"exempt": n_ex, "elements": g.numel()}
+
+
+def ln_affine_f32(norm):
+    """The fp32 copies of γ and β the fused kernels read (`CudaOps._affine_f32`), and eps as the fp32 they get."""
+    return (norm.weight.detach().float(), norm.bias.detach().float(),
+            float(torch.tensor(float(norm.eps), dtype=torch.float32)))
+
+
+def layernorm_fp64(x: torch.Tensor, norm) -> dict:
+    """LayerNorm of fp16 x [..., dim] with the kernel's fp32 γ, β and eps, in fp64, as [rows, dim] tensors: y, the unit
+    rows y / ||y||, z = (x - μ) rstd, and per row rstd, var + eps and mean |x|."""
+    dim = x.shape[-1]
+    g, b, eps = ln_affine_f32(norm)
+    xd = x.detach().reshape(-1, dim).double()
+    mu = xd.mean(-1, keepdim=True)
+    v = ((xd - mu) ** 2).mean(-1, keepdim=True) + eps
+    rstd = 1.0 / torch.sqrt(v)
+    z = (xd - mu) * rstd
+    g, b = g.to(xd.device).double(), b.to(xd.device).double()
+    y = z * g + b
+    return {"y": y, "unit": y / y.norm(dim=-1, keepdim=True), "z": z, "rstd": rstd, "v": v,
+            "abs_mean": xd.abs().mean(-1, keepdim=True), "gamma": g}
+
+
+def layernorm_deltas(ref: dict, dim: int):
+    """(δ_y, δ_u) [rows, dim]: first-order bounds on |ŷ - y| of the kernel's fp32 y and on its fp32 unit-row quotient.
+
+    With u = 2^-24 and s = ceil(dim / 256) register slots per lane (tf_layernorm_rows: one warp per row, lane l holding
+    the 8-channel vectors l, l + 32, ...):
+      * Σx: each element passes one pair add, at most 4s chained adds in its lane and 5 butterfly adds, so the fp32 sum
+        is within (4s + 6) u Σ|x|; the mean multiplies by fp32(1/dim) (u) and rounds (u):
+            |Δμ| <= (4s + 8) u A,  A = mean |x|.
+      * Σd² (two-pass, d = x - μ̂): d rounds once (2u in d²), the square once (u), each term passes at most 8s chained
+        adds and 5 butterfly adds, all terms >= 0; Σ(d_i - Δμ)² = Σd_i² + dim Δμ² because Σd_i = 0; then × fp32(1/dim)
+        (2u) and + eps (u):
+            |v̂ - v| / v <= (8s + 5 + 6) u + Δμ² / v,   v = var + eps.
+      * rstd = rsqrtf(v̂): half the relative error of v̂ plus 2 ulp of rsqrtf (2 ulp <= 4u relative):
+            ρ = |v̂ - v| / (2v) + 4u.
+      * y = ((x - μ̂) · rstd) · γ + β in fp32 (d, × rstd, × γ, + β: one rounding each; FMA contraction only removes
+        roundings):
+            δ_y = rstd |γ| |Δμ| + |z γ| (3u + ρ) + u |y|.
+      * unit = fp32(ŷ / fp32(sqrt(Σŷ² in fp64))): with ŷ = y + e, |e| <= δ_y, to first order
+            δ_u = δ_y / N + |unit| Σ_j |unit_j| δ_y,j / N + 3u |unit|,  N = ||y||,
+        the last term being the rounding of the norm (u) and a quotient within 1 ulp (2u).
+    Both carry a relative 2^-20 for the neglected second-order terms and one fp32 ulp of the reference for the check's
+    own fp64 -> fp32 -> fp16 conversion of the interval ends."""
+    s = -(-dim // LN_SLOT_CHANNELS)
+    dmu = (4 * s + 8) * U32 * ref["abs_mean"]
+    rel_v = (8 * s + 11) * U32 + dmu ** 2 / ref["v"]
+    rho = rel_v / 2 + 2 * RSQRTF_ULPS * U32
+    zg = (ref["z"] * ref["gamma"]).abs()
+    d_y = ref["rstd"] * ref["gamma"].abs() * dmu + zg * (3 * U32 + rho) + U32 * ref["y"].abs()
+    unit = ref["unit"]
+    n = ref["y"].norm(dim=-1, keepdim=True)
+    d_u = d_y / n + unit.abs() * (unit.abs() * d_y).sum(-1, keepdim=True) / n + 3 * U32 * unit.abs()
+    margin = lambda d, r: d * (1 + 2.0 ** -20) + _ulp32(r)
+    return margin(d_y, ref["y"]), margin(d_u, unit)
+
+
+def _interval_use(got: torch.Tensor, ref: torch.Tensor, delta: torch.Tensor, what: str, tag: str):
+    """Largest fraction of δ that some t with fp16(t) == got must be from ref; asserts it is <= 1 and that got is
+    finite.  Returns (max use, fraction of elements not equal to fp16(ref))."""
+    g = got.detach().to(ref.device).reshape(ref.shape)
+    assert torch.isfinite(g).all(), f"{tag}: {int((~torch.isfinite(g)).sum())} NaN / Inf {what} elements where the " \
+                                    "fp64 value is finite"
+    o = _ord16(g)
+    gd = g.double()
+    hi = (gd + _from_ord16(o + 1).double()) / 2          # the rounding interval of got (inf beyond 65504)
+    lo = (gd + _from_ord16(o - 1).double()) / 2
+    dist = torch.clamp(lo - ref, min=0) + torch.clamp(ref - hi, min=0)
+    use = dist / delta
+    worst = use.max().item() if use.numel() else 0.0
+    if worst > 1.0:
+        i = int(use.flatten().argmax())
+        dim = ref.shape[-1]
+        raise AssertionError(
+            f"{tag}: {int((use > 1).sum())} of {use.numel()} {what} elements outside fp16([ref - δ, ref + δ]); worst at "
+            f"row {i // dim} channel {i % dim}: got {gd.flatten()[i].item():.8g}, fp64 {ref.flatten()[i].item():.10g}, "
+            f"δ {delta.flatten()[i].item():.3g} ({worst:.3g} δ)")
+    miss = (g != ref.float().half()).double().mean().item() if g.numel() else 0.0
+    return worst, miss
+
+
+def check_layernorm_rows(y: Optional[torch.Tensor], unit: Optional[torch.Tensor], x: torch.Tensor, norm, n_unit: int,
+                         tag: str = "") -> dict:
+    """Assert that y = fp16(LN(x)) and unit = fp16 unit rows of LN(x) for x[:n_unit] are what tf_layernorm_rows
+    computes: every element within the interval rule of `layernorm_deltas` around `layernorm_fp64`, no NaN / Inf.
+    x is fp16 [b, ..., dim] (or [rows, dim]); y None (the frame pass writes none) or x's shape; unit None when
+    n_unit == 0, else the shape of x[:n_unit].  Returns the largest fraction of δ used and the fraction of elements
+    not correctly rounded, for y and for the unit rows."""
+    dim = x.shape[-1]
+    ref = layernorm_fp64(x, norm)
+    d_y, d_u = layernorm_deltas(ref, dim)
+    stats = {}
+    if y is not None:
+        assert y.dtype == torch.float16 and tuple(y.shape) == tuple(x.shape), (y.dtype, tuple(y.shape))
+        stats["y_use"], stats["y_not_rn"] = _interval_use(y, ref["y"], d_y, "y", tag)
+    if n_unit:
+        assert unit is not None and unit.dtype == torch.float16 and tuple(unit.shape) == tuple(x[:n_unit].shape), \
+            (None if unit is None else (unit.dtype, tuple(unit.shape)))
+        r = unit.numel() // dim
+        stats["u_use"], stats["u_not_rn"] = _interval_use(unit, ref["unit"][:r], d_u[:r], "unit-row", tag)
+    return stats
+
+
+NORM1_PROBES = ("randn", "var_10eps", "var_1eps", "var_0.1eps", "offset_200", "offset_-3000", "constant",
+                "outlier_1000", "outlier_30000", "near_60000")
+
+
+def norm1_probe(kind: str, rows: int, dim: int, generator=None) -> torch.Tensor:
+    """fp16 [rows, dim] norm1 inputs of one statistics probe: well-conditioned ("randn": 2z + 0.3), variance near eps
+    ("var_<f>eps": σ² = f * 1e-5, μ = 0), a large common offset (μ = 200, σ = 1; μ = -3000, σ = 16), constant rows,
+    one outlier channel per row at ±1000 / ±30000, or values near ±60000."""
+    z = torch.randn(rows, dim, generator=generator)
+    if kind == "randn":
+        x = 2 * z + 0.3
+    elif kind.startswith("var_"):
+        x = z * math.sqrt(float(kind[4:-3]) * 1e-5)
+    elif kind == "offset_200":
+        x = 200 + z
+    elif kind == "offset_-3000":
+        x = -3000 + 16 * z
+    elif kind == "constant":
+        x = (4 * torch.randn(rows, 1, generator=generator)).expand(rows, dim)
+    elif kind.startswith("outlier_"):
+        x = z.clone()
+        col = torch.randint(0, dim, (rows,), generator=generator)
+        sign = torch.where(torch.rand(rows, generator=generator) < 0.5, -1.0, 1.0)
+        x[torch.arange(rows), col] = sign * float(kind[8:])
+    elif kind == "near_60000":
+        x = torch.sign(z) * (60000 - 3000 * torch.rand(rows, dim, generator=generator))
+    else:
+        raise ValueError(kind)
+    return x.half()
+
+
+def norm1_module(dim: int, gamma: str = "positive", generator=None) -> torch.nn.LayerNorm:
+    """fp16 LayerNorm(dim) (CPU): γ uniform in [0.5, 1.5] ("positive") or standard normal with every 7th channel 0
+    ("signed"); β uniform in [-0.3, 0.3]."""
+    norm = torch.nn.LayerNorm(dim)
+    with torch.no_grad():
+        if gamma == "positive":
+            norm.weight.copy_(0.5 + torch.rand(dim, generator=generator))
+        else:
+            w = torch.randn(dim, generator=generator)
+            w[::7] = 0
+            norm.weight.copy_(w)
+        norm.bias.copy_(0.6 * torch.rand(dim, generator=generator) - 0.3)
+    return norm.half()
+
+
+def guarded_unit_rows(lib, x: torch.Tensor, guard: int = 256) -> torch.Tensor:
+    """tf_unit_rows straight through the C ABI (x a [rows, dim] fp32 / fp16 view with unit last stride) into a
+    NaN-filled buffer with guard bands.  Asserts that every output element was written and nothing outside, and that
+    the call launched once.  Returns the output [rows, dim]."""
+    rows, dim = x.shape
+    assert x.stride(1) == 1
+    buf = torch.full((rows * dim + 2 * guard,), float("nan"), dtype=torch.float16, device=x.device)
+    out = buf[guard:guard + rows * dim]
+    n0 = lib.tf_launch_count()
+    st = lib.tf_unit_rows(x.data_ptr(), int(x.dtype == torch.float32), rows, dim, x.stride(0), out.data_ptr(),
+                          torch.cuda.current_stream().cuda_stream)
+    assert st == 0, lib.tf_last_error()
+    torch.cuda.synchronize()
+    assert lib.tf_launch_count() == n0 + (1 if rows else 0)
+    assert torch.isnan(buf[:guard]).all() and torch.isnan(buf[guard + rows * dim:]).all(), "write outside the output"
+    out = out.view(rows, dim)
+    want_nan = torch.isnan(unit_rows_exact(x)[0])
+    assert torch.equal(torch.isnan(out), want_nan), "output element left unwritten (or NaN where the reference is not)"
+    return out
+
+
+def guarded_layernorm_rows(lib, x: torch.Tensor, norm, unit_rows: int, y_pitch: Optional[int] = None,
+                           unit_pitch: Optional[int] = None, with_y: bool = True, guard: int = 256):
+    """tf_layernorm_rows (or, with `with_y=False` and unit rows of every row, tf_layernorm_unit_rows) straight through
+    the C ABI, x a [rows, dim] fp16 view, into NaN-filled outputs of row pitch `y_pitch` / `unit_pitch` (default dim)
+    with guard bands.  Asserts that exactly the [rows, dim] / [unit_rows, dim] elements were written: not the gap
+    columns of a pitch > dim, not the guard bands.  Returns (y or None, unit or None) as [rows, dim] views."""
+    rows, dim = x.shape
+    assert x.stride(1) == 1 and x.dtype == torch.float16
+    gamma, beta, eps = ln_affine_f32(norm)
+    gamma, beta = gamma.to(x.device).contiguous(), beta.to(x.device).contiguous()
+
+    def sentinel(n, pitch):
+        buf = torch.full((n * pitch + 2 * guard,), float("nan"), dtype=torch.float16, device=x.device)
+        return buf, buf[guard:guard + n * pitch].view(n, pitch)
+
+    y_pitch, unit_pitch = y_pitch or dim, unit_pitch or dim
+    ybuf, ymat = sentinel(rows, y_pitch) if with_y else (None, None)
+    ubuf, umat = sentinel(unit_rows, unit_pitch) if unit_rows else (None, None)
+    n0 = lib.tf_launch_count()
+    stream = torch.cuda.current_stream().cuda_stream
+    if with_y:
+        st = lib.tf_layernorm_rows(x.data_ptr(), rows, dim, x.stride(0), gamma.data_ptr(), beta.data_ptr(), eps,
+                                   ymat.data_ptr(), y_pitch, umat.data_ptr() if unit_rows else None, unit_pitch,
+                                   unit_rows, stream)
+    else:
+        assert unit_rows == rows and unit_pitch == dim
+        st = lib.tf_layernorm_unit_rows(x.data_ptr(), rows, dim, x.stride(0), gamma.data_ptr(), beta.data_ptr(), eps,
+                                        umat.data_ptr(), stream)
+    assert st == 0, lib.tf_last_error()
+    torch.cuda.synchronize()
+    assert lib.tf_launch_count() == n0 + (1 if rows and (with_y or unit_rows) else 0)
+    outs = []
+    for buf, mat, n in ((ybuf, ymat, rows), (ubuf, umat, unit_rows)):
+        if buf is None:
+            outs.append(None)
+            continue
+        assert torch.isnan(buf[:guard]).all() and torch.isnan(buf[guard + n * mat.shape[1]:]).all(), \
+            "write outside the output"
+        assert torch.isnan(mat[:, dim:]).all(), "write into the gap columns of a packed output"
+        assert not torch.isnan(mat[:, :dim]).any(), "output element left unwritten"
+        outs.append(mat[:, :dim])
+    return tuple(outs)

@@ -14,7 +14,8 @@ counted, bounded, and every one of them is checked.
 import pytest
 import torch
 
-from oracle.kernel_checks import check_ext_attn, check_nn_field, ext_attn_samples, tie_class
+from oracle.kernel_checks import (check_ext_attn, check_layernorm_rows, check_nn_field, check_unit_rows,
+                                  ext_attn_samples, tie_class)
 from oracle.oracle_ops import OracleOps
 from oracle import golden
 
@@ -50,14 +51,12 @@ def test_unit_rows(ops, rows, dim):
     torch.manual_seed(rows + dim)
     x = torch.randn(rows, dim, device="cuda") * 3 + 0.5
     got = ops.unit_rows(x)
-    want = (x / x.norm(dim=-1, keepdim=True)).half()
     assert got.dtype == torch.float16 and got.shape == x.shape
-    diff = (got.float() - want.float()).abs()
-    # identical up to the last-ulp rounding of the fp32 norm reduction order
-    assert diff.max().item() <= 1e-3
-    assert (got != want).float().mean().item() < 2e-3
-    got16 = ops.unit_rows(x.half())
-    assert (got16.float() - want.float()).abs().max().item() < 2e-3
+    check_unit_rows(got, x, tag=f"fp32 {rows}x{dim}")                 # fp16(x / fp32(||x||)), bit for bit
+    check_unit_rows(ops.unit_rows(x.half()), x.half(), tag=f"fp16 {rows}x{dim}")
+    # reference semantics: torch's x / x.norm(), up to the last-ulp rounding of its fp32 norm reduction
+    want = (x / x.norm(dim=-1, keepdim=True)).half()
+    assert (got.float() - want.float()).abs().max().item() <= 1e-3
 
 
 @pytest.mark.parametrize("rows,dim", [(3, 8), (100, 40), (4096, 320), (2048, 640), (512, 1280)])
@@ -70,11 +69,14 @@ def test_layernorm_unit_rows(ops, rows, dim):
         norm.bias.uniform_(-0.3, 0.3)
     x = (torch.randn(rows, dim, device="cuda") * 2 + 0.3).half()
     got = ops.layernorm_unit_rows(x, norm)
-    y = torch.nn.functional.layer_norm(x.float(), (dim,), norm.weight.float(), norm.bias.float(), norm.eps)
-    want = (y / y.norm(dim=-1, keepdim=True)).half()
     assert got.dtype == torch.float16 and got.shape == x.shape
+    check_layernorm_rows(None, got, x, norm, rows, tag=f"{rows}x{dim}")
+    # reference semantics: autocast's fp32 norm1 output, normalised in fp32
+    with torch.autocast("cuda", dtype=torch.float16):
+        y = norm(x)
+    assert y.dtype == torch.float32
+    want = (y / y.norm(dim=-1, keepdim=True)).half()
     assert (got.float() - want.float()).abs().max().item() <= 1e-3
-    assert (got != want).float().mean().item() < 5e-3         # last-ulp rounding of the fp32 statistics only
     # strided source-stream view (first third of a [3B, S, dim] tensor)
     x3 = torch.cat([x, x * 2, x + 1]).view(3, rows, dim)
     assert torch.equal(ops.layernorm_unit_rows(x3[0], norm), got)

@@ -18,12 +18,51 @@ namespace {
 constexpr int kWarpsPerBlock = 8;
 
 // x / y with one reciprocal per row: q = x*r, then one Newton correction q + (x - y*q)*r (Markstein).
-// With r the correctly rounded 1/y this is the correctly rounded quotient except in rare half-ulp
-// cases — i.e. the IEEE division the reference's `x / norm` performs, at 3 FMA-pipe instructions per
+// With r the correctly rounded 1/y, and the remainder x - y*q exact, this is the correctly rounded
+// quotient — the IEEE division the reference's `x / norm` performs — at 3 FMA-pipe instructions per
 // element instead of a MUFU.RCP + fix-up sequence per element (the kernel was XU-bound on divisions).
+// Both conditions fail at extreme norms: 1/y is subnormal above 2^126 and infinite below 2^-128, and the
+// remainder of an element below about 2^-103 underflows.  Every element that can reach a non-zero fp16
+// output is at least 2^-26 * y, so for y in [2^-64, 2^64] both hold; rows outside that range (a zero
+// or non-finite norm included) take the IEEE division.  The choice is made once per row (the norm is the
+// same on every lane), so the element loop of ordinary rows is unchanged.
+__device__ __forceinline__ bool div_by_needs_ieee(float y) { return !(y >= 0x1p-64f && y <= 0x1p64f); }
+
+template <bool kIeee>
 __device__ __forceinline__ float div_by(float x, float y, float r) {
+  if (kIeee) return __fdiv_rn(x, y);
   const float q = x * r;
   return fmaf(fmaf(-y, q, x), r, q);
+}
+
+template <bool kInF32, bool kIeee>
+__device__ __forceinline__ void write_unit_row(const void* __restrict__ x, long long r, int dim, long long row_stride,
+                                               int lane, float nrm, float rcp, __half* __restrict__ orow) {
+  if (kInF32) {
+    const float* xr = static_cast<const float*>(x) + r * row_stride;
+    for (int c = lane * 4; c < dim; c += 128) {
+      float4 v = *reinterpret_cast<const float4*>(xr + c);
+      __half2 lo = __floats2half2_rn(div_by<kIeee>(v.x, nrm, rcp), div_by<kIeee>(v.y, nrm, rcp));
+      __half2 hi = __floats2half2_rn(div_by<kIeee>(v.z, nrm, rcp), div_by<kIeee>(v.w, nrm, rcp));
+      uint2 o2;
+      o2.x = *reinterpret_cast<uint32_t*>(&lo);
+      o2.y = *reinterpret_cast<uint32_t*>(&hi);
+      *reinterpret_cast<uint2*>(orow + c) = o2;
+    }
+  } else {
+    const __half* xr = static_cast<const __half*>(x) + r * row_stride;
+    for (int c = lane * 4; c < dim; c += 128) {
+      uint2 raw = *reinterpret_cast<const uint2*>(xr + c);
+      float2 a = __half22float2(*reinterpret_cast<__half2*>(&raw.x));
+      float2 b = __half22float2(*reinterpret_cast<__half2*>(&raw.y));
+      __half2 lo = __floats2half2_rn(div_by<kIeee>(a.x, nrm, rcp), div_by<kIeee>(a.y, nrm, rcp));
+      __half2 hi = __floats2half2_rn(div_by<kIeee>(b.x, nrm, rcp), div_by<kIeee>(b.y, nrm, rcp));
+      uint2 o2;
+      o2.x = *reinterpret_cast<uint32_t*>(&lo);
+      o2.y = *reinterpret_cast<uint32_t*>(&hi);
+      *reinterpret_cast<uint2*>(orow + c) = o2;
+    }
+  }
 }
 
 template <bool kInF32>
@@ -55,31 +94,10 @@ unit_rows_kernel(const void* __restrict__ x, long long rows, int dim, long long 
     const float nrm = (float)sqrt(ss);
     const float rcp = __frcp_rn(nrm);
     __half* orow = out + r * dim;
-    if (kInF32) {
-      const float* xr = static_cast<const float*>(x) + r * row_stride;
-      for (int c = lane * 4; c < dim; c += 128) {
-        float4 v = *reinterpret_cast<const float4*>(xr + c);
-        __half2 lo = __floats2half2_rn(div_by(v.x, nrm, rcp), div_by(v.y, nrm, rcp));
-        __half2 hi = __floats2half2_rn(div_by(v.z, nrm, rcp), div_by(v.w, nrm, rcp));
-        uint2 o2;
-        o2.x = *reinterpret_cast<uint32_t*>(&lo);
-        o2.y = *reinterpret_cast<uint32_t*>(&hi);
-        *reinterpret_cast<uint2*>(orow + c) = o2;
-      }
-    } else {
-      const __half* xr = static_cast<const __half*>(x) + r * row_stride;
-      for (int c = lane * 4; c < dim; c += 128) {
-        uint2 raw = *reinterpret_cast<const uint2*>(xr + c);
-        float2 a = __half22float2(*reinterpret_cast<__half2*>(&raw.x));
-        float2 b = __half22float2(*reinterpret_cast<__half2*>(&raw.y));
-        __half2 lo = __floats2half2_rn(div_by(a.x, nrm, rcp), div_by(a.y, nrm, rcp));
-        __half2 hi = __floats2half2_rn(div_by(b.x, nrm, rcp), div_by(b.y, nrm, rcp));
-        uint2 o2;
-        o2.x = *reinterpret_cast<uint32_t*>(&lo);
-        o2.y = *reinterpret_cast<uint32_t*>(&hi);
-        *reinterpret_cast<uint2*>(orow + c) = o2;
-      }
-    }
+    if (div_by_needs_ieee(nrm))
+      write_unit_row<kInF32, true>(x, r, dim, row_stride, lane, nrm, rcp, orow);
+    else
+      write_unit_row<kInF32, false>(x, r, dim, row_stride, lane, nrm, rcp, orow);
   }
 }
 
@@ -121,6 +139,23 @@ namespace tf {
 namespace {
 
 constexpr int kLnMaxVecPerLane = 5;     // 5 x 8 halves x 32 lanes = 1280 channels
+
+template <bool kIeee>
+__device__ __forceinline__ void write_ln_unit_row(const float (&v)[kLnMaxVecPerLane][8], int lane, int nvec, float nrm,
+                                                  float rcp, __half* __restrict__ orow) {
+#pragma unroll
+  for (int j = 0; j < kLnMaxVecPerLane; ++j) {
+    const int vi = lane + 32 * j;
+    if (vi < nvec) {
+      uint4 w;
+      __half2* h = reinterpret_cast<__half2*>(&w);
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        h[e] = __floats2half2_rn(div_by<kIeee>(v[j][2 * e], nrm, rcp), div_by<kIeee>(v[j][2 * e + 1], nrm, rcp));
+      *reinterpret_cast<uint4*>(orow + vi * 8) = w;
+    }
+  }
+}
 
 __global__ void __launch_bounds__(kWarpsPerBlock * 32)
 layernorm_rows_kernel(const __half* __restrict__ x, long long rows, int dim, long long row_stride,
@@ -202,18 +237,10 @@ layernorm_rows_kernel(const __half* __restrict__ x, long long rows, int dim, lon
     const float nrm = (float)sqrt(ss);
     const float rcp = __frcp_rn(nrm);
     __half* orow = unit_out + r * unit_row_stride;
-#pragma unroll
-    for (int j = 0; j < kLnMaxVecPerLane; ++j) {
-      const int vi = lane + 32 * j;
-      if (vi < nvec) {
-        uint4 w;
-        __half2* h = reinterpret_cast<__half2*>(&w);
-#pragma unroll
-        for (int e = 0; e < 4; ++e)
-          h[e] = __floats2half2_rn(div_by(v[j][2 * e], nrm, rcp), div_by(v[j][2 * e + 1], nrm, rcp));
-        *reinterpret_cast<uint4*>(orow + vi * 8) = w;
-      }
-    }
+    if (div_by_needs_ieee(nrm))
+      write_ln_unit_row<true>(v, lane, nvec, nrm, rcp, orow);
+    else
+      write_ln_unit_row<false>(v, lane, nvec, nrm, rcp, orow);
   }
 }
 

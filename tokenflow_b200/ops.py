@@ -206,8 +206,8 @@ class CudaOps:
             x = x.float()
         dim = x.shape[-1]
         x2 = x.reshape(-1, dim)
-        if x2.stride(-1) != 1:
-            x2 = x2.contiguous()
+        if x2.stride(-1) != 1 or x2.stride(0) % 4 or x2.data_ptr() % 16:
+            x2 = x2.clone(memory_format=torch.contiguous_format)     # rows the kernel's loads cannot address
         out = torch.empty(x2.shape, dtype=torch.float16, device=x.device)
         nbytes = x2.shape[0] * dim * (x2.element_size() + 2)
         self._timed("tf_unit_rows", nbytes, lambda: self._check(
@@ -240,8 +240,8 @@ class CudaOps:
             return self.unit_rows(norm(x))                       # shapes the fused kernel does not cover
         gamma, beta = self._affine_f32(norm, x.device)
         x2 = x.reshape(-1, dim)
-        if x2.stride(-1) != 1 or x2.stride(0) % 8:
-            x2 = x2.contiguous()
+        if x2.stride(-1) != 1 or x2.stride(0) % 8 or x2.data_ptr() % 16:
+            x2 = x2.clone(memory_format=torch.contiguous_format)     # rows the kernel's 16-byte loads cannot address
         out = torch.empty(x2.shape, dtype=torch.float16, device=x.device)
         self._timed("tf_layernorm_unit_rows", x2.shape[0] * dim * 4, lambda: self._check(
             self.lib.tf_layernorm_unit_rows(x2.data_ptr(), x2.shape[0], dim, x2.stride(0), gamma.data_ptr(),
@@ -267,8 +267,8 @@ class CudaOps:
             return y, unit
         gamma, beta = self._affine_f32(norm, x.device)
         x2 = x.reshape(-1, dim)
-        if x2.stride(-1) != 1 or x2.stride(0) % 8:
-            x2 = x2.contiguous()
+        if x2.stride(-1) != 1 or x2.stride(0) % 8 or x2.data_ptr() % 16:
+            x2 = x2.clone(memory_format=torch.contiguous_format)     # rows the kernel's 16-byte loads cannot address
         y = torch.empty((b, S, dim), dtype=torch.float16, device=x.device) if y_out is None else y_out
         unit = None
         if n_unit:
