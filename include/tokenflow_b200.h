@@ -154,21 +154,14 @@ int tf_ddim(const void* eps, const void* x, const float* coef, int64_t n, void* 
  *   gamma, beta  device [c] fp16 (the GroupNorm's weight / bias)
  *   silu         != 0: apply SiLU
  *   workspace    device, >= tf_group_norm_nhwc_workspace(n, hw, c, groups) bytes, 16-byte aligned, uninitialised
- * c % 8 == 0 and groups | c (else TF_ERR_INVALID_ARGUMENT); 8 <= c / groups and c <= 4096 (else unsupported). */
+ * c % 8 == 0 and groups | c (else TF_ERR_INVALID_ARGUMENT); c / groups == 4 or >= 8, and c <= 4096 (else unsupported).
+ * Exactly 4 channels per group is the VAE's 128-channel levels with 32 groups (every 16-byte vector of 8 channels spans
+ * two groups): the same rounding sequence and workspace format, but no bias add, so bias must be NULL there (else
+ * unsupported). */
 int64_t tf_group_norm_nhwc_workspace(int64_t n, int64_t hw, int c, int groups); /* bytes, or -1 for a bad shape */
 int tf_group_norm_nhwc(const void* x, const void* bias, int64_t bias_stride, const void* gamma, const void* beta,
                        int64_t n, int64_t hw, int c, int groups, float eps, int silu, void* workspace,
                        int64_t workspace_bytes, void* out, tf_stream_t stream);
-
-/* The same GroupNorm [+ SiLU] at exactly 4 channels per group and without the bias add: the VAE's 128-channel levels
- * with 32 groups (every 16-byte vector of 8 channels spans two groups).  Same rounding sequence, same determinism,
- * and the same workspace format, [n, groups, stats_chunks] of (sum d, sum d^2) in fp64.
- *   x, out       device [n, hw, c] fp16 dense NHWC;  gamma, beta  device [c] fp16
- *   workspace    device, >= tf_group_norm_nhwc_g4_workspace(n, hw, c, groups) bytes, 16-byte aligned, uninitialised
- * c % 8 == 0 and c == 4 * groups (else TF_ERR_INVALID_ARGUMENT); c <= 4096 (else unsupported). */
-int64_t tf_group_norm_nhwc_g4_workspace(int64_t n, int64_t hw, int c, int groups); /* bytes, or -1 for a bad shape */
-int tf_group_norm_nhwc_g4(const void* x, const void* gamma, const void* beta, int64_t n, int64_t hw, int c, int groups,
-                          float eps, int silu, void* workspace, int64_t workspace_bytes, void* out, tf_stream_t stream);
 
 /* GEGLU gate of the transformer blocks' feed-forward: out = fp16(xh * fp16(gelu(gate))), gelu in ATen's erf form
  * (x/2 * (1 + erff(x / sqrt(2)))), so the result equals the eager `F.linear(x, w_x, b_x) * F.gelu(F.linear(x, w_g,

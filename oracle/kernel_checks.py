@@ -232,14 +232,17 @@ def check_nn_field(idx_a: torch.Tensor, idx_b: Optional[torch.Tensor], x_unit: t
 GN_MAX_THREADS = 512            # tf_body.cu kGnMaxThreads
 GN_STATS_CHUNK_BYTES = 64 << 10  # kGnStatsChunkBytes
 GN_APPLY_CHUNK_BYTES = 128 << 10  # kGnApplyChunkBytes
+GN_G4_APPLY_CHUNKS_PER_SAMPLE = 64  # kGnG4ApplyChunksPerSample
 GN_WS_REL_TOL = 2.0 ** -16       # observed on one H100 80GB HBM3 (400 W): at most 7.6e-8 (Σd) and 2.6e-7 (Σd²) over
                                  # the 222 shapes of tests/test_gpu_body_kernels.py, 4.9e-8 / 6.5e-8 at the real UNet
                                  # sites; a dropped pixel moves a chunk by >= 2^-12
 
 
-def gn_layout(hw: int, c: int) -> dict:
+def gn_layout(hw: int, c: int, groups: Optional[int] = None) -> dict:
     """tf_body.cu `gn_layout`: one thread per 8-channel column, `rows` pixel rows per CTA, and the pixel chunk of a
-    statistics / apply CTA (a multiple of `rows` of about 64 / 128 KB of input)."""
+    statistics / apply CTA (a multiple of `rows` of about 64 / 128 KB of input).  At 4 channels per group
+    (c == 4 * groups) the library takes `gn_layout_g4`: the apply chunk is at least 1/64 of the sample, rounded up to
+    whole CTA rows."""
     cols = c // 8
     rows = max(1, GN_MAX_THREADS // cols)
 
@@ -249,6 +252,9 @@ def gn_layout(hw: int, c: int) -> dict:
         return max(px, rows)
 
     stats_px, apply_px = chunk(GN_STATS_CHUNK_BYTES), chunk(GN_APPLY_CHUNK_BYTES)
+    if groups is not None and c == 4 * groups:
+        px = -(-hw // GN_G4_APPLY_CHUNKS_PER_SAMPLE)
+        apply_px = max(apply_px, -(-px // rows) * rows)
     return {"cols": cols, "rows": rows, "threads": -(-cols * rows // 32) * 32, "stats_px": stats_px,
             "apply_px": apply_px, "stats_chunks": -(-hw // stats_px), "apply_chunks": -(-hw // apply_px)}
 

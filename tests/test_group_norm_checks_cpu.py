@@ -21,13 +21,13 @@ def lib():
 
 
 @pytest.mark.parametrize("c,g", [(8, 1), (64, 1), (72, 8), (80, 8), (256, 32), (320, 32), (2040, 255), (4000, 500),
-                                 (4096, 32), (4096, 512)])
+                                 (4096, 32), (4096, 512), (8, 2), (128, 32), (4096, 1024)])
 def test_gn_layout_matches_the_library_workspace_size(lib, c, g):
-    L0 = gn_layout(1, c)
+    L0 = gn_layout(1, c, g)
     hws = {1, 3, 64, 4096, 9216, L0["rows"], L0["stats_px"] - 1, L0["stats_px"], L0["stats_px"] + 1,
-           L0["apply_px"] + 1, 2 * L0["apply_px"] + L0["rows"] - 1, 7 * L0["stats_px"] + 5}
+           L0["apply_px"] + 1, 2 * L0["apply_px"] + L0["rows"] - 1, 7 * L0["stats_px"] + 5, 64 * L0["apply_px"] + 1}
     for hw in sorted(h for h in hws if h >= 1):
-        L = gn_layout(hw, c)
+        L = gn_layout(hw, c, g)
         assert L["stats_px"] % L["rows"] == 0 and L["apply_px"] % L["rows"] == 0
         assert L["cols"] * L["rows"] <= L["threads"] <= 512
         for n in (1, 3):

@@ -174,25 +174,23 @@ def lib():
     return tf_ops.load_library()
 
 
-def test_g4_and_pixel_entry_points_reject_bad_arguments_without_a_device(lib):
+def test_group_norm_and_pixel_entry_points_reject_bad_arguments_without_a_device(lib):
     buf = (ctypes.c_uint8 * 4096)()
     p = (ctypes.addressof(buf) + 15) & ~15
-    g4 = lambda c, groups, ws=4096, x=p, out=p, n=2, hw=64: lib.tf_group_norm_nhwc_g4(
-        x, p, p, n, hw, c, groups, 1e-6, 1, p, ws, out, None)
-    assert g4(132, 33) == 1 and b"c % 8" in lib.tf_last_error()                  # C % 8 != 0
-    assert g4(128, 16) == 1 and b"c / groups == 4" in lib.tf_last_error()          # 8 channels per group
-    assert g4(128, 64) == 1                                                         # 2 channels per group
-    assert lib.tf_group_norm_nhwc_g4_workspace(2, 64, 128, 16) == -1
-    assert g4(8192, 2048) == 3                                                      # C > 4096
-    need = lib.tf_group_norm_nhwc_g4_workspace(2, 512 * 512, 128, 32)
+    gn = lambda c, groups, ws=4096, x=p, out=p, n=2, hw=64, bias=None: lib.tf_group_norm_nhwc(
+        x, bias, 0, p, p, n, hw, c, groups, 1e-6, 1, p, ws, out, None)
+    assert gn(132, 33) == 1 and b"c % 8" in lib.tf_last_error()                  # C % 8 != 0
+    assert gn(128, 64) == 3 and b"c / groups" in lib.tf_last_error()              # 2 channels per group
+    assert lib.tf_group_norm_nhwc_workspace(2, 64, 128, 64) == -1
+    assert gn(8192, 2048) == 3                                                      # C > 4096
+    assert gn(128, 32, bias=p) == 3 and b"no bias" in lib.tf_last_error()         # no bias add at 4 per group
+    assert lib.tf_group_norm_nhwc_workspace(2, 64, 128, 32) == 2 * 32 * 1 * 16      # 4 channels per group accepted
+    need = lib.tf_group_norm_nhwc_workspace(2, 512 * 512, 128, 32)
     assert need == 2 * 32 * 1024 * 16                                               # [N, G, 64 KB chunks] x 16 B
-    assert g4(128, 32, ws=need - 16, hw=512 * 512) == 1 and b"workspace" in lib.tf_last_error()
-    assert g4(128, 32, x=p + 8) == 1 and b"misaligned" in lib.tf_last_error()
-    assert g4(128, 32, out=p + 2) == 1 and b"misaligned" in lib.tf_last_error()
-    assert g4(128, 32, n=0) == 0 and g4(128, 32, hw=0) == 0                       # empty: no-op
-    # the >= 8-channels-per-group entry point still refuses 4 channels per group
-    assert lib.tf_group_norm_nhwc(p, None, 0, p, p, 2, 64, 128, 32, 1e-6, 1, p, 4096, p, None) == 3
-    assert lib.tf_group_norm_nhwc_workspace(2, 64, 128, 32) == -1
+    assert gn(128, 32, ws=need - 16, hw=512 * 512) == 1 and b"workspace" in lib.tf_last_error()
+    assert gn(128, 32, x=p + 8) == 1 and b"misaligned" in lib.tf_last_error()
+    assert gn(128, 32, out=p + 2) == 1 and b"misaligned" in lib.tf_last_error()
+    assert gn(128, 32, n=0) == 0 and gn(128, 32, hw=0) == 0                       # empty: no-op
     for fn in (lib.tf_frames_to_nhwc, lib.tf_nhwc_to_frames):
         assert fn(p, -1, p, None) == 1
         assert fn(p, 0, None, None) == 0
@@ -208,4 +206,4 @@ def test_norm_act_keeps_aten_off_the_native_shapes():
     x = torch.randn(2, 128, 8, 8)
     assert torch.equal(norm_act(norm, x), torch.nn.functional.silu(norm(x)))
     assert torch.equal(norm_act(norm, x, silu=False), norm(x))
-    assert not tf_ops.CudaOps.group_norm_nhwc_g4_supported(x, norm)
+    assert not tf_ops.CudaOps.group_norm_nhwc_supported(x, norm)

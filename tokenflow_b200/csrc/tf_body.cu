@@ -24,9 +24,9 @@
 // group of unit spread), var = E[d^2] - mean(d)^2 cancels, the fp32 inner sums of d^2 carry that error, and rstd
 // rounds to the other fp16 neighbour more often than ATen's does (tests/test_gpu_body_kernels.py, outlier_shift).
 //
-// tf_group_norm_nhwc_g4 runs the same two kernels at exactly 4 channels per group (the VAE's 128-channel levels with
-// 32 groups), without the bias: a thread's 8-channel column then always spans two groups, the (lo, hi) pair of sums
-// the kernels already carry for columns that straddle a group boundary.  It is compiled for that constant and gets a
+// At exactly 4 channels per group (the VAE's 128-channel levels with 32 groups) tf_group_norm_nhwc runs the same two
+// kernels without the bias: a thread's 8-channel column then always spans two groups, the (lo, hi) pair of sums the
+// kernels already carry for columns that straddle a group boundary.  They are compiled for that constant and get a
 // larger apply chunk (gn_layout_g4).
 //
 // GEGLU.  out = fp16(float(xh) * float(fp16(gelu_erf(float(g))))) — the eager `F.linear(..) * F.gelu(F.linear(..))`
@@ -314,8 +314,8 @@ long long group_norm_nhwc_workspace(long long n, long long hw, int c, int groups
 
 namespace {
 
-// Both entry points: the same two kernels, the statistics layout of gn_layout (so the workspace has one format), and
-// an apply layout of the caller's choice.  kCpg = 4 has no bias path (no 4-channel-group site adds one).
+// Both channels-per-group cases: the same two kernels, the statistics layout of gn_layout (so the workspace has one
+// format), and an apply layout of the caller's choice.  kCpg = 4 has no bias path (no 4-channel-group site adds one).
 template <int kCpg>
 int launch_gn(const GnLayout& L, const __half* xp, const __half* bp, long long bias_stride, const __half* gp,
               const __half* btp, long long n, long long hw, int c, int groups, float eps, int silu, double2* ws,
@@ -360,18 +360,17 @@ int launch_gn(const GnLayout& L, const __half* xp, const __half* bp, long long b
 int launch_group_norm_nhwc(const void* x, const void* bias, long long bias_stride, const void* gamma, const void* beta,
                            long long n, long long hw, int c, int groups, float eps, int silu, void* workspace,
                            void* out, cudaStream_t stream) {
-  return launch_gn<0>(gn_layout(hw, c), static_cast<const __half*>(x), static_cast<const __half*>(bias), bias_stride,
-                      static_cast<const __half*>(gamma), static_cast<const __half*>(beta), n, hw, c, groups, eps, silu,
-                      static_cast<double2*>(workspace), static_cast<__half*>(out), stream,
-                      "tf_group_norm_nhwc statistics launch", "tf_group_norm_nhwc apply launch");
-}
-
-int launch_group_norm_nhwc_g4(const void* x, const void* gamma, const void* beta, long long n, long long hw, int c,
-                              float eps, int silu, void* workspace, void* out, cudaStream_t stream) {
-  return launch_gn<4>(gn_layout_g4(hw, c), static_cast<const __half*>(x), nullptr, 0, static_cast<const __half*>(gamma),
-                      static_cast<const __half*>(beta), n, hw, c, c / 4, eps, silu, static_cast<double2*>(workspace),
-                      static_cast<__half*>(out), stream, "tf_group_norm_nhwc_g4 statistics launch",
-                      "tf_group_norm_nhwc_g4 apply launch");
+  const __half* xp = static_cast<const __half*>(x);
+  const __half* gp = static_cast<const __half*>(gamma);
+  const __half* btp = static_cast<const __half*>(beta);
+  double2* ws = static_cast<double2*>(workspace);
+  __half* op = static_cast<__half*>(out);
+  if (c == 4 * groups)       // no bias here: tf_group_norm_nhwc refuses one at 4 channels per group
+    return launch_gn<4>(gn_layout_g4(hw, c), xp, nullptr, 0, gp, btp, n, hw, c, groups, eps, silu, ws, op, stream,
+                        "tf_group_norm_nhwc statistics launch", "tf_group_norm_nhwc apply launch");
+  return launch_gn<0>(gn_layout(hw, c), xp, static_cast<const __half*>(bias), bias_stride, gp, btp, n, hw, c, groups,
+                      eps, silu, ws, op, stream, "tf_group_norm_nhwc statistics launch",
+                      "tf_group_norm_nhwc apply launch");
 }
 
 int launch_geglu(const void* xh, const void* gate, long long n, void* out, cudaStream_t stream) {

@@ -96,22 +96,9 @@ static int check_group_norm_shape(int64_t n, int64_t hw, int c, int groups) {
                    (long long)n, (long long)hw, c, groups);
     return TF_ERR_INVALID_ARGUMENT;
   }
-  if (c / groups < 8 || c > kGnMaxChannels) {
-    set_last_error("tf_group_norm_nhwc: c=%d groups=%d not supported (8 <= c / groups, c <= %d)", c, groups,
+  if ((c / groups != 4 && c / groups < 8) || c > kGnMaxChannels) {
+    set_last_error("tf_group_norm_nhwc: c=%d groups=%d not supported (c / groups == 4 or >= 8, c <= %d)", c, groups,
                    kGnMaxChannels);
-    return TF_ERR_UNSUPPORTED;
-  }
-  return TF_OK;
-}
-
-static int check_group_norm_g4_shape(int64_t n, int64_t hw, int c, int groups) {
-  if (n < 0 || hw < 0 || c <= 0 || (c & 7) || groups <= 0 || c != 4 * groups) {
-    set_last_error("tf_group_norm_nhwc_g4: bad shape n=%lld hw=%lld c=%d groups=%d (c %% 8 == 0 and c / groups == 4 "
-                   "required)", (long long)n, (long long)hw, c, groups);
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  if (c > kGnMaxChannels) {
-    set_last_error("tf_group_norm_nhwc_g4: c=%d not supported (c <= %d)", c, kGnMaxChannels);
     return TF_ERR_UNSUPPORTED;
   }
   return TF_OK;
@@ -223,6 +210,10 @@ int tf_group_norm_nhwc(const void* x, const void* bias, int64_t bias_stride, con
                        int64_t n, int64_t hw, int c, int groups, float eps, int silu, void* workspace,
                        int64_t workspace_bytes, void* out, tf_stream_t stream) {
   if (int e = check_group_norm_shape(n, hw, c, groups)) return e;
+  if (bias && c == 4 * groups) {
+    set_last_error("tf_group_norm_nhwc: c=%d groups=%d: no bias add at 4 channels per group", c, groups);
+    return TF_ERR_UNSUPPORTED;
+  }
   if (bias && (bias_stride < 0 || (bias_stride & 7) || (bias_stride > 0 && bias_stride < c))) {
     set_last_error("tf_group_norm_nhwc: bias row stride %lld (0, or >= c and a multiple of 8)", (long long)bias_stride);
     return TF_ERR_INVALID_ARGUMENT;
@@ -240,30 +231,6 @@ int tf_group_norm_nhwc(const void* x, const void* bias, int64_t bias_stride, con
   }
   int e = launch_group_norm_nhwc(x, bias, bias_stride, gamma, beta, n, hw, c, groups, eps, silu, workspace, out,
                                  static_cast<cudaStream_t>(stream));
-  if (!e) g_launches += 2 * ((n + 65534) / 65535);
-  return e;
-}
-
-int64_t tf_group_norm_nhwc_g4_workspace(int64_t n, int64_t hw, int c, int groups) {
-  if (check_group_norm_g4_shape(n, hw, c, groups)) return -1;
-  return (int64_t)group_norm_nhwc_workspace(n, hw, c, groups);
-}
-
-int tf_group_norm_nhwc_g4(const void* x, const void* gamma, const void* beta, int64_t n, int64_t hw, int c, int groups,
-                          float eps, int silu, void* workspace, int64_t workspace_bytes, void* out, tf_stream_t stream) {
-  if (int e = check_group_norm_g4_shape(n, hw, c, groups)) return e;
-  if (n == 0 || hw == 0) return TF_OK;
-  const long long need = group_norm_nhwc_workspace(n, hw, c, groups);
-  if (workspace_bytes < need) {
-    set_last_error("tf_group_norm_nhwc_g4: workspace of %lld bytes, %lld needed", (long long)workspace_bytes, need);
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  if (!x || !gamma || !beta || !workspace || !out || !aligned16(x) || !aligned16(out) || !aligned16(workspace)) {
-    set_last_error("tf_group_norm_nhwc_g4: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  int e = launch_group_norm_nhwc_g4(x, gamma, beta, n, hw, c, eps, silu, workspace, out,
-                                    static_cast<cudaStream_t>(stream));
   if (!e) g_launches += 2 * ((n + 65534) / 65535);
   return e;
 }

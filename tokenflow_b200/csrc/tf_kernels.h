@@ -30,15 +30,12 @@ int launch_cfg_ddim(const void* eps_uncond, const void* eps_cond, const void* x,
                     long long n, void* out, cudaStream_t stream);
 int launch_ddim(const void* eps, const void* x, const float* coef_dev, long long n, void* out, cudaStream_t stream);
 
-// Channels-last GroupNorm (tf_body.cu): 8 <= C / groups, C % 8 == 0, C <= kGnMaxChannels.
+// Channels-last GroupNorm (tf_body.cu): C / groups == 4 (no bias) or >= 8, C % 8 == 0, C <= kGnMaxChannels.
 constexpr int kGnMaxChannels = 4096;
 long long group_norm_nhwc_workspace(long long n, long long hw, int c, int groups);
 int launch_group_norm_nhwc(const void* x, const void* bias, long long bias_stride, const void* gamma, const void* beta,
                            long long n, long long hw, int c, int groups, float eps, int silu, void* workspace,
                            void* out, cudaStream_t stream);
-// The same kernels at exactly 4 channels per group, no bias (the VAE's 128-channel levels).
-int launch_group_norm_nhwc_g4(const void* x, const void* gamma, const void* beta, long long n, long long hw, int c,
-                              float eps, int silu, void* workspace, void* out, cudaStream_t stream);
 int launch_geglu(const void* xh, const void* gate, long long n, void* out, cudaStream_t stream);
 
 // Pixel conversions around the VAE (tf_pixels.cu); n = elements (pixels x 3).

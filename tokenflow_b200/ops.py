@@ -66,10 +66,6 @@ _SIGNATURES = {
                                           ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int,
                                           ctypes.c_float, ctypes.c_int, ctypes.c_void_p, ctypes.c_int64,
                                           ctypes.c_void_p, ctypes.c_void_p]),
-    "tf_group_norm_nhwc_g4_workspace": (ctypes.c_int64, [ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int]),
-    "tf_group_norm_nhwc_g4": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64,
-                                             ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_int,
-                                             ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
     "tf_frames_to_nhwc": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
     "tf_nhwc_to_frames": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
     "tf_geglu": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
@@ -416,33 +412,30 @@ class CudaOps:
 
     # -- UNet body ----------------------------------------------------------------------------
     @staticmethod
-    def _group_norm_nhwc_operands(x: torch.Tensor, norm: torch.nn.GroupNorm) -> bool:
-        """CUDA fp16 channels_last [N, C, H, W] with C % 8 == 0, C <= 4096, groups dividing C and fp16 affine
-        parameters: what both GroupNorm entry points need besides their channels per group."""
+    def group_norm_nhwc_supported(x: torch.Tensor, norm: torch.nn.GroupNorm,
+                                  bias: Optional[torch.Tensor] = None) -> bool:
+        """Operands tf_group_norm_nhwc covers: CUDA fp16 channels_last [N, C, H, W] with C % 8 == 0, C <= 4096, groups
+        dividing C, fp16 affine parameters, and either at least 8 channels per group with an fp16 or no bias, or
+        exactly 4 channels per group without a bias."""
         if not (x.is_cuda and x.dtype == torch.float16 and x.dim() == 4
                 and x.is_contiguous(memory_format=torch.channels_last)):
             return False
         c, g = x.shape[1], norm.num_groups
         w, b = norm.weight, norm.bias
-        return (c % 8 == 0 and c <= 4096 and c % g == 0 and w is not None and b is not None
-                and w.dtype == b.dtype == torch.float16 and w.is_contiguous() and b.is_contiguous())
-
-    @staticmethod
-    def group_norm_nhwc_supported(x: torch.Tensor, norm: torch.nn.GroupNorm) -> bool:
-        """Shapes tf_group_norm_nhwc covers: CUDA fp16 channels_last [N, C, H, W] with C % 8 == 0, C <= 4096, at least
-        8 channels per group and fp16 affine parameters."""
-        return CudaOps._group_norm_nhwc_operands(x, norm) and x.shape[1] // norm.num_groups >= 8
-
-    @staticmethod
-    def group_norm_nhwc_g4_supported(x: torch.Tensor, norm: torch.nn.GroupNorm) -> bool:
-        """Shapes tf_group_norm_nhwc_g4 covers: the same operands with exactly 4 channels per group."""
-        return CudaOps._group_norm_nhwc_operands(x, norm) and x.shape[1] == 4 * norm.num_groups
+        if not (c % 8 == 0 and c <= 4096 and c % g == 0 and w is not None and b is not None
+                and w.dtype == b.dtype == torch.float16 and w.is_contiguous() and b.is_contiguous()):
+            return False
+        if c == 4 * g:
+            return bias is None
+        return c // g >= 8 and (bias is None or bias.dtype == torch.float16)
 
     def group_norm_nhwc(self, x: torch.Tensor, norm: torch.nn.GroupNorm, bias: Optional[torch.Tensor] = None,
                         silu: bool = False) -> torch.Tensor:
         """[SiLU](GroupNorm(x [+ bias[:, :, None, None]])) of a channels_last fp16 [N, C, H, W] tensor, channels_last
         out, with the eager fp16 rounding sequence.  `bias` is fp16 [N, C] or [1, C] (the resnet's time-embedding
-        projection).  Two launches; the statistics workspace comes from the caching allocator on this stream."""
+        projection), and None at 4 channels per group.  Two launches, timed as "tf_group_norm_g4" at 4 channels per
+        group (the VAE's 128-channel levels) and "tf_group_norm" otherwise; the statistics workspace comes from the
+        caching allocator on this stream."""
         n, c, h, w = x.shape
         if bias is not None:
             assert bias.dtype == torch.float16 and bias.dim() == 2 and bias.shape[1] == c and bias.shape[0] in (1, n)
@@ -455,25 +448,11 @@ class CudaOps:
         ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=x.device)
         out = torch.empty_like(x, memory_format=torch.channels_last)
         work = 3.0 * x.numel() * 2 + (n * c * 2 if bias is not None else 0)
-        self._timed("tf_group_norm", work, lambda: self._check(self.lib.tf_group_norm_nhwc(
+        name = "tf_group_norm_g4" if c == 4 * norm.num_groups else "tf_group_norm"
+        self._timed(name, work, lambda: self._check(self.lib.tf_group_norm_nhwc(
             x.data_ptr(), bias.data_ptr() if bias is not None else None, bias_stride if bias is not None else 0,
             norm.weight.data_ptr(), norm.bias.data_ptr(), n, h * w, c, norm.num_groups, float(norm.eps), int(bool(silu)),
             ws.data_ptr(), ws.numel(), out.data_ptr(), self._stream()), "tf_group_norm_nhwc"))
-        return out
-
-    def group_norm_nhwc_g4(self, x: torch.Tensor, norm: torch.nn.GroupNorm, silu: bool = False) -> torch.Tensor:
-        """[SiLU](GroupNorm(x)) of a channels_last fp16 [N, C, H, W] tensor with 4 channels per group (no bias add),
-        channels_last out, with the eager fp16 rounding sequence; the statistics workspace comes from the caching
-        allocator on this stream."""
-        n, c, h, w = x.shape
-        ws_bytes = int(self.lib.tf_group_norm_nhwc_g4_workspace(n, h * w, c, norm.num_groups))
-        if ws_bytes < 0:
-            self._check(1, "tf_group_norm_nhwc_g4_workspace")
-        ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=x.device)
-        out = torch.empty_like(x, memory_format=torch.channels_last)
-        self._timed("tf_group_norm_g4", 3.0 * x.numel() * 2, lambda: self._check(self.lib.tf_group_norm_nhwc_g4(
-            x.data_ptr(), norm.weight.data_ptr(), norm.bias.data_ptr(), n, h * w, c, norm.num_groups, float(norm.eps),
-            int(bool(silu)), ws.data_ptr(), ws.numel(), out.data_ptr(), self._stream()), "tf_group_norm_nhwc_g4"))
         return out
 
     def frames_to_nhwc(self, frames: torch.Tensor) -> torch.Tensor:

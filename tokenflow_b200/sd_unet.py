@@ -76,17 +76,14 @@ class GroupNorm(nn.GroupNorm):
 def norm_act(norm: nn.GroupNorm, x: torch.Tensor, bias: Optional[torch.Tensor] = None,
              silu: bool = True) -> torch.Tensor:
     """[SiLU](norm(x [+ bias[:, :, None, None]])): one tf_group_norm_nhwc call (two launches, three passes over x)
-    for CUDA fp16 channels_last input, tf_group_norm_nhwc_g4 for 4 channels per group without a bias (the VAE's
-    128-channel levels), else the eager ATen sequence (fp16 add, GroupNorm, SiLU)."""
+    for the operands `CudaOps.group_norm_nhwc_supported` accepts (CUDA fp16 channels_last, at least 8 channels per
+    group, or 4 without a bias: the VAE's 128-channel levels), else the eager ATen sequence (fp16 add, GroupNorm,
+    SiLU)."""
     from .ops import CudaOps, body_ops
-    if CudaOps.group_norm_nhwc_supported(x, norm) and (bias is None or bias.dtype == torch.float16):
+    if CudaOps.group_norm_nhwc_supported(x, norm, bias):
         ops = body_ops()
         if ops is not None:
             return ops.group_norm_nhwc(x, norm, bias, silu)
-    elif bias is None and CudaOps.group_norm_nhwc_g4_supported(x, norm):
-        ops = body_ops()
-        if ops is not None:
-            return ops.group_norm_nhwc_g4(x, norm, silu)
     if bias is not None:
         x = x + bias[:, :, None, None]
     x = norm(x)

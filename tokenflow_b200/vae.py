@@ -14,9 +14,8 @@ SD's VAE: block_out_channels (128, 256, 512, 512), 2 resnets per encoder block (
 channels, 32 groups, eps 1e-6, one single-head attention in each mid block.  `tiny_config()` keeps the topology at toy
 width for CPU tests (8 groups, so its first level has 4 channels per group like SD's).
 
-Every GroupNorm(+SiLU) goes through `sd_unet.norm_act`: on CUDA fp16 channels_last tensors the 128-channel levels (4
-channels per group) run tf_group_norm_nhwc_g4, the 256- and 512-channel levels tf_group_norm_nhwc; CPU, NCHW and fp32
-runs keep ATen.  Convolutions are cuDNN, and the mid-block attention (head dim 512, S = 4096 at 512^2) is SDPA.
+Every GroupNorm(+SiLU) goes through `sd_unet.norm_act`: on CUDA fp16 channels_last tensors every level runs
+tf_group_norm_nhwc, the 128-channel levels at 4 channels per group; CPU, NCHW and fp32 runs keep ATen.  Convolutions are cuDNN, and the mid-block attention (head dim 512, S = 4096 at 512^2) is SDPA.
 """
 from __future__ import annotations
 

@@ -4,14 +4,15 @@ alternated over rounds.
     python tools/vae_bench.py [--configs C2,C4] [--frames 40] [--batch 10] [--rounds 3] [--out FILE]
 
 C2 is SD1.5's 512^2 frames, C4 SD2.1's 768^2 (the VAE is the same).  Arms:
-  native   fp16 channels_last; GroupNorm(+SiLU) on tf_group_norm_nhwc_g4 / tf_group_norm_nhwc, pixels on
+  native   fp16 channels_last; GroupNorm(+SiLU) on tf_group_norm_nhwc, pixels on
            tf_frames_to_nhwc / tf_nhwc_to_frames (`preprocess.encode_imgs` / `decode_latents`)
   aten_cl  the same model and calls with ATen's GroupNorm (NCHW-only: it copies around every norm)
   nchw     the same weights in NCHW, ATen's GroupNorm
 Per config it prints the median ms per frame of encode (uint8 frames on the host -> latents) and decode (latents ->
 uint8 frames on the device) per arm, kernel time per category of one profiled encode + decode per arm (the categories
 of tools/prof_body.py; the `sdpa` entry names the attention backend that ran), the algorithmic bytes per second of
-tf_group_norm_g4 (3 passes of 2 bytes an element over CUDA-event time of each call), and the card's name, power limit
+the 4-channels-per-group tf_group_norm_nhwc calls, timed as tf_group_norm_g4 (3 passes of 2 bytes an element over
+CUDA-event time of each call), and the card's name, power limit
 and SM clock read by nvidia-smi before and after the measurement.
 """
 from __future__ import annotations
