@@ -2,16 +2,20 @@
 
 A plain-torch restatement of tf_ext_attn's arithmetic (128- or 64-key tiles per slab, zero-filled
 padding keys masked, online softmax with fp16 P and an fp32 normaliser, fp16 output) must pass
-`check_ext_attn`; the same computation with one deliberate mistake each must fail it.  Likewise for
-`check_nn_field` and the NN field's padding guard and first-index rule.  Everything here is CPU torch:
-no wrong computation is compiled into the library or run on a GPU."""
+`check_ext_attn`; the same computation with one deliberate mistake each must fail it.  At 204 800 keys
+(1 600 tiles) a thread-by-thread restatement of the normaliser shows that the kernel's earlier arithmetic
+(P <= 1, one fp32 addition per key) fails the error model on a subnormal-tail probe, that the current one
+(P <= 2^8, one addition per tile) meets it on every probe, and that one dropped or stale tile out of 1 600 is
+rejected.  Likewise for `check_nn_field` and the NN field's padding guard and first-index rule.  Everything
+here is CPU torch: no wrong computation is compiled into the library or run on a GPU."""
 import math
 
 import pytest
 import torch
 
-from oracle.kernel_checks import (check_ext_attn, check_nn_field, ext_attn_samples, logit_shift_probe,
-                                  negative_similarity_probe, nn_similarity)
+from oracle.kernel_checks import (ATTN_P_OFFSET, TAIL_BANDS, attn_block_n, check_ext_attn, check_nn_field,
+                                  ext_attn_samples, late_jump_probe, logit_shift_probe, negative_similarity_probe,
+                                  nn_similarity, staircase_probe, subnormal_tail_probe)
 
 
 def _flash(q, k, v, table, heads, scale, row0=0, nrows=None, *, leak_pad=False, drop_last_key=False,
@@ -219,3 +223,131 @@ def test_check_nn_field_rejects_a_wrong_index_outside_the_tie_class():
     idx_a[0, 5] = (idx_a[0, 5] + 1) % 64
     with pytest.raises(AssertionError):
         check_nn_field(idx_a, None, xu, pu, [0], [-1])
+
+
+# ------------------------------------------------------------------------------------------------
+# long rows: the kernel's per-thread arithmetic at 204 800 keys (1 600 tiles)
+# ------------------------------------------------------------------------------------------------
+def _per_thread(q, k, v, scale, nrows, *, p_offset=ATTN_P_OFFSET, tile_local=True, drop_tile=None, stale_tile=None):
+    """tf_ext_attn's arithmetic for the table [(0, 0, 0, KV)], one head, query rows [0, nrows), thread by thread.
+
+    `_flash` sums each tile in one torch sum; here the normaliser is what the kernel adds: 4 threads share a row,
+    thread t owning columns 8j + 2t and 8j + 2t + 1 of every tile; each adds its pair sums p0 + p1 in fp32 either
+    into a fresh per-tile partial that then goes into its l (`tile_local`, the kernel's arithmetic) or straight
+    into l (the earlier kernel, with `p_offset=0`); the final shuffles add (l0 + l1) + (l2 + l3).  Scores,
+    m, corr and P are fp32 (exp2 flushing results below 2^-126 to zero, as ex2.approx.ftz does), P is rounded
+    to fp16 with P <= 2^p_offset, the P V accumulation is fp64, the output fp16(fp32(O) * fp32(1 / l)).
+    `drop_tile` skips one tile; `stale_tile` reads the previous tile's keys and values in its place."""
+    KV, S, d = k.shape
+    block_n = attn_block_n(d)
+    tps = -(-S // block_n)
+    sl2 = torch.tensor(scale * math.log2(math.e), dtype=torch.float32)
+    qq = q[0, :nrows].float()
+    m = torch.full((nrows, 1), -math.inf)
+    l = torch.zeros(nrows, 4)
+    o = torch.zeros(nrows, d, dtype=torch.float64)
+    tiny = 2.0 ** -126
+    for t in range(KV * tps):
+        if t == drop_tile:
+            continue
+        slab, n0 = divmod(t - 1 if t == stale_tile else t, tps)
+        n0 *= block_n
+        valid = min(block_n, S - n0)
+        kt, vt = torch.zeros(block_n, d), torch.zeros(block_n, d)
+        kt[:valid], vt[:valid] = k[slab, n0:n0 + valid].float(), v[slab, n0:n0 + valid].float()
+        s = qq @ kt.T
+        s[:, valid:] = -math.inf
+        m_new = torch.maximum(m, s.amax(dim=-1, keepdim=True) * sl2)
+        corr = torch.exp2(m - m_new)
+        corr[corr < tiny] = 0.0
+        m = m_new
+        l = l * corr
+        mneg = p_offset - m_new
+        p = (s.double() * sl2.double() + mneg.double()).float().exp2()      # fmaf: one rounding
+        p[p < tiny] = 0.0
+        pairs = p.view(nrows, block_n // 8, 4, 2)
+        pairs = pairs[..., 0] + pairs[..., 1]
+        if tile_local:
+            part = pairs[:, 0]
+            for j in range(1, block_n // 8):
+                part = part + pairs[:, j]
+            l = l + part
+        else:
+            for j in range(block_n // 8):
+                l = l + pairs[:, j]
+        o = o * corr.double() + p.half().double() @ vt.double()
+    lsum = (l[:, 0] + l[:, 1]) + (l[:, 2] + l[:, 3])
+    return (o.float() * (1.0 / lsum)[:, None]).half().unsqueeze(0)
+
+
+LONG_S, LONG_KV, LONG_D, LONG_ROWS = 4096, 50, 40, 8          # C5 stride 4: 204 800 keys per row, 1 600 tiles
+
+
+def _long_inputs(seed, video=True):
+    g = torch.Generator().manual_seed(seed)
+    q = torch.randn(1, LONG_S, LONG_D, generator=g)
+    k = torch.randn(LONG_KV, LONG_S, LONG_D, generator=g) + (1.5 * q if video else 0)
+    v = torch.randn(LONG_KV, LONG_S, LONG_D, generator=g)
+    return q.half(), k.half(), v.half(), LONG_D ** -0.5, g
+
+
+def _check_long(got, q, k, v, scale):
+    return check_ext_attn(got, q, k, v, [(0, 0, 0, LONG_KV)], 1, scale, 0, LONG_ROWS, row_chunk=LONG_ROWS)
+
+
+@pytest.mark.parametrize("band", [(-25.5, -25.0), (-25.0, -24.0)])
+def test_earlier_normaliser_fails_the_error_model_on_the_subnormal_tail(band):
+    """P <= 1 and one fp32 addition per key: the thread holding the maximum drops every tail key from l while the
+    numerator rounds them to 0 or 2^-24.  At 204 800 keys that is several 1e-3 of the output."""
+    q, k, v, scale, g = _long_inputs(1)
+    offsets = subnormal_tail_probe(q, k, v, 1, scale, band, "first", generator=g)
+    assert band[0] < offsets[0, 1:].min().item() and offsets[0, 1:].max().item() < band[1]
+    got = _per_thread(q, k, v, scale, LONG_ROWS, p_offset=0, tile_local=False)
+    err = (got.double() - v[0, 0].double()).abs().max().item()
+    assert err > 2e-3, err
+    with pytest.raises(AssertionError, match="outside the fp16 error model"):
+        _check_long(got, q, k, v, scale)
+    # the offset alone or the tile partial alone does not repair it
+    for p_offset, tile_local in ((ATTN_P_OFFSET, False), (0, True)):
+        with pytest.raises(AssertionError):
+            _check_long(_per_thread(q, k, v, scale, LONG_ROWS, p_offset=p_offset, tile_local=tile_local),
+                        q, k, v, scale)
+
+
+@pytest.mark.parametrize("where", ["first", "last"])
+@pytest.mark.parametrize("band", TAIL_BANDS)
+def test_kernel_normaliser_meets_the_error_model_on_the_subnormal_tail(band, where):
+    q, k, v, scale, g = _long_inputs(2)
+    subnormal_tail_probe(q, k, v, 1, scale, band, where, generator=g)
+    got = _per_thread(q, k, v, scale, LONG_ROWS)
+    stats = _check_long(got, q, k, v, scale)
+    assert stats["max_err_scaled"] < 1e-3 and stats["bound_use"] < 0.3, stats
+
+
+@pytest.mark.parametrize("probe", ["video", "staircase_0.0625", "staircase_1", "late_jump"])
+def test_kernel_normaliser_meets_the_error_model_at_1600_tiles(probe):
+    q, k, v, scale, g = _long_inputs(3)
+    if probe.startswith("staircase"):
+        staircase_probe(q, k, 1, scale, float(probe.split("_")[1]), generator=g)
+    elif probe == "late_jump":
+        offsets = late_jump_probe(q, k, 1, scale, generator=g)
+        assert offsets[0, :-128].max().item() < -126
+    stats = _check_long(_per_thread(q, k, v, scale, LONG_ROWS), q, k, v, scale)
+    assert stats["max_err_scaled"] < 1e-3, stats
+
+
+@pytest.mark.parametrize("mutant,probe", [("drop_tile", "video"), ("stale_tile", "video"),
+                                          ("drop_last_tile", "late_jump"), ("stale_tile", "staircase_1")])
+def test_check_ext_attn_rejects_one_wrong_tile_out_of_1600(mutant, probe):
+    """One tile dropped or read stale (the previous tile's keys and values) out of 1 600: tile 800 is the first
+    tile of slab 25, which holds the key correlated with query rows 0..7 (video-like inputs)."""
+    q, k, v, scale, g = _long_inputs(4)
+    if probe == "late_jump":
+        late_jump_probe(q, k, 1, scale, generator=g)
+    elif probe == "staircase_1":
+        staircase_probe(q, k, 1, scale, 1.0, generator=g)
+    T = LONG_KV * LONG_S // 128
+    kw = {"drop_tile": dict(drop_tile=800), "stale_tile": dict(stale_tile=T - 1 if probe != "video" else 800),
+          "drop_last_tile": dict(drop_tile=T - 1)}[mutant]
+    with pytest.raises(AssertionError):
+        _check_long(_per_thread(q, k, v, scale, LONG_ROWS, **kw), q, k, v, scale)

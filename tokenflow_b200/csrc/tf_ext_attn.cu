@@ -15,8 +15,20 @@
 //
 // CTA = 2 warpgroups, 64 query rows each (FlashAttention-2 online softmax, fp32 statistics):
 //   S = Q K_t^T      wgmma, both operands from shared memory (K-major, 128-byte swizzle)
-//   P = exp2(S * scale*log2e - m)   in registers, rounded to fp16 into the wgmma A-fragment layout
-//   O += P V_t       wgmma, P from registers, V from shared memory (MN-major)
+//   P = exp2(S * scale*log2e - m + 8)   in registers, rounded to fp16 into the wgmma A-fragment layout
+//   O = O*corr + P V_t   wgmma, P from registers, V from shared memory (MN-major), into a fresh accumulator
+//                    that is added to O with one fp32 FMA per tile
+//   l += sum_t(P)    fp32: each thread sums its columns of the tile into a fresh partial, then adds it to l
+//
+// Rounding: P is at most 2^8, so fp16 P is relative to 2^-11 down to 2^-22 of the row maximum and below that
+// absolute to 2^-33 of it (fp16 subnormals; the offset keeps that far below the relative term even over
+// 204 800 keys).  Both running sums, O and l, take one rounding per tile, not one per key: a running sum near
+// the row maximum would otherwise swamp every key below about 2^-24 of it.  The tensor core's fp32
+// accumulation drops such products from O, and l summed key by key dropped them on its own terms, so the two
+// disagreed by up to N * 2^-25 of the row mass: on an H100 (700 W), at 204 800 keys whose tail sits 2^-25
+// below a maximum in the first tile, the output was 0.4 % off with both sums taken key by key and 0.5 % off
+// with only l taken per tile.  The fresh accumulator costs kO registers per value tensor: the paired kernels
+// at d = 40 and 64 reach 255 registers and spill 24-28 bytes, and run 2-3.5 % slower than with O += P V_t.
 // Thread 0 also issues the TMA loads: the Q tile once, then a ring of {K tile, V tile} stages; a
 // stage is refilled one tile after both warpgroups released it, so neither waits on the other.
 // The two warpgroups' softmax and MMA phases interleave on the SM.
@@ -44,6 +56,7 @@ namespace {
 constexpr int kBlockM = 128;
 constexpr int kMaxStages = 8;
 constexpr int kSmemBudget = 227 * 1024;
+constexpr float kPOffset = 8.f;   // log2 of the largest P: moves the fp16 subnormal range 8 octaves further down
 
 struct AttnCtl {
   uint64_t q_full;
@@ -209,42 +222,47 @@ ext_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
       const float m_new = fmaxf(m_r[r], mx[r] * sl2);
       corr[r] = fast_exp2(m_r[r] - m_new);
       m_r[r] = m_new;
-      mneg[r] = -m_new;
+      mneg[r] = kPOffset - m_new;
       l_r[r] *= corr[r];
     }
     uint32_t pa[kBlockN / 16][4];
+    float lt[2] = {0.f, 0.f};                                     // this tile's share of l
 #pragma unroll
     for (int j = 0; j < kBlockN / 8; ++j) {
       const float p0 = fast_exp2(fmaf(s[4 * j], sl2, mneg[0]));
       const float p1 = fast_exp2(fmaf(s[4 * j + 1], sl2, mneg[0]));
       const float p2 = fast_exp2(fmaf(s[4 * j + 2], sl2, mneg[1]));
       const float p3 = fast_exp2(fmaf(s[4 * j + 3], sl2, mneg[1]));
-      l_r[0] += p0 + p1;
-      l_r[1] += p2 + p3;
+      lt[0] += p0 + p1;
+      lt[1] += p2 + p3;
       pa[j >> 1][(j & 1) * 2 + 0] = pack_f16x2_rn(p0, p1);
       pa[j >> 1][(j & 1) * 2 + 1] = pack_f16x2_rn(p2, p3);
     }
-#pragma unroll
-    for (int v = 0; v < kNV; ++v)
-#pragma unroll
-      for (int j = 0; j < kO / 4; ++j) {
-        o[v][4 * j] *= corr[0]; o[v][4 * j + 1] *= corr[0];
-        o[v][4 * j + 2] *= corr[1]; o[v][4 * j + 3] *= corr[1];
-      }
+    l_r[0] += lt[0];
+    l_r[1] += lt[1];
 
-    // ---- O += P V ----
-#pragma unroll
-    for (int v = 0; v < kNV; ++v) reg_fence(o[v]);
+    // ---- O = O * corr + P V_t (the tile's product in a fresh accumulator, added with one rounding) ----
+    float ot[kNV][kO];
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < kBlockN / 16; ++kk)
 #pragma unroll
       for (int v = 0; v < kNV; ++v)
-        wgmma_rs<kNPV>(o[v], pa[kk], wgmma_desc(k_addr + (1 + v) * kTileBytes + kk * 16 * 128, kKVChunkBytes, 1024), 1u);
+        wgmma_rs<kNPV>(ot[v], pa[kk], wgmma_desc(k_addr + (1 + v) * kTileBytes + kk * 16 * 128, kKVChunkBytes, 1024),
+                       kk > 0 ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<0>();
 #pragma unroll
-    for (int v = 0; v < kNV; ++v) reg_fence(o[v]);
+    for (int v = 0; v < kNV; ++v) {
+      reg_fence(ot[v]);
+#pragma unroll
+      for (int j = 0; j < kO / 4; ++j) {
+        o[v][4 * j] = fmaf(o[v][4 * j], corr[0], ot[v][4 * j]);
+        o[v][4 * j + 1] = fmaf(o[v][4 * j + 1], corr[0], ot[v][4 * j + 1]);
+        o[v][4 * j + 2] = fmaf(o[v][4 * j + 2], corr[1], ot[v][4 * j + 2]);
+        o[v][4 * j + 3] = fmaf(o[v][4 * j + 3], corr[1], ot[v][4 * j + 3]);
+      }
+    }
 
     __syncwarp();
     if (lane == 0) mbar_arrive(&ctl->empty[st]);
