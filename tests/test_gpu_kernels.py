@@ -312,12 +312,13 @@ def test_ext_attn_other_configs(ops, n, S, heads, d):
         check_ext_attn(got, q, k, v, ext_attn_samples(n, inject), heads, d ** -0.5, rtol=1.5e-3)
 
 
-def test_ext_attn_table_matches_whole_pass(ops):
-    """The sharded-pass entry point (per-sample q/k/v slab table) reproduces the whole-pass result
-    rank by rank — the arithmetic behind tests/test_sharded_cpu.py, on the CUDA kernel."""
+def test_ext_attn_row_split_matches_whole_pass(ops):
+    """The sharded pass's attention: every rank evaluates the global sample table for its query rows
+    (`PivotalShard.row_split`) on the gathered, padded q/k/v; the ranks' rows stacked reproduce the whole-pass
+    result bit for bit (same kernels, same 128-row tiles; injected uncond / cond pairs stay paired)."""
     from tokenflow_b200.tokenflow_utils import PivotalShard
     torch.manual_seed(5)
-    K, S, heads, d = 5, 320, 2, 40
+    K, S, heads, d = 5, 1088, 2, 40          # 8.5 row tiles: at G = 8 four ranks hold two, one a half tile, three none
     dim = heads * d
     q, k, v = (torch.randn(3 * K, S, dim, device="cuda").half() for _ in range(3))
     for inject in (False, True):
@@ -326,21 +327,14 @@ def test_ext_attn_table_matches_whole_pass(ops):
             m = -(-3 * K // G)
             pad = G * m - 3 * K
             padded = [torch.cat([t, t[-1:].expand(pad, S, dim)]) if pad else t for t in (q, k, v)]
+            parts = []
             for r in range(G):
                 sh = PivotalShard(G, r, K)
-                q_local = padded[0][r * m:(r + 1) * m]
-                q_src = padded[0] if inject else q_local
-                rank_table = sh.attention_table(inject)
-                out = ops.ext_attn_table(q_src, padded[1], padded[2], rank_table, heads, d ** -0.5)
-                for j, i in enumerate(sh.slots):
-                    if i < 3 * K:
-                        if inject and i >= K:
-                            # the whole pass pairs the uncond / cond sample of a keyframe (shared q, k: one kernel computes
-                            # their probabilities once); a rank that holds only one of the two runs the per-sample kernel
-                            check_ext_attn(out[j:j + 1], q_src, padded[1], padded[2], rank_table[j:j + 1], heads,
-                                           d ** -0.5)
-                        else:
-                            assert torch.equal(out[j], whole[i]), (G, r, j)
+                row0, nrows = sh.row_split(S)
+                parts.append(ops.ext_attn_table(*padded, sh.global_attention_table(inject), heads, d ** -0.5,
+                                                row0=row0, nrows=nrows))
+            got = torch.stack(parts).permute(1, 0, 2, 3).reshape(3 * K, G * nrows, dim)[:, :S]
+            assert torch.equal(got, whole), (inject, G, (got.float() - whole.float()).abs().max().item())
 
 
 def test_nn_field_sd21_token_counts(ops):

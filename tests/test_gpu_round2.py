@@ -422,12 +422,13 @@ class _ThreadWorld:
         return _ThreadWorld._Rank(self, r)
 
 
-@pytest.mark.parametrize("token_split,dual", [(True, True), (True, False), (False, False)])
-@pytest.mark.parametrize("world", [2, 4])
-def test_sharded_cuda_path_in_one_process(world, token_split, dual):
+@pytest.mark.parametrize("dual", [True, False])
+@pytest.mark.parametrize("world", [2, 4, 8])
+def test_sharded_cuda_path_in_one_process(world, dual):
     """The multi-GPU code path of the hooks on the CUDA kernels (packed q|k|v|unit gather, query-row split of the
     extended attention with the paired kernel, output re-assembly, sharded conv injection) with `world` rank threads
-    on one GPU == the single-rank edit."""
+    on one GPU == the single-rank edit.  At 8 ranks the 3K = 12 pivotal samples fill 16 slots: padding slots, and
+    ranks that hold no sample and no query rows."""
     import threading
     steps, n_frames, batch = 4, 8, 2
 
@@ -435,7 +436,7 @@ def test_sharded_cuda_path_in_one_process(world, token_split, dual):
         try:
             cfg = {"n_frames": n_frames, "batch_size": batch, "n_timesteps": steps, "guidance_scale": 7.5, "mode": "pnp",
                    "pnp_attn_t": 0.5, "pnp_f_t": 0.8, "fused_pass": True, "cuda_graph": False, "keyframe_seed": 1,
-                   "token_split": token_split, "dual_stream": dual and world_size > 1}
+                   "dual_stream": dual and world_size > 1}
             x, text, pnp, src = synthetic_inputs(n_frames, 16, unet.config.cross_attention_dim, steps, seed=1,
                                                  device="cuda", dtype=torch.float16, ctx_len=7)
             ed = TokenFlowEditor(unet, DDIMScheduler(), tfu, cfg, text, pnp, source_latents=lambda t: src[t],

@@ -1,6 +1,6 @@
 """CPU tier: the multi-GPU path (frames sharded, keyframe tensors all-gathered) on 2 gloo ranks with
-the oracle ops == the single-process loop.  Covers the shard plan, the all-gather ordering, the
-per-frame keyframe/weight tables and the sharded attention table."""
+the oracle ops == the single-process loop.  Covers the shard plan, the all-gather ordering and routing,
+the per-frame keyframe/weight tables and the sharded attention table."""
 import os
 
 import pytest
@@ -68,27 +68,58 @@ def test_two_rank_edit_equals_single_process(mode, steps, fused):
         assert torch.allclose(torch.tensor(out), want, atol=2e-4, rtol=1e-4), f"rank {rank}"
 
 
-def test_shard_plan_and_attention_table():
+def test_shard_plan_and_global_attention_table():
     K = 5
     for G in (2, 4, 8):
+        m = -(-15 // G)
         seen = []
         for r in range(G):
             sh = tfu.PivotalShard(G, r, K)
-            assert len(sh.slots) == -(-15 // G)
+            assert len(sh.slots) == m
             seen += sh.slots
-            tab = sh.attention_table(False)
-            tab_inj = sh.attention_table(True)
-            for j, i in enumerate(sh.slots):
-                if i >= 15:
-                    assert tab[j][3] == 1 and tab_inj[j][3] == 1
-                    continue
+            tab = sh.global_attention_table(False)
+            tab_inj = sh.global_attention_table(True)
+            assert len(tab) == len(tab_inj) == 15
+            for i in range(15):
+                for qs, k0, v0, nkv in (tab[i], tab_inj[i]):       # inside the G*m gathered slabs
+                    assert 0 <= qs < G * m and 0 <= k0 and k0 + nkv <= G * m and 0 <= v0 and v0 + nkv <= G * m
                 s, f = divmod(i, K)
                 if s == 0:
-                    assert tab[j] == (j, i, i, 1) and tab_inj[j] == (i, i, i, 1)
+                    assert tab[i] == tab_inj[i] == (i, i, i, 1)
                 else:
-                    assert tab[j] == (j, s * K, s * K, K)
-                    assert tab_inj[j] == (f, 0, s * K, K)       # q and k of the source stream, own v
-        assert seen[:15] == list(range(15)) and len(seen) == G * -(-15 // G)
+                    assert tab[i] == (i, s * K, s * K, K)
+                    assert tab_inj[i] == (f, 0, s * K, K)       # q and k of the source stream, own v
+        assert seen == list(range(G * m))                       # every slot once; the first 15 are the samples
+
+
+def test_all_gather_routes(monkeypatch):
+    """`ops.all_gather`: one rank returns its input; a CPU tensor never reaches an attached communicator (tf_allgather
+    would read it as device memory) but goes through torch.distributed, contiguous; the communicator itself refuses
+    anything that is not on the current CUDA device."""
+    from tokenflow_b200 import ops
+    t = torch.arange(12.0).view(3, 4)
+    assert ops.all_gather(t, 1, comm=object()) is t
+
+    class RecordingComm:
+        calls = 0
+
+        def all_gather(self, t):
+            RecordingComm.calls += 1
+            return t
+
+    recorded = []
+
+    def all_gather_into_tensor(out, t, group=None):
+        recorded.append((tuple(out.shape), t.is_contiguous(), group))
+        out.copy_(torch.cat([t, t + 100]))
+
+    monkeypatch.setattr(dist, "all_gather_into_tensor", all_gather_into_tensor)
+    got = ops.all_gather(t.t(), 2, group="g", comm=RecordingComm())     # a strided view
+    assert RecordingComm.calls == 0
+    assert recorded == [((8, 3), True, "g")]
+    assert torch.equal(got, torch.cat([t.t(), t.t() + 100]))
+    with pytest.raises(ops.TokenflowB200Error):
+        ops.Communicator.__new__(ops.Communicator).all_gather(t)
 
 
 def test_frame_table_matches_batch_idx_arithmetic():

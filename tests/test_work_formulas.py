@@ -51,23 +51,27 @@ def test_ops_flop_accounting_matches_formula():
     assert per_batch * (2 * 40 / B - 1) / 2 == pytest.approx(773.1e9, rel=1e-3)
 
 
-@given(K=st.integers(1, 50), G=st.sampled_from([1, 2, 3, 4, 8]))
+@given(K=st.integers(1, 50), G=st.sampled_from([1, 2, 3, 4, 8]), S=st.integers(1, 10000))
 @settings(max_examples=60, deadline=None)
-def test_pivotal_shard_covers_every_sample_once(K, G):
-    seen = []
+def test_pivotal_shard_covers_every_sample_and_row_once(K, G, S):
+    seen, rows = [], []
     m = -(-3 * K // G)
     for r in range(G):
         sh = tfu.PivotalShard(G, r, K)
         assert len(sh.slots) == m
         seen += sh.slots
         for inject in (False, True):
-            for j, (qs, k0, v0, nkv) in enumerate(sh.attention_table(inject)):
-                i = sh.slots[j]
+            tab = sh.global_attention_table(inject)
+            assert len(tab) == 3 * K
+            for i, (qs, k0, v0, nkv) in enumerate(tab):
                 assert 0 <= k0 and k0 + nkv <= G * m and 0 <= v0 and v0 + nkv <= G * m
-                assert 0 <= qs < (G * m if inject else m)
-                if i < 3 * K and i >= K:                       # extended streams see all K keyframes of the stream
+                assert 0 <= qs < G * m
+                if i >= K:                                     # extended streams see all K keyframes of the stream
                     assert nkv == K and v0 == (i // K) * K
+        row0, nrows = sh.row_split(S)
+        rows += range(row0, min(S, row0 + nrows))
     assert seen == list(range(G * m)) and G * m >= 3 * K
+    assert rows == list(range(S))                              # every query row on exactly one rank, in order
 
 
 @given(B=st.integers(1, 16), batches=st.integers(1, 12))

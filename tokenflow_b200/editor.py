@@ -23,6 +23,8 @@ from typing import Callable, Dict, Optional
 import torch
 import torch.nn as nn
 
+from .ops import all_gather
+
 
 class TokenFlowEditor(nn.Module):
     def __init__(self, unet: nn.Module, scheduler, hooks, config: Dict, text_embeds: torch.Tensor,
@@ -199,7 +201,6 @@ class TokenFlowEditor(nn.Module):
 
     @torch.no_grad()
     def _sharded_step(self, x, t, indices):
-        import torch.distributed as dist
         h, G, r = self.hooks, self.world_size, self.rank
         N, B = len(x), self.config["batch_size"]
         K = N // B
@@ -209,7 +210,7 @@ class TokenFlowEditor(nn.Module):
         src_all = self.source_latents_t(int(t))[indices].to(x.device, x.dtype)
         h.register_time(self, int(t))
         # ---- pivotal pass: this rank's m of the 3K (stream, keyframe) samples ----
-        shard = h.PivotalShard(G, r, K, self.group, comm=self.comm, token_split=self.config.get("token_split", True))
+        shard = h.PivotalShard(G, r, K, self.group, comm=self.comm)
         lat, emb = [], []
         for i in shard.slots:
             i = min(i, 3 * K - 1)                             # padding slots recompute the last sample
@@ -233,9 +234,7 @@ class TokenFlowEditor(nn.Module):
         _, npu, npc = noise_pred.chunk(3)
         noise_pred = npu + self.config["guidance_scale"] * (npc - npu)
         x_local = self.scheduler.step(noise_pred, t, xs)['prev_sample'].contiguous()
-        out = torch.empty_like(x)
-        dist.all_gather_into_tensor(out, x_local, group=self.group)
-        return out
+        return all_gather(x_local, G, self.group, self.comm)
 
     def _timestep_pair(self, t):
         """(host int, device scalar) of a timestep without reading the device when `t` is a host value."""
@@ -266,8 +265,7 @@ class TokenFlowEditor(nn.Module):
         key = (K, id(self.comm))
         shard = self._shard_cache.get(key)
         if shard is None:                     # one shard context per (K, communicator): it caches device index tensors
-            shard = self._shard_cache[key] = self.hooks.PivotalShard(G, r, K, self.group, comm=self.comm,
-                                                                     token_split=self.config.get("token_split", True))
+            shard = self._shard_cache[key] = self.hooks.PivotalShard(G, r, K, self.group, comm=self.comm)
         return [divmod(min(i, 3 * K - 1), K) for i in shard.slots], shard
 
     def _fused_text(self, slots, per):
@@ -303,21 +301,7 @@ class TokenFlowEditor(nn.Module):
         finally:
             h.register_fused(self, 0)
             h.register_shard(self, None)
-        _, npu, npc = noise_pred.chunk(3)
-        ops = self._cuda_ops()
-        if ops is not None and coef is not None and npu.dtype == torch.float16 and xs.dtype == torch.float16:
-            x_local = ops.cfg_ddim(npu, npc, xs, coef, self.config["guidance_scale"])     # one kernel, same roundings
-        else:
-            noise_pred = npu + self.config["guidance_scale"] * (npc - npu)
-            x_local = self.scheduler.step(noise_pred, t_int, xs)['prev_sample'].contiguous()
-        if G == 1:
-            return x_local
-        if self.comm is not None and x_local.is_cuda:
-            return self.comm.all_gather(x_local)
-        import torch.distributed as dist
-        out = torch.empty_like(x)
-        dist.all_gather_into_tensor(out, x_local, group=self.group)
-        return out
+        return self._update_and_gather(noise_pred, xs, coef, t_int)
 
     def _dual_compute(self, x, src_all, piv_idx, t_dev, t_int, coef, slots, shard):
         """The same step as `_fused_compute` as TWO UNet calls on two CUDA streams: the pivotal samples (few, and all
@@ -356,21 +340,19 @@ class TokenFlowEditor(nn.Module):
             h.register_dual_stream(self, False)
             h.register_shard(self, None)
         del piv_lat
+        return self._update_and_gather(noise_pred, xs, coef, t_int)
+
+    def _update_and_gather(self, noise_pred, xs, coef, t_int):
+        """Tail of a fused step: classifier-free guidance + DDIM update of this rank's frames `xs` from their
+        [source | uncond | cond] noise predictions, then the all-gather of every rank's frames."""
         _, npu, npc = noise_pred.chunk(3)
         ops = self._cuda_ops()
         if ops is not None and coef is not None and npu.dtype == torch.float16 and xs.dtype == torch.float16:
-            x_local = ops.cfg_ddim(npu, npc, xs, coef, self.config["guidance_scale"])
+            x_local = ops.cfg_ddim(npu, npc, xs, coef, self.config["guidance_scale"])     # one kernel, same roundings
         else:
             noise_pred = npu + self.config["guidance_scale"] * (npc - npu)
             x_local = self.scheduler.step(noise_pred, t_int, xs)['prev_sample'].contiguous()
-        if G == 1:
-            return x_local
-        if self.comm is not None and x_local.is_cuda:
-            return self.comm.all_gather(x_local)
-        import torch.distributed as dist
-        out = torch.empty_like(x)
-        dist.all_gather_into_tensor(out, x_local, group=self.group)
-        return out
+        return all_gather(x_local, self.world_size, self.group, self.comm)
 
     def _step_compute(self, *a):
         # Off unless asked for: on one GPU the concurrent chains slow each other down, and with real NCCL ranks this

@@ -517,6 +517,21 @@ def body_ops() -> Optional[CudaOps]:
     return _BODY_OPS
 
 
+def all_gather(t: torch.Tensor, world_size: int, group=None, comm=None) -> torch.Tensor:
+    """[n, ...] on every rank -> [world_size * n, ...] in rank order: the one collective of the package.  A CUDA tensor
+    goes through `comm` (a `Communicator`) when one is attached, everything else through torch.distributed on
+    `group`; one rank returns `t` itself."""
+    if world_size == 1:
+        return t
+    if comm is not None and t.is_cuda:
+        return comm.all_gather(t)
+    import torch.distributed as dist
+    t = t.contiguous()
+    out = torch.empty((world_size * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
+    dist.all_gather_into_tensor(out, t, group=group)
+    return out
+
+
 class Communicator:
     """NCCL all-gather through the C ABI (tf_comm_init / tf_allgather, include/tokenflow_b200.h): the data
     plane of the multi-GPU pivotal pass.  The 128-byte NCCL id travels over torch.distributed (control
@@ -545,6 +560,10 @@ class Communicator:
                                      f"{self.lib.tf_last_error().decode(errors='replace')}")
 
     def all_gather(self, t: torch.Tensor) -> torch.Tensor:
+        # tf_allgather reads numel * esz bytes from the pointer: it must be device memory of this rank's GPU, dense
+        if not t.is_cuda or t.device.index != torch.cuda.current_device():
+            raise TokenflowB200Error(f"Communicator.all_gather needs a tensor on the current CUDA device, got one on "
+                                     f"{t.device}")
         t = t.contiguous()
         out = torch.empty((self.world_size * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
         self._check(self.lib.tf_allgather(self.handle, t.data_ptr(), out.data_ptr(), t.numel() * t.element_size(),

@@ -27,6 +27,8 @@ from typing import Dict, Iterable, List, Optional, Tuple
 
 import torch
 
+from .ops import all_gather
+
 # Which attn1 the graphed path runs: the module's own SDPA forward (False) or the native per-sample attention of
 # `tokenflow_utils.register_native_self_attention`, installed for the duration of the call (True).  SDPA stays: on an
 # H100 80GB HBM3 at a 400 W power limit the native route made the C2 inversion step slower, 132.2 ms against 124.2 ms
@@ -112,16 +114,14 @@ class LatentInverter:
         return self.rank * per, min(n, (self.rank + 1) * per)
 
     def _gathered(self, x_local, n: int):
+        """All N frames from every rank's share (the last shares may be short: padded to equal size)."""
         if self.world_size == 1:
             return x_local
-        import torch.distributed as dist
         per = -(-n // self.world_size)
         pad = per - x_local.shape[0]
         if pad:
             x_local = torch.cat([x_local, x_local.new_zeros((pad,) + tuple(x_local.shape[1:]))])
-        out = torch.empty((self.world_size * per,) + tuple(x_local.shape[1:]), dtype=x_local.dtype, device=x_local.device)
-        dist.all_gather_into_tensor(out, x_local.contiguous(), group=self.group)
-        return out[:n]
+        return all_gather(x_local, self.world_size, self.group, self.comm)[:n]
 
     @torch.no_grad()
     def ddim_inversion(self, cond: torch.Tensor, latent_frames: torch.Tensor, save_path: Optional[str], batch_size: int,
@@ -262,16 +262,6 @@ class LatentInverter:
             if native:
                 tfu.remove_native_self_attention(self.unet)
 
-    def _all_gather(self, t: torch.Tensor) -> torch.Tensor:
-        if self.world_size == 1:
-            return t
-        if self.comm is not None:
-            return self.comm.all_gather(t.contiguous())
-        import torch.distributed as dist
-        out = torch.empty((self.world_size * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
-        dist.all_gather_into_tensor(out, t.contiguous(), group=self.group)
-        return out
-
     def _share(self, frames: torch.Tensor) -> Tuple[torch.Tensor, int]:
         n = frames.shape[0]
         lo, hi = self._local(n)
@@ -288,7 +278,8 @@ class LatentInverter:
         saved = torch.zeros((len(plan), per) + tuple(latent_frames.shape[1:]), dtype=torch.float16, device=self.device)
         self._run_steps(x_share, cond, batch_size, inv_coef, ts_up_dev, slots, saved)
         # one collective after the last step: [G * n_saved, per, ...] -> per saved timestep, the N frames in order
-        full = self._all_gather(saved).view((self.world_size, len(plan), per) + tuple(latent_frames.shape[1:]))
+        full = all_gather(saved, self.world_size, self.group, self.comm)
+        full = full.view((self.world_size, len(plan), per) + tuple(latent_frames.shape[1:]))
         self._saved = {t: full[:, k].reshape((self.world_size * per,) + tuple(latent_frames.shape[1:]))[:n].clone()
                        for k, t in enumerate(plan)}
         del full, saved
@@ -301,15 +292,8 @@ class LatentInverter:
     @torch.no_grad()
     def _device_sample(self, x, cond, batch_size):
         _, rec_coef, _, ts_dn_dev = self._device_tables()
-        n = x.shape[0]
-        x_share, per = self._share(x)
-        out = self._run_steps(x_share, cond, batch_size, rec_coef, ts_dn_dev)
-        if self.world_size == 1:
-            return out
-        pad = per - out.shape[0]
-        if pad:
-            out = torch.cat([out, out.new_zeros((pad,) + tuple(out.shape[1:]))])
-        return self._all_gather(out)[:n]
+        x_share, _ = self._share(x)
+        return self._gathered(self._run_steps(x_share, cond, batch_size, rec_coef, ts_dn_dev), x.shape[0])
 
 
 def _native_vae(vae) -> bool:

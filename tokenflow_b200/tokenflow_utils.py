@@ -19,7 +19,10 @@ Differences from the reference that do not change results:
     device sync per attn1 call (reference :124);
   * PnP q/k injection (:124-130) copies nothing — the kernel reads the source stream's q/k;
   * the frame pass can be driven per frame (`register_frame_table`) so frames, not only whole
-    batches, shard across GPUs (SURVEY.md §8e); `register_batch_idx` keeps the reference meaning.
+    batches, shard across GPUs (SURVEY.md §8e); `register_batch_idx` keeps the reference meaning;
+  * the pivotal pass can be sharded over GPUs (`PivotalShard`, `register_shard`): per block, one
+    all-gather of the packed [q | k | v | pivot unit rows], the extended attention of every sample
+    for this rank's query rows (tf_ext_attn_fwd_rows), one all-gather of the attention output.
 """
 from __future__ import annotations
 
@@ -29,6 +32,7 @@ from typing import List, Optional, Sequence, Type
 
 import torch
 
+from . import ops as tf_ops
 from .sd_unet import norm_act
 from .util import isinstance_str, batch_cosine_sim  # noqa: F401  (re-exported like the reference)
 
@@ -123,14 +127,14 @@ class PivotalShard:
     """Multi-GPU pivotal pass (SURVEY.md §8e).  The 3K (stream, keyframe) samples of the pass, in the
     reference's batch order i = stream*K + keyframe, are dealt to the G ranks in contiguous groups of
     m = ceil(3K/G) slots (the tail is padded with dummy samples); an all-gather along that axis
-    therefore reproduces the reference's [3K, S, dim] layout in its first 3K slabs.  Collectives go
-    through torch.distributed (NCCL over NVLink on GPUs, gloo in the CPU tests)."""
+    therefore reproduces the reference's [3K, S, dim] layout in its first 3K slabs.  The extended
+    attention is split by query rows (`row_split`): every rank evaluates all 3K samples for its rows,
+    which balances the work exactly and keeps q/k-injected sample pairs together.  Collectives go
+    through `ops.all_gather` (tf_allgather when a Communicator is attached, else torch.distributed:
+    NCCL over NVLink on GPUs, gloo in the CPU tests)."""
 
-    def __init__(self, world_size: int, rank: int, n_keyframes: int, group=None, comm=None, token_split: bool = True):
+    def __init__(self, world_size: int, rank: int, n_keyframes: int, group=None, comm=None):
         self.world_size, self.rank, self.K, self.group = world_size, rank, n_keyframes, group
-        # token_split: every rank computes the extended attention of ALL samples for its share of the query rows
-        # (exactly balanced, and paired q/k-injected samples stay together) instead of all rows of its own samples
-        self.token_split = bool(token_split)
         self.comm = comm                      # ops.Communicator (tf_allgather through the C ABI) or None
         self.m = -(-3 * n_keyframes // world_size)
         self.slots = list(range(rank * self.m, (rank + 1) * self.m))     # global sample ids (>= 3K: padding)
@@ -150,13 +154,7 @@ class PivotalShard:
 
     def all_gather(self, t: torch.Tensor) -> torch.Tensor:
         self.n_collectives += 1
-        if self.comm is not None and t.is_cuda:
-            return self.comm.all_gather(t)
-        import torch.distributed as dist
-        t = t.contiguous()
-        out = torch.empty((self.world_size * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
-        dist.all_gather_into_tensor(out, t, group=self.group)
-        return out
+        return tf_ops.all_gather(t, self.world_size, self.group, self.comm)
 
     def row_split(self, S: int):
         """Query-token range [row0, row0 + nrows) of this rank when the extended attention of ALL 3K samples is
@@ -185,22 +183,6 @@ class PivotalShard:
             idx = torch.tensor([min(i, 3 * self.K - 1) for i in self.slots], dtype=torch.int64).to(device)
             self._src_index[key] = idx
         return idx
-
-    def attention_table(self, inject: bool):
-        """Per local slot: (q slab, first k slab, first v slab, number of key slabs) in the coordinates of
-        the gathered K/V (global sample order); q is global when injecting (the source stream's q may live
-        on another rank), local otherwise.  Reference :124-138."""
-        K, tab = self.K, []
-        for j, i in enumerate(self.slots):
-            if i >= 3 * K:                       # padding slot: harmless self-attention on its own slab
-                tab.append((i if inject else j, i, i, 1))
-                continue
-            s, f = divmod(i, K)
-            if s == 0:
-                tab.append((i if inject else j, i, i, 1))
-            else:
-                tab.append((f if inject else j, 0 if inject else s * K, s * K, K))
-        return tab
 
 
 def _conv_injection_site(diffusion_model):
@@ -392,7 +374,7 @@ def _fused_weight(attn, names, dtype):
     return hit[1]
 
 
-def _token_split_attention(attn, to_out, shard, q_all, k_all, v_all, inject):
+def _row_split_attention(attn, to_out, shard, q_all, k_all, v_all, inject):
     """Extended attention of ALL 3K samples for this rank's query rows, `to_out` on those rows, all-gather, and
     re-assembly of the complete [3K, S, dim] output (stashed on the module for the block); returns the rows of the
     local samples."""
@@ -428,49 +410,23 @@ def _sa_forward(attn, pnp: bool):
         shard = getattr(attn, "_tf_shard", None)
         dim = attn.to_q.weight.shape[0]
         if fast_path(x, encoder_hidden_states):
-            if shard is None:
-                qkv = torch.nn.functional.linear(x, _fused_weight(attn, ("to_q", "to_k", "to_v"), torch.float16))
-                q, k, v = qkv[..., :dim], qkv[..., dim:2 * dim], qkv[..., 2 * dim:]
-                out = _ops().ext_attn(q, k, v, attn.heads, attn.scale, inject)
-            elif shard.token_split:
-                # sharded pivotal pass, query rows split over the ranks: ONE all-gather of [q | k | v | pivot unit rows]
-                # per sample, attention of all 3K samples for this rank's query rows, to_out on those rows, ONE
-                # all-gather of the result (the block picks the complete [3K, S, dim] output up from the closure)
-                q = torch.nn.functional.linear(x, _fused_weight(attn, ("to_q",), torch.float16))
-                kv = torch.nn.functional.linear(x, _fused_weight(attn, ("to_k", "to_v"), torch.float16))
-                unit = attn.__dict__.pop("_tf_unit_local", None)
-                packed = shard.all_gather(torch.cat([q, kv] + ([unit] if unit is not None else []), dim=-1))
-                if unit is not None:
-                    attn._tf_unit_gathered = packed[..., 3 * dim:]
-                return _token_split_attention(attn, to_out, shard, packed[..., :dim], packed[..., dim:2 * dim],
-                                              packed[..., 2 * dim:3 * dim], inject)
-            else:
-                # sharded pivotal pass: ONE all-gather of [k | v | pivot unit rows] along the sample axis
-                # (+ one of q only while PnP-injecting, when the source stream's q lives on another rank)
-                q = torch.nn.functional.linear(x, _fused_weight(attn, ("to_q",), torch.float16))
-                kv = torch.nn.functional.linear(x, _fused_weight(attn, ("to_k", "to_v"), torch.float16))
-                unit = attn.__dict__.pop("_tf_unit_local", None)
-                packed = shard.all_gather(kv if unit is None else torch.cat([kv, unit], dim=-1))
-                if unit is not None:
-                    attn._tf_unit_gathered = packed[..., 2 * dim:]
-                k_all, v_all = packed[..., :dim], packed[..., dim:2 * dim]
-                q_src = shard.all_gather(q) if inject else q
-                out = _ops().ext_attn_table(q_src, k_all, v_all, shard.attention_table(inject), attn.heads, attn.scale)
-            return to_out(out)
-        ctx = x if encoder_hidden_states is None else encoder_hidden_states
-        q = attn.to_q(x)
-        k = attn.to_k(ctx)
-        v = attn.to_v(ctx)
-        if shard is None:
-            out = _ops().ext_attn(q, k, v, attn.heads, attn.scale, inject)
-        elif shard.token_split:
-            qkv_all = shard.all_gather(torch.cat([q, k, v], dim=-1))
-            return _token_split_attention(attn, to_out, shard, qkv_all[..., :dim], qkv_all[..., dim:2 * dim],
-                                          qkv_all[..., 2 * dim:], inject)
-        else:                                    # keyframe K/V (and, when injecting, Q) all-gathered over NVLink
-            k_all, v_all = shard.all_gather(k), shard.all_gather(v)
-            q_src = shard.all_gather(q) if inject else q
-            out = _ops().ext_attn_table(q_src, k_all, v_all, shard.attention_table(inject), attn.heads, attn.scale)
+            qkv = torch.nn.functional.linear(x, _fused_weight(attn, ("to_q", "to_k", "to_v"), torch.float16))
+            q, k, v = qkv[..., :dim], qkv[..., dim:2 * dim], qkv[..., 2 * dim:]
+        else:
+            ctx = x if encoder_hidden_states is None else encoder_hidden_states
+            q, k, v = attn.to_q(x), attn.to_k(ctx), attn.to_v(ctx)
+        if shard is not None:
+            # sharded pivotal pass: ONE all-gather of [q | k | v | pivot unit rows] per sample, attention of all 3K
+            # samples for this rank's query rows, to_out on those rows, ONE all-gather of the result (the block picks
+            # the gathered unit rows and the complete [3K, S, dim] output up from the module)
+            unit = attn.__dict__.pop("_tf_unit_local", None)
+            packed = shard.all_gather(torch.cat([q, k, v] + ([unit] if unit is not None else []), dim=-1))
+            if unit is not None:
+                # torch.cat promotes (fp16 unit rows next to fp32 q): back to the unit rows' dtype, exact
+                attn._tf_unit_gathered = packed[..., 3 * dim:].to(unit.dtype)
+            return _row_split_attention(attn, to_out, shard, packed[..., :dim], packed[..., dim:2 * dim],
+                                        packed[..., 2 * dim:3 * dim], inject)
+        out = _ops().ext_attn(q, k, v, attn.heads, attn.scale, inject)
         if not torch.is_autocast_enabled() and out.dtype != to_out.weight.dtype:
             out = out.to(to_out.weight.dtype)       # fp16 kernel output feeding a non-autocast fp32 module
         return to_out(out)
@@ -616,46 +572,38 @@ def make_tokenflow_attention_block(block_class: Type[torch.nn.Module]) -> Type[t
             fused_ln = (hidden_states.is_cuda and hidden_states.dtype == torch.float16
                         and hasattr(ops, "layernorm_rows") and not self.only_cross_attention
                         and (torch.is_autocast_enabled() or self.norm1.weight.dtype == torch.float16))
-            if shard is not None:
-                # sharded pivotal pass: this rank holds m of the 3K (stream, keyframe) samples
-                if fused_ln:
-                    # one read of hidden_states -> fp16 norm1 output (QKV operand) + its unit rows; the unit rows
-                    # ride in the attention's K/V all-gather (one collective instead of two)
-                    norm_hidden_states, unit = ops.layernorm_rows(hidden_states, self.norm1, batch_size)
-                    self.attn1._tf_unit_local = unit
-                    self.pivot_hidden_states = norm_hidden_states
-                    self.attn_output = self.attn1(norm_hidden_states, **cross_attention_kwargs)
-                    unit_all = self.attn1.__dict__.pop("_tf_unit_gathered", None)
-                    if unit_all is None:                      # the closure took its generic path
-                        unit_all = shard.all_gather(self.attn1.__dict__.pop("_tf_unit_local", unit))
-                    self._tf_pivot_unit = unit_all[:shard.K].contiguous()              # source stream
-                else:
-                    norm_hidden_states = self.norm1(hidden_states)
-                    unit_all = shard.all_gather(ops.unit_rows(norm_hidden_states))
-                    self._tf_pivot_unit = unit_all[:shard.K]                              # source stream
-                    self.pivot_hidden_states = norm_hidden_states
-                    self.attn_output = self.attn1(norm_hidden_states, **cross_attention_kwargs)
-                full = self.attn1.__dict__.pop("_tf_attn_full", None)         # token-split closure: already complete
-                self.kf_attn_output = full if full is not None else shard.all_gather(self.attn_output)[:3 * shard.K]
-                self._tf_record_ready()
+            # unit rows of the pivot features for the NN field: of the source stream, or, when sharded (this rank holds
+            # m of the 3K (stream, keyframe) samples), of every local sample — the source samples may be on any rank
+            n_unit = batch_size if shard is not None else batch_size // 3
+            if fused_ln:
+                # one read of hidden_states -> fp16 norm1 output (QKV operand) + its unit rows
+                norm_hidden_states, unit = ops.layernorm_rows(hidden_states, self.norm1, n_unit)
             else:
-                n_frames = batch_size // 3
-                if fused_ln:
-                    norm_hidden_states, unit = ops.layernorm_rows(hidden_states, self.norm1, n_frames)
-                    self._tf_pivot_unit = unit
-                else:
-                    norm_hidden_states = self.norm1(hidden_states)
-                    self._tf_pivot_unit = None
+                norm_hidden_states = self.norm1(hidden_states)
+                unit = ops.unit_rows(norm_hidden_states[:n_unit])
+            if shard is not None:
+                # the unit rows ride in the attention's q|k|v all-gather, which also re-assembles the complete output
+                self.attn1._tf_unit_local = unit
+                self.pivot_hidden_states = norm_hidden_states
+                self.attn_output = self.attn1(norm_hidden_states, **cross_attention_kwargs)
+                unit_all = self.attn1.__dict__.pop("_tf_unit_gathered", None)
+                full = self.attn1.__dict__.pop("_tf_attn_full", None)
+                if unit_all is None or full is None:
+                    raise RuntimeError("tokenflow_b200: a sharded pivotal pass needs the extended-attention attn1 of "
+                                       "register_extended_attention[_pnp]; this block's attn1 did not gather the pivot "
+                                       "unit rows and the attention output")
+                self._tf_pivot_unit = unit_all[:shard.K].contiguous()              # source stream
+                self.kf_attn_output = full
+            else:
                 # cache keyframe features (:326-327) — plus their fp16 unit rows for the NN field
-                self.pivot_hidden_states = norm_hidden_states.view(3, n_frames, sequence_length, dim)
-                if self._tf_pivot_unit is None:
-                    self._tf_pivot_unit = ops.unit_rows(self.pivot_hidden_states[0])
+                self._tf_pivot_unit = unit
+                self.pivot_hidden_states = norm_hidden_states.view(3, n_unit, sequence_length, dim)
                 self.attn_output = self.attn1(
                     norm_hidden_states,
                     encoder_hidden_states=encoder_hidden_states if self.only_cross_attention else None,
                     **cross_attention_kwargs)
                 self.kf_attn_output = self.attn_output                                   # :360
-                self._tf_record_ready()
+            self._tf_record_ready()
             return self.attn_output + hidden_states                                      # :397
 
         def _tf_record_ready(self):
