@@ -184,6 +184,28 @@ int tf_frames_to_nhwc(const void* frames_u8, int64_t n_px, void* out_f16, tf_str
  *   frames_u8   device [n_px, 3] uint8 ([N, H, W, 3]), 16-byte aligned */
 int tf_nhwc_to_frames(const void* x_f16, int64_t n_px, void* frames_u8, tf_stream_t stream);
 
+/* Pillow's `Image.resize((w, h), Image.LANCZOS)` of RGB uint8 frames, bit for bit (libImaging/Resample.c): the
+ * reference's frame resize (util.py:28 to (W, H); run_tokenflow_pnp.py:174-175, run_tokenflow_sdedit.py:136-137,
+ * preprocess.py:191-192 square frames to 512x512).  Per axis, Lanczos-3 weights in double, normalised and rounded to
+ * int32 with 22 fractional bits; a horizontal pass into a uint8 intermediate, then a vertical pass, each value
+ * clamp((2^21 + sum v * k) >> 22, 0, 255).  A pass whose axis keeps its size is skipped; equal sizes are a copy.
+ * Sizes are in [1, 65536].
+ *
+ * tf_resize_taps      taps per output pixel of the table for one axis `in` -> `out` (-1 for bad sizes)
+ * tf_resize_coeffs    fills that axis's tables on the host:
+ *                       bounds  host [out, 2] int32: first input pixel, number of taps used (<= taps)
+ *                       coeffs  host [out, taps] int32 fixed-point weights, zero past the used taps
+ * tf_resize_u8        in [n, h_in, w_in, 3] -> out [n, h, w, 3], both device uint8, any alignment
+ *   h_bounds, h_coeffs, h_taps   device copies of the tables for w_in -> w (unused, may be NULL, when w == w_in)
+ *   v_bounds, v_coeffs, v_taps   the same for h_in -> h (unused when h == h_in)
+ *   tmp                          device [n, h_in, w, 3] uint8 intermediate, used only when both axes change
+ * The device tables are trusted: they must be what tf_resize_coeffs wrote for the same sizes. */
+int tf_resize_taps(int in, int out);
+int tf_resize_coeffs(int in, int out, int32_t* bounds, int32_t* coeffs);
+int tf_resize_u8(const void* in, int64_t n, int h_in, int w_in, int h, int w, const int32_t* h_bounds,
+                 const int32_t* h_coeffs, int h_taps, const int32_t* v_bounds, const int32_t* v_coeffs, int v_taps,
+                 void* tmp, void* out, tf_stream_t stream);
+
 /* ---- multi-GPU: all-gather of keyframe tensors along the pivotal-sample axis (SURVEY.md §8e) ----
  * NCCL (all-gather over NVLink 5 / NVSwitch) bound at run time; one communicator per process/GPU.
  * Rendezvous: rank 0 calls tf_comm_unique_id and ships the TF_COMM_ID_BYTES to the other ranks by any

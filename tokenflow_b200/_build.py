@@ -19,13 +19,14 @@ LIB_PATH = PKG_DIR / "libtokenflow_b200.so"
 STAMP = PKG_DIR / ".libtokenflow_b200.stamp"
 
 SOURCES = ["tf_capi.cu", "tf_unit_rows.cu", "tf_propagate.cu", "tf_nn_field.cu", "tf_ext_attn.cu", "tf_cfg_ddim.cu",
-           "tf_comm.cu", "tf_body.cu", "tf_pixels.cu"]
+           "tf_comm.cu", "tf_body.cu", "tf_pixels.cu", "tf_resize.cu"]
 HEADERS = ["tf_common.cuh", "tf_kernels.h", "tf_wgmma.cuh", "../../include/tokenflow_b200.h"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
+    "-Xcompiler", "-ffp-contract=off",     # host code: tf_resize_coeffs must round like Pillow's C build
     "-Xptxas", "-v",
     "--expt-relaxed-constexpr",
     "-cudart", "static",

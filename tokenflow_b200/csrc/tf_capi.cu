@@ -104,13 +104,23 @@ static int check_group_norm_shape(int64_t n, int64_t hw, int c, int groups) {
   return TF_OK;
 }
 
+constexpr int kResizeMaxSide = 1 << 16;
+
+static bool resize_sizes_ok(int in, int out, const char* who) {
+  if (in < 1 || out < 1 || in > kResizeMaxSide || out > kResizeMaxSide) {
+    set_last_error("%s: sizes in=%d out=%d outside [1, %d]", who, in, out, kResizeMaxSide);
+    return false;
+  }
+  return true;
+}
+
 }  // namespace tf
 
 using namespace tf;
 
 extern "C" {
 
-int tf_version(void) { return 1000; }
+int tf_version(void) { return 1001; }
 
 const char* tf_last_error(void) { return g_err; }
 
@@ -257,6 +267,56 @@ int tf_nhwc_to_frames(const void* x_f16, int64_t n_px, void* frames_u8, tf_strea
   int e = launch_nhwc_to_frames(x_f16, 3 * n_px, frames_u8, static_cast<cudaStream_t>(stream));
   if (!e) g_launches += 1;
   return e;
+}
+
+int tf_resize_taps(int in, int out) {
+  if (!resize_sizes_ok(in, out, "tf_resize_taps")) return -1;
+  return resize_taps(in, out);
+}
+
+int tf_resize_coeffs(int in, int out, int32_t* bounds, int32_t* coeffs) {
+  if (!resize_sizes_ok(in, out, "tf_resize_coeffs")) return TF_ERR_INVALID_ARGUMENT;
+  if (!bounds || !coeffs) { set_last_error("tf_resize_coeffs: NULL table"); return TF_ERR_INVALID_ARGUMENT; }
+  resize_coeffs(in, out, bounds, coeffs);
+  return TF_OK;
+}
+
+int tf_resize_u8(const void* in, int64_t n, int h_in, int w_in, int h, int w, const int32_t* h_bounds,
+                 const int32_t* h_coeffs, int h_taps, const int32_t* v_bounds, const int32_t* v_coeffs, int v_taps,
+                 void* tmp, void* out, tf_stream_t stream) {
+  if (n < 0 || !resize_sizes_ok(w_in, w, "tf_resize_u8") || !resize_sizes_ok(h_in, h, "tf_resize_u8")) {
+    if (n < 0) set_last_error("tf_resize_u8: n=%lld", (long long)n);
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  const bool need_h = w != w_in, need_v = h != h_in;
+  if (need_h && h_taps != resize_taps(w_in, w)) {
+    set_last_error("tf_resize_u8: horizontal table of %d taps, %d -> %d has %d", h_taps, w_in, w, resize_taps(w_in, w));
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  if (need_v && v_taps != resize_taps(h_in, h)) {
+    set_last_error("tf_resize_u8: vertical table of %d taps, %d -> %d has %d", v_taps, h_in, h, resize_taps(h_in, h));
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  if (n == 0) return TF_OK;
+  if (!in || !out || (need_h && (!h_bounds || !h_coeffs)) || (need_v && (!v_bounds || !v_coeffs)) ||
+      (need_h && need_v && !tmp)) {
+    set_last_error("tf_resize_u8: NULL pointer");
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!need_h && !need_v)          // Pillow returns a copy when the size is unchanged
+    return check_cuda(cudaMemcpyAsync(out, in, (size_t)n * h * w * 3, cudaMemcpyDeviceToDevice, st), "tf_resize_u8 copy");
+  if (need_h) {
+    int e = launch_resize_h(in, n * h_in, w_in, w, h_bounds, h_coeffs, h_taps, need_v ? tmp : out, st);
+    if (e) return e;
+    g_launches += 1;
+  }
+  if (need_v) {
+    int e = launch_resize_v(need_h ? tmp : in, n, h_in, h, w, v_bounds, v_coeffs, v_taps, out, st);
+    if (e) return e;
+    g_launches += 1;
+  }
+  return TF_OK;
 }
 
 int tf_geglu(const void* xh, const void* gate, int64_t n, void* out, tf_stream_t stream) {

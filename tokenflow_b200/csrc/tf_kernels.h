@@ -42,6 +42,14 @@ int launch_geglu(const void* xh, const void* gate, long long n, void* out, cudaS
 int launch_frames_to_nhwc(const void* frames, long long n, void* out, cudaStream_t stream);
 int launch_nhwc_to_frames(const void* x, long long n, void* frames, cudaStream_t stream);
 
+// Pillow's LANCZOS resize of RGB uint8 frames (tf_resize.cu): host-side tables, then one launch per pass.
+int resize_taps(int in, int out);
+void resize_coeffs(int in, int out, int32_t* bounds, int32_t* coeffs);
+int launch_resize_h(const void* in, long long n_rows, int w_in, int w, const int32_t* bounds, const int32_t* coeffs,
+                    int taps, void* out, cudaStream_t stream);
+int launch_resize_v(const void* in, long long n, int h_in, int h, int w, const int32_t* bounds, const int32_t* coeffs,
+                    int taps, void* out, cudaStream_t stream);
+
 int launch_propagate(const void* A, const int32_t* idx_a, const int32_t* idx_b, const FrameTable& tab, int F,
                      int S, int dim, int K, const void* residual, void* out, int out_is_f32, long long F_total,
                      cudaStream_t stream);

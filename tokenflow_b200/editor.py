@@ -532,17 +532,18 @@ class TokenFlowEditor(nn.Module):
 # --------------------------------------------------------------------------------------------
 # synthetic inputs (SURVEY.md §8d): no SD weights / VAE / CLIP exist here
 # --------------------------------------------------------------------------------------------
-def synthetic_inputs(n_frames: int, latent_size: int, ctx_dim: int, n_timesteps: int, seed: int = 1,
+def synthetic_inputs(n_frames: int, latent_size, ctx_dim: int, n_timesteps: int, seed: int = 1,
                      device="cpu", dtype=torch.float32, ctx_len: int = 77):
-    """x ~ N(0,1) [N,4,L,L]; one source latent tensor per sampling timestep; text embeddings
-    ~ N(0,1).  Deterministic in `seed` and independent of device."""
+    """x ~ N(0,1) [N,4,h,w] (`latent_size` is h = w, or an (h, w) pair); one source latent tensor per sampling
+    timestep; text embeddings ~ N(0,1).  Deterministic in `seed` and independent of device."""
+    h, w = (latent_size, latent_size) if isinstance(latent_size, int) else tuple(latent_size)
     g = torch.Generator().manual_seed(seed)
-    x = torch.randn(n_frames, 4, latent_size, latent_size, generator=g)
+    x = torch.randn(n_frames, 4, h, w, generator=g)
     text = torch.randn(2, ctx_len, ctx_dim, generator=g)
     pnp = torch.randn(1, ctx_len, ctx_dim, generator=g)
     ratio = 1000 // n_timesteps
     timesteps = [(n_timesteps - 1 - i) * ratio + 1 for i in range(n_timesteps)]
-    src = {t: torch.randn(n_frames, 4, latent_size, latent_size, generator=g) for t in timesteps}
+    src = {t: torch.randn(n_frames, 4, h, w, generator=g) for t in timesteps}
     conv = lambda z: z.to(device=device, dtype=dtype)
     return conv(x), conv(text), conv(pnp), {t: conv(v) for t, v in src.items()}
 

@@ -68,6 +68,11 @@ _SIGNATURES = {
                                           ctypes.c_void_p, ctypes.c_void_p]),
     "tf_frames_to_nhwc": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
     "tf_nhwc_to_frames": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
+    "tf_resize_taps": (ctypes.c_int, [ctypes.c_int, ctypes.c_int]),
+    "tf_resize_coeffs": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "tf_resize_u8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                    ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
+                                    ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "tf_geglu": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
 }
 
@@ -477,6 +482,47 @@ class CudaOps:
         out = torch.empty((n, h, w, 3), dtype=torch.uint8, device=x.device)
         self._timed("tf_nhwc_to_frames", 3.0 * n * h * w, lambda: self._check(self.lib.tf_nhwc_to_frames(
             x.data_ptr(), n * h * w, out.data_ptr(), self._stream()), "tf_nhwc_to_frames"))
+        return out
+
+    def _resize_tables(self, n_in: int, n_out: int, device):
+        """Device (bounds, coeffs, taps) of one axis n_in -> n_out (tf_resize_coeffs), made once per pair and device."""
+        cache = self.__dict__.setdefault("_resize_cache", {})
+        key = (n_in, n_out, str(device))
+        if key not in cache:
+            taps = int(self.lib.tf_resize_taps(n_in, n_out))
+            if taps < 0:
+                self._check(1, "tf_resize_taps")
+            bounds = torch.empty((n_out, 2), dtype=torch.int32)
+            coeffs = torch.empty((n_out, taps), dtype=torch.int32)
+            self._check(self.lib.tf_resize_coeffs(n_in, n_out, bounds.data_ptr(), coeffs.data_ptr()), "tf_resize_coeffs")
+            cache[key] = (bounds.to(device), coeffs.to(device), taps)
+        return cache[key]
+
+    def resize_frames(self, frames: torch.Tensor, size: Tuple[int, int], tmp: Optional[torch.Tensor] = None,
+                      out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """uint8 RGB frames [N, H_in, W_in, 3] (CUDA) -> [N, H, W, 3] for size = (H, W), bit-equal to PIL's
+        `Image.resize((W, H), Image.LANCZOS)` of every frame.  `tmp` ([N, H_in, W, 3] uint8) and `out` may be given;
+        they are made here otherwise."""
+        assert frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[-1] == 3 and frames.is_cuda
+        frames = frames.contiguous()
+        n, h_in, w_in, _ = frames.shape
+        h, w = int(size[0]), int(size[1])
+        dev = frames.device
+        need_h, need_v = w != w_in, h != h_in
+        hb, hk, ht = self._resize_tables(w_in, w, dev) if need_h else (None, None, 0)
+        vb, vk, vt = self._resize_tables(h_in, h, dev) if need_v else (None, None, 0)
+        if out is None:
+            out = torch.empty((n, h, w, 3), dtype=torch.uint8, device=dev)
+        assert out.shape == (n, h, w, 3) and out.dtype == torch.uint8 and out.is_contiguous()
+        if need_h and need_v and tmp is None:
+            tmp = torch.empty((n, h_in, w, 3), dtype=torch.uint8, device=dev)
+        if tmp is not None:
+            assert tmp.numel() >= n * h_in * w * 3 and tmp.dtype == torch.uint8 and tmp.is_contiguous()
+        work = 3.0 * n * (h_in * w_in + (2 * h_in * w if need_h and need_v else 0) + h * w)
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        self._timed("tf_resize_u8", work, lambda: self._check(self.lib.tf_resize_u8(
+            frames.data_ptr(), n, h_in, w_in, h, w, ptr(hb), ptr(hk), ht, ptr(vb), ptr(vk), vt, ptr(tmp), out.data_ptr(),
+            self._stream()), "tf_resize_u8"))
         return out
 
     def geglu(self, xh: torch.Tensor, gate: torch.Tensor) -> torch.Tensor:

@@ -296,6 +296,27 @@ class LatentInverter:
         return self._gathered(self._run_steps(x_share, cond, batch_size, rec_coef, ts_dn_dev), x.shape[0])
 
 
+def resize_frames(frames_u8: torch.Tensor, size) -> torch.Tensor:
+    """uint8 RGB frames [N, H_in, W_in, 3] at their native size -> [N, H, W, 3], size = (H, W) or an int for a square:
+    PIL's `Image.resize((W, H), Image.LANCZOS)` of every frame, which is how the reference brings frames to the size
+    it edits at.  Its `save_video_frames` resizes every frame to the `--W x --H` it is given (util.py:28; preprocess.py
+    recommends 672 x 384 for landscape and 384 x 672 for portrait videos), and its drivers resize square frames to
+    512 x 512 (run_tokenflow_pnp.py:174-175, run_tokenflow_sdedit.py:136-137, preprocess.py:191-192).  Sides that
+    are multiples of 8 give latents of (H / 8, W / 8); the UNet takes any latent shape.
+
+    CUDA frames are resized on the device by `tf_resize_u8`, bit for bit PIL's result; CPU frames go through PIL
+    itself.  An unchanged size returns a copy, as PIL does."""
+    h, w = (size, size) if isinstance(size, int) else (int(size[0]), int(size[1]))
+    assert frames_u8.dtype == torch.uint8 and frames_u8.dim() == 4 and frames_u8.shape[-1] == 3
+    if frames_u8.is_cuda:
+        from . import ops as tf_ops
+        return tf_ops.default_ops().resize_frames(frames_u8, (h, w))
+    import numpy as np
+    from PIL import Image
+    return torch.from_numpy(np.stack([np.asarray(Image.fromarray(f).resize((w, h), Image.LANCZOS))
+                                      for f in frames_u8.contiguous().numpy()]))
+
+
 def _native_vae(vae) -> bool:
     p = next(vae.parameters())
     return p.is_cuda and p.dtype == torch.float16

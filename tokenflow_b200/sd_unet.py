@@ -284,8 +284,13 @@ class Upsample2D(nn.Module):
         super().__init__()
         self.conv = nn.Conv2d(channels, channels, 3, padding=1)
 
-    def forward(self, x):
-        return self.conv(F.interpolate(x, scale_factor=2.0, mode="nearest"))
+    def forward(self, x, output_size=None):
+        """Nearest-neighbour doubling, or nearest-neighbour to `output_size` (h, w): the size of the skip the next up
+        block concatenates, when a latent side is not a multiple of the UNet's overall downsampling (diffusers'
+        `upsample_size`)."""
+        if output_size is None:
+            return self.conv(F.interpolate(x, scale_factor=2.0, mode="nearest"))
+        return self.conv(F.interpolate(x, size=output_size, mode="nearest"))
 
 
 class CrossAttnDownBlock2D(nn.Module):
@@ -346,11 +351,11 @@ class UpBlock2D(nn.Module):
         self.resnets = nn.ModuleList(res)
         self.upsamplers = nn.ModuleList([Upsample2D(cout)]) if add_upsample else None
 
-    def forward(self, x, skips, temb, ctx=None):
+    def forward(self, x, skips, temb, ctx=None, upsample_size=None):
         for r in self.resnets:
             x = r(torch.cat([x, skips.pop()], dim=1), temb)
         if self.upsamplers is not None:
-            x = self.upsamplers[0](x)
+            x = self.upsamplers[0](x, upsample_size)
         return x
 
 
@@ -366,12 +371,12 @@ class CrossAttnUpBlock2D(nn.Module):
         self.attentions = nn.ModuleList([Transformer2DModel(cout, heads, ctx, groups, linear_proj) for _ in range(layers)])
         self.upsamplers = nn.ModuleList([Upsample2D(cout)]) if add_upsample else None
 
-    def forward(self, x, skips, temb, ctx):
+    def forward(self, x, skips, temb, ctx, upsample_size=None):
         for r, a in zip(self.resnets, self.attentions):
             x = r(torch.cat([x, skips.pop()], dim=1), temb)
             x = a(x, encoder_hidden_states=ctx)
         if self.upsamplers is not None:
-            x = self.upsamplers[0](x)
+            x = self.upsamplers[0](x, upsample_size)
         return x
 
 
@@ -452,8 +457,16 @@ class UNet2DConditionModel(nn.Module):
             x, outs = blk(x, emb, encoder_hidden_states)
             skips.extend(outs)
         x = self.mid_block(x, emb, encoder_hidden_states)
+        # diffusers' rule for latents whose sides are not multiples of 2 ** (number of upsamplers): every up block but
+        # the last upsamples to the size of the skip it will concatenate next (a plain doubling would give 22 rows
+        # where the skip has 21); other latents keep the doubling
+        factor = 2 ** sum(b.upsamplers is not None for b in self.up_blocks)
+        ragged = any(s % factor for s in sample.shape[-2:])
         for blk in self.up_blocks:
-            x = blk(x, skips, emb, encoder_hidden_states)
+            size = None
+            if ragged and blk.upsamplers is not None:
+                size = skips[-len(blk.resnets) - 1].shape[-2:]
+            x = blk(x, skips, emb, encoder_hidden_states, upsample_size=size)
         x = self.conv_out(norm_act(self.conv_norm_out, x))          # conv_norm_out + conv_act (SiLU)
         return UNetOutput(sample=x)
 
