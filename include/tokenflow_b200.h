@@ -102,21 +102,15 @@ int tf_propagate(const void* A, const int32_t* idx_a, const int32_t* idx_b, cons
 int tf_ext_attn_fwd(const void* q, const void* k, const void* v, int64_t tok_stride, int n_frames, int S,
                     int heads, int d, float scale, int inject, void* out, tf_stream_t stream);
 
-/* General form used when the pivotal pass is sharded across GPUs: `n_out` output samples, each
- * described by host arrays (all length n_out): which slab of `out` it writes, which slab of q it
- * reads, the first k / v slab it attends to and how many consecutive slabs (1 = own frame, n = all
- * keyframes).  q has q_slabs slabs of [S, heads, d]; k and v have kv_slabs. */
-int tf_ext_attn_fwd_table(const void* q, int q_slabs, int64_t q_tok_stride, const void* k, const void* v,
-                          int kv_slabs, int64_t kv_tok_stride, int n_out, const int32_t* out_slab,
-                          const int32_t* q_slab, const int32_t* k_slab0, const int32_t* v_slab0,
-                          const int32_t* n_kv, int S, int heads, int d, float scale, void* out,
-                          tf_stream_t stream);
-
-/* The same for a RANGE of query tokens: only queries [q_row0, q_row0 + q_nrows) of every sample are computed
- * (against all keys), and `out` is [slabs, q_nrows, heads*d] with row = token - q_row0.  q_row0 must be a
- * multiple of 128.  The multi-GPU pivotal pass splits the query rows of ALL samples evenly over the ranks this
- * way (every rank holds all K/V after the all-gather), which balances the attention work exactly and keeps
- * paired (q/k-injected) samples together. */
+/* General form: `n_out` output samples, each described by host arrays (all length n_out): which slab
+ * of `out` it writes, which slab of q it reads, the first k / v slab it attends to and how many
+ * consecutive slabs (1 = own frame, n = all keyframes).  q has q_slabs slabs of [S, heads, d]; k and
+ * v have kv_slabs.  Only queries [q_row0, q_row0 + q_nrows) of every sample are computed (against all
+ * keys), and `out` is [slabs, q_nrows, heads*d] with row = token - q_row0; q_row0 = 0, q_nrows = S is
+ * the whole pass.  q_row0 must be a multiple of 128.  The multi-GPU pivotal pass splits the query
+ * rows of ALL samples evenly over the ranks this way (every rank holds all K/V after the
+ * all-gather), which balances the attention work exactly and keeps paired (q/k-injected) samples
+ * together. */
 int tf_ext_attn_fwd_rows(const void* q, int q_slabs, int64_t q_tok_stride, const void* k, const void* v,
                          int kv_slabs, int64_t kv_tok_stride, int n_out, const int32_t* out_slab,
                          const int32_t* q_slab, const int32_t* k_slab0, const int32_t* v_slab0,

@@ -1,7 +1,6 @@
 """GPU tier (-m gpu): the inversion stage on the H100 — tf_ddim against the reference's expression, the graphed path
-against its eager form and against the reference's loop (oracle/inversion.py), the native per-sample self-attention
-on real activations, the in-memory hand-off to the editor, and two ranks against one."""
-import copy
+against its eager form and against the reference's loop (oracle/inversion.py), the in-memory hand-off to the editor,
+and two ranks against one."""
 import os
 import socket
 import subprocess
@@ -11,8 +10,7 @@ import pytest
 import torch
 
 from oracle import inversion as OI
-from oracle.kernel_checks import check_ext_attn
-from tokenflow_b200 import preprocess, sd_unet
+from tokenflow_b200 import sd_unet
 from tokenflow_b200 import tokenflow_utils as tfu
 from tokenflow_b200.editor import TokenFlowEditor
 from tokenflow_b200.preprocess import LatentInverter, inversion_coef_tables
@@ -40,10 +38,6 @@ def _inputs(n, latent, ctx, seed=3):
     x0 = torch.randn(n, 4, latent, latent, generator=g).half().cuda()
     cond = torch.randn(1, 77, ctx, generator=g).half().cuda()
     return x0, cond
-
-
-def _rel(a, b):
-    return ((a.double() - b.double()).norm() / b.double().norm()).item()
 
 
 # ------------------------------------------------------------------------------------------------
@@ -78,9 +72,7 @@ def test_ddim_equals_the_reference_expression(ops, direction, case):
 # ------------------------------------------------------------------------------------------------
 # 2. graph replay == the same device path run eagerly
 # ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("native", [False, True])
-def test_graph_replay_equals_eager(ops, sd15, monkeypatch, native):
-    monkeypatch.setattr(preprocess, "_NATIVE_ATTN1", native)
+def test_graph_replay_equals_eager(ops, sd15):
     x0, cond = _inputs(4, 64, sd15.config.cross_attention_dim)
     res = {}
     for graphed in (True, False):
@@ -94,15 +86,12 @@ def test_graph_replay_equals_eager(ops, sd15, monkeypatch, native):
     assert sorted(res[True][2]) == sorted(res[False][2])
     for t in res[True][2]:
         assert torch.equal(res[True][2][t], res[False][2][t]), t
-    assert all(not hasattr(m.attn1, "_tf_plain_prev") and "forward" not in m.attn1.__dict__
-               for m in tfu._transformer_blocks(sd15))                 # the hook is gone after the call
 
 
 # ------------------------------------------------------------------------------------------------
 # 3. the whole inversion against the reference's loop
 # ------------------------------------------------------------------------------------------------
-def test_sdpa_route_equals_the_reference_loop(ops, sd15, monkeypatch):
-    monkeypatch.setattr(preprocess, "_NATIVE_ATTN1", False)
+def test_sdpa_route_equals_the_reference_loop(ops, sd15):
     x0, cond = _inputs(4, 64, sd15.config.cross_attention_dim)
     inv = LatentInverter(sd15, DDIMScheduler(), 10)
     ts_up = [int(t) for t in reversed(inv.scheduler.timesteps.tolist())]
@@ -118,60 +107,8 @@ def test_sdpa_route_equals_the_reference_loop(ops, sd15, monkeypatch):
     assert torch.equal(rec, want_rec), (rec.float() - want_rec.float()).abs().max().item()
 
 
-def test_native_route_is_as_close_to_fp32_as_the_reference_loop(ops, sd15, monkeypatch):
-    """After 20 inversion steps at 8 frames: rel-L2 of the path with native attn1 from an fp32 run of the same weights
-    is at most 1.1x that of the reference's fp16 loop (SDPA attn1)."""
-    monkeypatch.setattr(preprocess, "_NATIVE_ATTN1", True)
-    x0, cond = _inputs(8, 64, sd15.config.cross_attention_dim, seed=5)
-    inv = LatentInverter(sd15, DDIMScheduler(), 20)
-    got = inv.ddim_inversion(cond, x0, None, batch_size=8).float()
-    fp16_ref, _ = OI.ddim_inversion(sd15, inv.scheduler, cond, x0.clone(), 8)
-    unet32 = copy.deepcopy(sd15).float()
-    fp32_ref, _ = OI.ddim_inversion(unet32, inv.scheduler, cond.float(), x0.float(), 8)
-    del unet32
-    ours, theirs = _rel(got, fp32_ref), _rel(fp16_ref.float(), fp32_ref)
-    print(f"rel-L2 to fp32 after 20 steps: native {ours:.4g}, reference fp16 loop {theirs:.4g}")
-    assert torch.isfinite(got).all() and ours <= 1.1 * theirs, (ours, theirs)
-
-
 # ------------------------------------------------------------------------------------------------
-# 4. the native self-attention of every block, on the q/k/v the hook hands the kernel
-# ------------------------------------------------------------------------------------------------
-class _Recorder:
-    def __init__(self, inner):
-        self.inner, self.calls = inner, []
-
-    def __getattr__(self, name):
-        return getattr(self.inner, name)
-
-    def ext_attn_table(self, q, k, v, table, heads, scale, row0=0, nrows=None):
-        out = self.inner.ext_attn_table(q, k, v, table, heads, scale, row0, nrows)
-        self.calls.append((q, k, v, list(table), heads, scale, out))
-        return out
-
-
-@pytest.mark.parametrize("kind,latent", [("sd15", 64), ("sd21", 96)])
-def test_native_self_attention_per_block(ops, sd15, kind, latent):
-    unet = sd15 if kind == "sd15" else sd_unet.build_unet(
-        "sd21", seed=1, device="cuda", dtype=torch.float16, init_on_device=True).to(memory_format=torch.channels_last)
-    x0, cond = _inputs(2, latent, unet.config.cross_attention_dim, seed=7)
-    rec = _Recorder(ops)
-    tfu._install_ops_for_testing(rec)
-    tfu.register_native_self_attention(unet)
-    try:
-        with torch.no_grad():
-            unet(x0, torch.tensor(501, device="cuda"), encoder_hidden_states=cond.repeat(2, 1, 1))
-    finally:
-        tfu.remove_native_self_attention(unet)
-        tfu._install_ops_for_testing(None)
-    assert len(rec.calls) == 16                                          # one per transformer block, attn2 untouched
-    for q, k, v, table, heads, scale, out in rec.calls:
-        assert table == [(0, 0, 0, 1), (1, 1, 1, 1)]
-        check_ext_attn(out, q, k, v, table, heads, scale, rtol=2e-3)
-
-
-# ------------------------------------------------------------------------------------------------
-# 5. hand-off: files and saved_latents() feed the same edit
+# 4. hand-off: files and saved_latents() feed the same edit
 # ------------------------------------------------------------------------------------------------
 def test_in_memory_hand_off_equals_the_files(ops, tmp_path):
     steps, n = 4, 4
@@ -203,7 +140,7 @@ def test_in_memory_hand_off_equals_the_files(ops, tmp_path):
 
 
 # ------------------------------------------------------------------------------------------------
-# 6. two ranks over tf_allgather == one rank  (skipped with fewer than two GPUs)
+# 5. two ranks over tf_allgather == one rank  (skipped with fewer than two GPUs)
 # ------------------------------------------------------------------------------------------------
 _WORKER = r"""
 import os, sys, json, torch

@@ -107,7 +107,7 @@ def test_keyframe_generator_is_rank_independent_and_checked():
     eds = []
     for r in range(2):
         unet = sd_unet.build_unet("tiny", seed=1)
-        cfg = {"n_frames": 8, "batch_size": 2, "n_timesteps": 4, "guidance_scale": 7.5, "mode": "pnp"}
+        cfg = {"n_frames": 8, "batch_size": 2, "n_timesteps": 4, "guidance_scale": 7.5, "mode": "pnp", "fused_pass": True}
         x, text, pnp, src = synthetic_inputs(8, 16, unet.config.cross_attention_dim, 4, seed=1, ctx_len=7)
         eds.append(TokenFlowEditor(unet, DDIMScheduler(), tfu, cfg, text, pnp, source_latents=lambda t: src[t],
                                    world_size=2, rank=r))
@@ -117,6 +117,30 @@ def test_keyframe_generator_is_rank_independent_and_checked():
     assert draws[0] == draws[1]
     for d in draws[0]:
         assert all(2 * i <= k < 2 * i + 2 for i, k in enumerate(d))      # one frame inside every batch
+
+
+def test_constructor_refuses_schedules_that_do_not_exist():
+    """A step runs one way: no dual-stream schedule, and several ranks only with the fused step.  Asking for anything
+    else fails in the constructor instead of running another schedule under its name."""
+    unet = sd_unet.build_unet("tiny", seed=1)
+    x, text, pnp, src = synthetic_inputs(8, 16, unet.config.cross_attention_dim, 4, seed=1, ctx_len=7)
+    base = {"n_frames": 8, "batch_size": 2, "n_timesteps": 4, "guidance_scale": 7.5, "mode": "pnp"}
+
+    def make(cfg, world):
+        return TokenFlowEditor(unet, DDIMScheduler(), tfu, dict(base, **cfg), text, pnp,
+                               source_latents=lambda t: src[t], world_size=world, rank=0)
+    for world in (1, 2):
+        with pytest.raises(ValueError, match="dual_stream"):
+            make({"dual_stream": True, "fused_pass": True}, world)
+    for cfg in ({}, {"fused_pass": False}, {"fused_pass": False, "dual_stream": None}):
+        with pytest.raises(ValueError, match="fused_pass"):
+            make(cfg, 2)
+    tfu._install_ops_for_testing(OracleOps())
+    for dual in (None, False):
+        ed = make({"dual_stream": dual, "fused_pass": True}, 2)
+        ed.init_method()
+        assert ed.world_size == 2 and ed.config["fused_pass"]
+        assert make({"dual_stream": dual, "fused_pass": False}, 1).world_size == 1
 
 
 def test_register_fused_and_shard_reach_the_conv_site_from_the_unet_itself():

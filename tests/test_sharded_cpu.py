@@ -1,6 +1,6 @@
-"""CPU tier: the multi-GPU path (frames sharded, keyframe tensors all-gathered) on 2 gloo ranks with
-the oracle ops == the single-process loop.  Covers the shard plan, the all-gather ordering and routing,
-the per-frame keyframe/weight tables and the sharded attention table."""
+"""CPU tier: the multi-GPU path (the fused step: frames sharded, keyframe tensors all-gathered) on 2 gloo
+ranks with the oracle ops == the single-process loop of the reference's schedule.  Covers the shard plan, the
+all-gather ordering and routing, the per-frame keyframe/weight tables and the sharded attention table."""
 import os
 
 import pytest
@@ -37,11 +37,11 @@ def _edit(world, rank, mode, steps, fused=False):
     return ed.sample_loop(x), ed.keyframe_log
 
 
-def _worker(rank, world, rdzv, mode, steps, q, fused=False):
+def _worker(rank, world, rdzv, mode, steps, q):
     torch.set_num_threads(2)
     dist.init_process_group("gloo", init_method=f"file://{rdzv}", rank=rank, world_size=world)
     try:
-        out, kf = _edit(world, rank, mode, steps, fused)
+        out, kf = _edit(world, rank, mode, steps, fused=True)
         # plain Python data on the queue: a torch tensor would travel by file-descriptor passing, which needs
         # the sender alive until the parent has rebuilt it (the worker exits right after the put)
         q.put((rank, out.numpy().tolist(), kf))
@@ -49,14 +49,13 @@ def _worker(rank, world, rdzv, mode, steps, q, fused=False):
         dist.destroy_process_group()
 
 
-@pytest.mark.parametrize("mode,steps,fused", [("pnp", 2, False), ("sdedit", 10, False), ("pnp", 2, True),
-                                              ("sdedit", 10, True)])
-def test_two_rank_edit_equals_single_process(mode, steps, fused):
+@pytest.mark.parametrize("mode,steps", [("pnp", 2), ("sdedit", 10)])
+def test_two_rank_edit_equals_single_process(mode, steps):
     want, kf_want = _edit(1, 0, mode, steps)
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     rdzv = _init_file()
-    procs = [ctx.Process(target=_worker, args=(r, 2, rdzv, mode, steps, q, fused)) for r in range(2)]
+    procs = [ctx.Process(target=_worker, args=(r, 2, rdzv, mode, steps, q)) for r in range(2)]
     for p in procs:
         p.start()
     results = [q.get(timeout=300) for _ in procs]

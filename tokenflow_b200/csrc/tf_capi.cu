@@ -120,7 +120,7 @@ using namespace tf;
 
 extern "C" {
 
-int tf_version(void) { return 1001; }
+int tf_version(void) { return 1002; }
 
 const char* tf_last_error(void) { return g_err; }
 
@@ -503,15 +503,6 @@ int tf_ext_attn_fwd_rows(const void* q, int q_slabs, int64_t q_tok_stride, const
   return TF_OK;
 }
 
-int tf_ext_attn_fwd_table(const void* q, int q_slabs, int64_t q_tok_stride, const void* k, const void* v,
-                          int kv_slabs, int64_t kv_tok_stride, int n_out, const int32_t* out_slab,
-                          const int32_t* q_slab, const int32_t* k_slab0, const int32_t* v_slab0,
-                          const int32_t* n_kv, int S, int heads, int d, float scale, void* out,
-                          tf_stream_t stream) {
-  return tf_ext_attn_fwd_rows(q, q_slabs, q_tok_stride, k, v, kv_slabs, kv_tok_stride, n_out, out_slab, q_slab, k_slab0,
-                              v_slab0, n_kv, S, heads, d, scale, 0, S, out, stream);
-}
-
 int tf_ext_attn_fwd(const void* q, const void* k, const void* v, int64_t tok_stride, int n_frames, int S,
                     int heads, int d, float scale, int inject, void* out, tf_stream_t stream) {
   const int n = n_frames;
@@ -534,8 +525,8 @@ int tf_ext_attn_fwd(const void* q, const void* k, const void* v, int64_t tok_str
       }
     }
   }
-  return tf_ext_attn_fwd_table(q, 3 * n, tok_stride, k, v, 3 * n, tok_stride, 3 * n, out_slab.data(), q_slab.data(),
-                               k0.data(), v0.data(), nkv.data(), S, heads, d, scale, out, stream);
+  return tf_ext_attn_fwd_rows(q, 3 * n, tok_stride, k, v, 3 * n, tok_stride, 3 * n, out_slab.data(), q_slab.data(),
+                              k0.data(), v0.data(), nkv.data(), S, heads, d, scale, 0, S, out, stream);
 }
 
 }  // extern "C"

@@ -38,6 +38,12 @@ class TokenFlowEditor(nn.Module):
         self.scheduler = scheduler
         self.hooks = hooks
         self.config = dict(config)
+        if self.config.get("dual_stream"):
+            raise ValueError("config['dual_stream'] is not supported: a step runs as one fused UNet call on one stream "
+                             "(config['fused_pass'])")
+        if world_size > 1 and not self.config.get("fused_pass", False):
+            raise ValueError(f"world_size = {world_size} needs config['fused_pass']: the fused step is the only "
+                             "multi-rank schedule")
         self.text_embeds = text_embeds
         self.pnp_guidance_embeds = pnp_guidance_embeds
         self.latents_path = self.config.get("latents_path")
@@ -72,7 +78,6 @@ class TokenFlowEditor(nn.Module):
         self._g_static = None
         self._text_cache = {}
         self._shard_cache = {}
-        self._side_stream = None
 
     # ------------------------------------------------------------------------------------
     def init_method(self):
@@ -152,16 +157,14 @@ class TokenFlowEditor(nn.Module):
         self.comm = comm
 
     def batched_denoise_step(self, x, t, indices):
-        """run_tokenflow_pnp.py:220-233 (one process), or its frame-sharded form (world_size > 1).
-        With config["fused_pass"] the pivotal samples and the frame samples go through the UNet in ONE
-        call (the keyframe caches a block fills from the first part of the batch are consumed by the
-        second part inside the same block) — identical arithmetic, half the kernel launches."""
+        """run_tokenflow_pnp.py:220-233.  With config["fused_pass"] the pivotal samples and the frame samples go
+        through the UNet in ONE call (the keyframe caches a block fills from the first part of the batch are consumed
+        by the second part inside the same block) — identical arithmetic, half the kernel launches; this is also the
+        only multi-rank form.  Otherwise the reference's schedule on one rank: the pivotal pass, then a frame pass per
+        batch or per config["frames_per_pass"] frames."""
         if self.config.get("fused_pass", False):
             with self._autocast():
                 return self._fused_step(x, t, indices)
-        if self.world_size > 1:
-            with self._autocast():
-                return self._sharded_step(x, t, indices)
         h = self.hooks
         batch_size = self.config["batch_size"]
         with self._autocast():
@@ -186,9 +189,6 @@ class TokenFlowEditor(nn.Module):
                 denoised.append(self.denoise_step(x[b:b + per_pass], t, indices[b:b + per_pass]))
             return torch.cat(denoised)
 
-    # ------------------------------------------------------------------------------------
-    # multi-GPU: one process per GPU, frames sharded, keyframe tensors all-gathered (SURVEY.md §8e)
-    # ------------------------------------------------------------------------------------
     def frame_table(self, frames):
         """Per-frame (keyframe, previous keyframe, blend weight) for global frame ids — the reference's
         batch_idx arithmetic (tokenflow_utils.py:331-333, :375-383) evaluated per frame."""
@@ -198,43 +198,6 @@ class TokenFlowEditor(nn.Module):
         kf_a = [g // B for g in frames]
         kf_b = [(g // B) - 1 if g >= B else -1 for g in frames]
         return kf_a, kf_b, [w[g % B] for g in frames]
-
-    @torch.no_grad()
-    def _sharded_step(self, x, t, indices):
-        h, G, r = self.hooks, self.world_size, self.rank
-        N, B = len(x), self.config["batch_size"]
-        K = N // B
-        assert N % G == 0, "frames must divide evenly over the ranks"
-        pivotal_idx = self.draw_keyframes(N)                  # same CPU seed on every rank -> same keyframes
-        self.keyframe_log.append(pivotal_idx.tolist())
-        src_all = self.source_latents_t(int(t))[indices].to(x.device, x.dtype)
-        h.register_time(self, int(t))
-        # ---- pivotal pass: this rank's m of the 3K (stream, keyframe) samples ----
-        shard = h.PivotalShard(G, r, K, self.group, comm=self.comm)
-        lat, emb = [], []
-        for i in shard.slots:
-            i = min(i, 3 * K - 1)                             # padding slots recompute the last sample
-            s, f = divmod(i, K)
-            frame = int(pivotal_idx[f])
-            lat.append(src_all[frame] if s == 0 else x[frame])
-            emb.append(self.pnp_guidance_embeds[0] if s == 0 else self.text_embeds[s - 1])
-        h.register_shard(self, shard)
-        h.register_pivotal(self, True)
-        self.unet(torch.stack(lat), t, encoder_hidden_states=torch.stack(emb))
-        h.register_pivotal(self, False)
-        h.register_shard(self, None)
-        # ---- frame pass: this rank's contiguous frames, per-frame keyframe table ----
-        per = N // G
-        frames = list(range(r * per, (r + 1) * per))
-        h.register_frame_table(self, *self.frame_table(frames))
-        xs = x[frames[0]:frames[-1] + 1]
-        latent_model_input = torch.cat([src_all[frames[0]:frames[-1] + 1], xs, xs])
-        text = torch.cat([self.pnp_guidance_embeds.repeat(per, 1, 1), torch.repeat_interleave(self.text_embeds, per, dim=0)])
-        noise_pred = self.unet(latent_model_input, t, encoder_hidden_states=text)['sample']
-        _, npu, npc = noise_pred.chunk(3)
-        noise_pred = npu + self.config["guidance_scale"] * (npc - npu)
-        x_local = self.scheduler.step(noise_pred, t, xs)['prev_sample'].contiguous()
-        return all_gather(x_local, G, self.group, self.comm)
 
     def _timestep_pair(self, t):
         """(host int, device scalar) of a timestep without reading the device when `t` is a host value."""
@@ -301,50 +264,7 @@ class TokenFlowEditor(nn.Module):
         finally:
             h.register_fused(self, 0)
             h.register_shard(self, None)
-        return self._update_and_gather(noise_pred, xs, coef, t_int)
-
-    def _dual_compute(self, x, src_all, piv_idx, t_dev, t_int, coef, slots, shard):
-        """The same step as `_fused_compute` as TWO UNet calls on two CUDA streams: the pivotal samples (few, and all
-        the collectives when sharded) on a side stream, this rank's frames on the current stream; each TokenFlow block
-        of the frame call waits for the event its pivotal counterpart recorded (`register_dual_stream`).  The pivotal
-        chain — latency-bound small kernels plus the all-gathers — then runs under the frame chain's compute."""
-        h, G, r = self.hooks, self.world_size, self.rank
-        N = x.shape[0]
-        per = N // G
-        lo = r * per
-        main = torch.cuda.current_stream()
-        if self._side_stream is None:
-            self._side_stream = torch.cuda.Stream(device=self.device)
-        side = self._side_stream
-        piv_lat = torch.cat([src_all, x]).index_select(0, piv_idx)
-        text = self._fused_text(slots, per)
-        n_piv = len(slots)
-        piv_emb, frame_emb = text[:n_piv], text[n_piv:]
-        xs, srcs = x[lo:lo + per], src_all[lo:lo + per]
-        frame_in = torch.cat([srcs, xs, xs])
-        h.register_time(self, t_int)
-        h.register_fused(self, 0)
-        h.register_dual_stream(self, True)
-        try:
-            side.wait_stream(main)
-            with torch.cuda.stream(side):                    # ---- pivotal chain
-                h.register_pivotal(self, True)
-                h.register_shard(self, shard)
-                self.unet(piv_lat, t_dev, encoder_hidden_states=piv_emb)
-            h.register_pivotal(self, False)                  # ---- frame chain
-            h.register_shard(self, None)
-            h.register_frame_table(self, *self.frame_table(list(range(lo, lo + per))))
-            noise_pred = self.unet(frame_in, t_dev, encoder_hidden_states=frame_emb)['sample']
-            main.wait_stream(side)                           # join (piv_lat and the caches stay referenced until here)
-        finally:
-            h.register_dual_stream(self, False)
-            h.register_shard(self, None)
-        del piv_lat
-        return self._update_and_gather(noise_pred, xs, coef, t_int)
-
-    def _update_and_gather(self, noise_pred, xs, coef, t_int):
-        """Tail of a fused step: classifier-free guidance + DDIM update of this rank's frames `xs` from their
-        [source | uncond | cond] noise predictions, then the all-gather of every rank's frames."""
+        # classifier-free guidance + DDIM update of this rank's frames, then the all-gather of every rank's frames
         _, npu, npc = noise_pred.chunk(3)
         ops = self._cuda_ops()
         if ops is not None and coef is not None and npu.dtype == torch.float16 and xs.dtype == torch.float16:
@@ -352,16 +272,7 @@ class TokenFlowEditor(nn.Module):
         else:
             noise_pred = npu + self.config["guidance_scale"] * (npc - npu)
             x_local = self.scheduler.step(noise_pred, t_int, xs)['prev_sample'].contiguous()
-        return all_gather(x_local, self.world_size, self.group, self.comm)
-
-    def _step_compute(self, *a):
-        # Off unless asked for: on one GPU the concurrent chains slow each other down, and with real NCCL ranks this
-        # schedule has not been run to completion — only its single-process forms are verified
-        # (tests/test_gpu_round2.py).
-        dual = bool(self.config.get("dual_stream", False))
-        if dual and self.device.type == "cuda":
-            return self._dual_compute(*a)
-        return self._fused_compute(*a)
+        return all_gather(x_local, G, self.group, self.comm)
 
     def _cuda_ops(self):
         """The CUDA op object if the hooks run on it (None under the oracle test seam / on CPU)."""
@@ -405,7 +316,7 @@ class TokenFlowEditor(nn.Module):
         if self.config.get("cuda_graph", False) and self.device.type == "cuda" and coef is not None:
             return self._graph_replay(x, src_all, idx_host, t_int, i, slots, shard)
         piv_idx = idx_host.to(x.device, non_blocking=True) if x.is_cuda else idx_host
-        return self._step_compute(x, src_all, piv_idx, t_dev, t_int, coef, slots, shard)
+        return self._fused_compute(x, src_all, piv_idx, t_dev, t_int, coef, slots, shard)
 
     # ------------------------------------------------------------------------------------
     # CUDA graphs (SURVEY.md §8 f-2): the fused step's shape is static, so it is captured once per injection
@@ -440,7 +351,7 @@ class TokenFlowEditor(nn.Module):
 
     def _capture(self, st, t_int, slots, shard):
         ops = self._cuda_ops()
-        run = lambda: self._step_compute(st["x"], st["src"], st["idx"], st["t"], t_int, st["coef"], slots, shard)
+        run = lambda: self._fused_compute(st["x"], st["src"], st["idx"], st["t"], t_int, st["coef"], slots, shard)
         # warm-up on a side stream (cuDNN autotuning, lazy initialisation, allocator growth) — not captured
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())

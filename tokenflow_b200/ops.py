@@ -57,10 +57,6 @@ _SIGNATURES = {
                                             _c_i32p, _c_i32p, _c_i32p, _c_i32p, ctypes.c_int, ctypes.c_int,
                                             ctypes.c_int, ctypes.c_float, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                             ctypes.c_void_p]),
-    "tf_ext_attn_fwd_table": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_void_p,
-                                             ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_int, _c_i32p,
-                                             _c_i32p, _c_i32p, _c_i32p, _c_i32p, ctypes.c_int, ctypes.c_int,
-                                             ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]),
     "tf_group_norm_nhwc_workspace": (ctypes.c_int64, [ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int]),
     "tf_group_norm_nhwc": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int,

@@ -29,13 +29,6 @@ import torch
 
 from .ops import all_gather
 
-# Which attn1 the graphed path runs: the module's own SDPA forward (False) or the native per-sample attention of
-# `tokenflow_utils.register_native_self_attention`, installed for the duration of the call (True).  SDPA stays: on an
-# H100 80GB HBM3 at a 400 W power limit the native route made the C2 inversion step slower, 132.2 ms against 124.2 ms
-# (tools/invert_bench.py, README.md).  A test seam for that script and the GPU tests, which time and check both
-# routes; not a user option.
-_NATIVE_ATTN1 = False
-
 
 def inversion_coef_tables(scheduler) -> Tuple[torch.Tensor, torch.Tensor]:
     """fp32 [steps, 4] coefficient rows (s1, inv_s2, s3, s4) of `tf_ddim` for every step of the inversion (ascending
@@ -83,7 +76,7 @@ class LatentInverter:
         self.world_size, self.rank, self.group = world_size, rank, group
         self.comm = None                      # ops.Communicator (C-ABI NCCL all-gather), see attach_communicator
         self._saved: Dict[int, torch.Tensor] = {}
-        self._graphs = {}                     # (share shape, batch size, cond shape, attn1 route) -> captured step
+        self._graphs = {}                     # (share shape, batch size, cond shape) -> captured step
         self._graph_pool = None
         self._tables = None
         self._use_graph = True                # test seam: False runs the same device path eagerly
@@ -192,7 +185,7 @@ class LatentInverter:
         from . import tokenflow_utils as tfu
         ops = tfu._ops()                      # the library is required: raises without it or without an H100
         bs = max(1, min(batch_size, share))
-        key = (share, tuple(shape), bs, tuple(cond.shape[1:]), _NATIVE_ATTN1, self._use_graph)
+        key = (share, tuple(shape), bs, tuple(cond.shape[1:]), self._use_graph)
         entry = self._graphs.get(key)
         if entry is not None:
             entry["cond"].copy_(cond.expand(bs, -1, -1))
@@ -237,30 +230,22 @@ class LatentInverter:
                    save_slots: Optional[Dict[int, int]] = None, saved: Optional[torch.Tensor] = None):
         """All steps of one direction over this rank's share: per step, refresh the timestep and the coefficient row,
         replay, and copy the latents of a saved step into its slot of `saved`.  Returns the share's final latents."""
-        from . import tokenflow_utils as tfu
         share = x_share.shape[0]
         if share == 0:
             return x_share
-        native = _NATIVE_ATTN1
-        if native:
-            tfu.register_native_self_attention(self.unet)
-        try:
-            entry = self._step_runner(share, x_share.shape[1:], batch_size, cond)
-            st = entry["st"]
-            st["x"].copy_(x_share)
-            for i in range(coef.shape[0]):
-                st["t"].copy_(ts[i])
-                st["coef"].copy_(coef[i])
-                if entry["graph"] is not None:
-                    entry["graph"].replay()
-                else:
-                    entry["step"]()
-                if save_slots is not None and i in save_slots:
-                    saved[save_slots[i], :share].copy_(st["x"])
-            return st["x"].clone()
-        finally:
-            if native:
-                tfu.remove_native_self_attention(self.unet)
+        entry = self._step_runner(share, x_share.shape[1:], batch_size, cond)
+        st = entry["st"]
+        st["x"].copy_(x_share)
+        for i in range(coef.shape[0]):
+            st["t"].copy_(ts[i])
+            st["coef"].copy_(coef[i])
+            if entry["graph"] is not None:
+                entry["graph"].replay()
+            else:
+                entry["step"]()
+            if save_slots is not None and i in save_slots:
+                saved[save_slots[i], :share].copy_(st["x"])
+        return st["x"].clone()
 
     def _share(self, frames: torch.Tensor) -> Tuple[torch.Tensor, int]:
         n = frames.shape[0]

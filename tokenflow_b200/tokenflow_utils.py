@@ -38,10 +38,10 @@ from .util import isinstance_str, batch_cosine_sim  # noqa: F401  (re-exported l
 
 __all__ = [
     "register_pivotal", "register_batch_idx", "register_frame_table", "register_shard", "register_fused",
-    "PivotalShard", "set_strict_dtype", "register_dual_stream",
+    "PivotalShard", "set_strict_dtype",
     "register_time", "load_source_latents_t",
     "register_conv_injection", "register_extended_attention_pnp", "register_extended_attention",
-    "register_native_self_attention", "remove_native_self_attention", "make_tokenflow_attention_block", "set_tokenflow", "isinstance_str", "batch_cosine_sim",
+    "make_tokenflow_attention_block", "set_tokenflow", "isinstance_str", "batch_cosine_sim",
 ]
 
 # --------------------------------------------------------------------------------------------
@@ -138,7 +138,6 @@ class PivotalShard:
         self.comm = comm                      # ops.Communicator (tf_allgather through the C ABI) or None
         self.m = -(-3 * n_keyframes // world_size)
         self.slots = list(range(rank * self.m, (rank + 1) * self.m))     # global sample ids (>= 3K: padding)
-        self.n_collectives = 0
         self._src_index = {}
 
     def source_index(self, device) -> torch.Tensor:
@@ -153,7 +152,6 @@ class PivotalShard:
         return idx
 
     def all_gather(self, t: torch.Tensor) -> torch.Tensor:
-        self.n_collectives += 1
         return tf_ops.all_gather(t, self.world_size, self.group, self.comm)
 
     def row_split(self, S: int):
@@ -208,17 +206,6 @@ def register_fused(diffusion_model, n_pivotal: int):
     res = _conv_injection_site(diffusion_model)
     if res is not None:
         res._tf_fused = int(n_pivotal)
-
-
-def register_dual_stream(diffusion_model, enabled: bool):
-    """Dual-stream schedule: the pivotal pass and the frame pass of a step are enqueued on two CUDA streams; every
-    TokenFlow block records an event when its keyframe caches are filled (pivotal pass) and the frame pass's block
-    waits for it before it reads them.  The pivotal chain (few samples, all the collectives) then runs under the
-    frame chain's compute instead of in front of it."""
-    for module in _transformer_blocks(diffusion_model):
-        module._tf_dual = bool(enabled)
-        if not enabled:
-            module._tf_ev_unit = module._tf_ev_out = None
 
 
 def register_shard(diffusion_model, shard: Optional[PivotalShard]):
@@ -328,22 +315,16 @@ def register_conv_injection(model, injection_schedule):
                     part[n:2 * n] = part[:n]    # uncond <- source   (:89)
                     part[2 * n:] = part[:n]     # cond   <- source   (:91)
 
-                def inject_sharded(part, shard):   # sharded pivotal samples: the source sample may be remote
-                    part_all = shard.all_gather(part)
-                    return part_all.index_select(0, shard.source_index(part.device))
-
                 shard = getattr(res, "_tf_shard", None)
                 n_piv = getattr(res, "_tf_fused", 0)
                 if n_piv:                       # fused pass: [pivotal samples | frame samples]
                     if shard is None:
                         inject_thirds(h[:n_piv])
-                    else:
-                        h[:n_piv] = inject_sharded(h[:n_piv], shard)
+                    else:                       # sharded pivotal samples: the source sample may be on another rank
+                        h[:n_piv] = shard.all_gather(h[:n_piv]).index_select(0, shard.source_index(h.device))
                     inject_thirds(h[n_piv:])
-                elif shard is None:
-                    inject_thirds(h)
                 else:
-                    h = inject_sharded(h, shard)
+                    inject_thirds(h)
             if res.conv_shortcut is not None:
                 skip = res.conv_shortcut(skip)
             out = skip + h
@@ -454,63 +435,6 @@ def register_extended_attention(model):
 
 
 # --------------------------------------------------------------------------------------------
-# plain self-attention (the inversion stage's UNet, preprocess.py:222 / :256)
-# --------------------------------------------------------------------------------------------
-_SELF_TABLES = {}
-
-
-def _self_table(n: int):
-    """Every sample attends to its own S keys: table entry (j, j, j, 1)."""
-    tab = _SELF_TABLES.get(n)
-    if tab is None:
-        tab = _SELF_TABLES[n] = [(j, j, j, 1) for j in range(n)]
-    return tab
-
-
-def _plain_sa_forward(attn, fallback):
-    """Per-sample self-attention on tf_ext_attn: q/k/v as one GEMM on the concatenated weight, the kernel reads them in
-    place by token stride, then to_out.  Other inputs (CPU, fp32, biased projections, cross-attention, a mask) go to
-    `fallback`, the forward the module had before."""
-    to_out = attn.to_out[0] if type(attn.to_out) is torch.nn.modules.container.ModuleList else attn.to_out
-
-    def forward(x, encoder_hidden_states=None, attention_mask=None):
-        if (encoder_hidden_states is not None or attention_mask is not None or not x.is_cuda
-                or x.dtype != torch.float16 or any(getattr(attn, n).bias is not None for n in ("to_q", "to_k", "to_v"))
-                or not (torch.is_autocast_enabled() or attn.to_q.weight.dtype == torch.float16)):
-            return fallback(x, encoder_hidden_states=encoder_hidden_states, attention_mask=attention_mask)
-        dim = attn.to_q.weight.shape[0]
-        qkv = torch.nn.functional.linear(x, _fused_weight(attn, ("to_q", "to_k", "to_v"), torch.float16))
-        q, k, v = qkv[..., :dim], qkv[..., dim:2 * dim], qkv[..., 2 * dim:]
-        out = _ops().ext_attn_table(q, k, v, _self_table(x.shape[0]), attn.heads, attn.scale)
-        return to_out(out)
-
-    return forward
-
-
-def register_native_self_attention(unet):
-    """Install the native per-sample self-attention on every transformer block's attn1 (attn2 stays as it is).
-    `remove_native_self_attention` restores the forward each attn1 had before."""
-    for module in _transformer_blocks(unet):
-        attn = module.attn1
-        if "_tf_plain_prev" in attn.__dict__:
-            continue
-        attn._tf_plain_prev = attn.__dict__.get("forward")
-        attn.forward = _plain_sa_forward(attn, attn.forward)
-
-
-def remove_native_self_attention(unet):
-    for module in _transformer_blocks(unet):
-        attn = module.attn1
-        if "_tf_plain_prev" not in attn.__dict__:
-            continue
-        prev = attn.__dict__.pop("_tf_plain_prev")
-        if prev is None:
-            attn.__dict__.pop("forward", None)
-        else:
-            attn.forward = prev
-
-
-# --------------------------------------------------------------------------------------------
 # TokenFlow block
 # --------------------------------------------------------------------------------------------
 _BLEND_CACHE = {}
@@ -603,16 +527,7 @@ def make_tokenflow_attention_block(block_class: Type[torch.nn.Module]) -> Type[t
                     encoder_hidden_states=encoder_hidden_states if self.only_cross_attention else None,
                     **cross_attention_kwargs)
                 self.kf_attn_output = self.attn_output                                   # :360
-            self._tf_record_ready()
             return self.attn_output + hidden_states                                      # :397
-
-        def _tf_record_ready(self):
-            """Dual-stream schedule: mark the point on the pivotal pass's stream where this block's keyframe caches
-            (pivot unit rows, extended-attention output) are complete."""
-            if getattr(self, "_tf_dual", False) and self.kf_attn_output.is_cuda:
-                ev = torch.cuda.Event()
-                ev.record()
-                self._tf_ev_unit = self._tf_ev_out = ev
 
         def _tf_frames(self, hidden_states):
             """Self-attention stage of a frame pass: NN field + propagation (reference :329-348, :361-397)."""
@@ -629,9 +544,6 @@ def make_tokenflow_attention_block(block_class: Type[torch.nn.Module]) -> Type[t
             n_kf = kf.shape[0] // 3
             # norm1 of the source stream only — the other two thirds are never used in this branch (:335)
             x_unit = ops.layernorm_unit_rows(hidden_states[:n_frames], self.norm1)
-            ev = getattr(self, "_tf_ev_out", None) if getattr(self, "_tf_dual", False) else None
-            if ev is not None:                       # dual-stream schedule: the caches are filled on the other stream
-                torch.cuda.current_stream().wait_event(ev)
             idx_a, idx_b = ops.nn_field(x_unit, self._tf_pivot_unit, kf_a, kf_b)          # :335-343
             out_dtype = torch.float32 if (_strict_dtype() and idx_b is not None) else None
             self._tf_nn_idx = (idx_a, idx_b)

@@ -3,20 +3,18 @@
     python tools/invert_bench.py [--config C2|C4] [--steps 24] [--warmup 3] [--rounds 3] [--batch B] [--no-full]
                                  [--out FILE]
 
-Three arms run in the same process on the same UNet and latents, alternated round by round, each timed over
+Two arms run in the same process on the same UNet and latents, alternated round by round, each timed over
 `--steps` inversion steps of the reference's 500-step grid after `--warmup` untimed steps:
   * oracle_eager   the reference's loop as oracle/inversion.py restates it (eager fp16 UNet, SDPA attn1, ATen
                    elementwise DDIM update per batch): what the stage costs without the graphed path;
-  * graph_sdpa     the graphed path (`LatentInverter` on a CUDA fp16 UNet) with attn1 left on SDPA;
-  * graph_native   the graphed path with attn1 on the native per-sample attention (tf_ext_attn).
-The attention route of the graphed arms is chosen through `preprocess._NATIVE_ATTN1`, the test seam.  Reported per
-arm: the median over rounds of ms per step.  Then, unless --no-full, one full run of the stage as the reference runs
-it (500 inversion steps saving the 50 sampling timesteps, then 500 reconstruction steps, graph capture included):
-its wall time, frames/s of the stage, and the reconstruction's relative L2 against the input latents.  The GPU's
-name, power limit and median SM clock over the timed regions are read in the same call.
+  * graph_sdpa     the graphed path (`LatentInverter` on a CUDA fp16 UNet), attn1 on SDPA.
+Reported per arm: the median over rounds of ms per step.  Then, unless --no-full, one full run of the stage as the
+reference runs it (500 inversion steps saving the 50 sampling timesteps, then 500 reconstruction steps, graph capture
+included): its wall time, frames/s of the stage, and the reconstruction's relative L2 against the input latents.  The
+GPU's name, power limit and median SM clock over the timed regions are read in the same call.
 
-The two graphed arms keep one captured step each, next to the eager arm's memory: at C4 with 40 frames per UNet
-call that exceeds 80 GB, so C4 is timed with --batch 20 (two UNet calls per step).
+The graphed arm keeps its captured step next to the eager arm's memory; the C4 figures in README.md were taken with
+--batch 20 (two UNet calls per step).
 
 Workloads (random-init UNet fp16 channels_last, synthetic N(0,1) latents, the reference's batch size 40):
   C2  40 frames, 512 x 512 (64 x 64 latents), SD1.5
@@ -51,7 +49,7 @@ def main():
     import torch
     from bench import ClockSampler
     from oracle import inversion as OI
-    from tokenflow_b200 import preprocess, sd_unet
+    from tokenflow_b200 import sd_unet
     from tokenflow_b200.preprocess import LatentInverter
     from tokenflow_b200.scheduler import DDIMScheduler
 
@@ -71,24 +69,13 @@ def main():
     def oracle_arm(n):
         OI.ddim_inversion(unet, sch, cond, x0.clone(), B, timesteps_to_save=[], n_steps=n)
 
-    inverters = {}
+    graph_inv = LatentInverter(unet, DDIMScheduler(), 500)
+    coef, _, ts_up, _ = graph_inv._device_tables()
 
-    def graph_arm(native):
-        inv = inverters.get(native)
-        if inv is None:
-            inv = inverters[native] = LatentInverter(unet, DDIMScheduler(), 500)
-        coef, _, ts_up, _ = inv._device_tables()
+    def graph_arm(n):
+        graph_inv._run_steps(x0, cond, B, coef[:n], ts_up[:n])
 
-        def run(n):
-            saved = preprocess._NATIVE_ATTN1
-            preprocess._NATIVE_ATTN1 = native
-            try:
-                inv._run_steps(x0, cond, B, coef[:n], ts_up[:n])
-            finally:
-                preprocess._NATIVE_ATTN1 = saved
-        return run
-
-    arms = {"oracle_eager": oracle_arm, "graph_sdpa": graph_arm(False), "graph_native": graph_arm(True)}
+    arms = {"oracle_eager": oracle_arm, "graph_sdpa": graph_arm}
     times = {name: [] for name in arms}
     clocks = ClockSampler(0)
     for name, fn in arms.items():                # warm-up: cuDNN / cuBLAS choices, graph capture
@@ -107,11 +94,8 @@ def main():
            "steps_per_arm": K, "rounds": args.rounds,
            "ms_per_step": {k: statistics.median(v) for k, v in times.items()},
            "ms_per_step_all": times}
-    res["speedup_native_vs_sdpa"] = res["ms_per_step"]["graph_sdpa"] / res["ms_per_step"]["graph_native"]
-    res["speedup_native_vs_oracle"] = res["ms_per_step"]["oracle_eager"] / res["ms_per_step"]["graph_native"]
 
     if not args.no_full:
-        inverters.clear()
         torch.cuda.empty_cache()
         toy = DDIMScheduler()
         toy.set_timesteps(50)
