@@ -200,6 +200,23 @@ int tf_resize_u8(const void* in, int64_t n, int h_in, int w_in, int h, int w, co
                  const int32_t* h_coeffs, int h_taps, const int32_t* v_bounds, const int32_t* v_coeffs, int v_taps,
                  void* tmp, void* out, tf_stream_t stream);
 
+/* OpenCV's `cv2.Canny(frame, low, high)` (aperture 3, L2gradient = false) of RGB uint8 frames, bit for bit: the edge
+ * maps the reference's ControlNet path conditions on (preprocess.py:113-127 get_canny_cond).  Per-channel 3x3 Sobel
+ * with replicated borders, the channel of largest |dx| + |dy| (first on a tie), OpenCV's integer non-maximum
+ * suppression, thresholds floor(low) < floor(high) (swapped when low > high; a magnitude must exceed them), and
+ * hysteresis over 8-connected candidates.  Five launches (classify, then union-find merge, compress, flag, write),
+ * nothing synchronised: capturable in a CUDA graph.  n <= 65535, 1 <= h, w <= 65536, n*h*w < 2^31.
+ * tf_canny_workspace  bytes of workspace for n frames of h x w (-1 for bad sizes)
+ * tf_canny_u8
+ *   frames      device [n, h, w, 3] uint8, any alignment
+ *   workspace   device, >= tf_canny_workspace(n, h, w) bytes, 16-byte aligned, uninitialised
+ *   edges_u8    device [n, h, w] uint8, 0 / 255 (cv2.Canny's output), or NULL
+ *   cond_f16    device [n, h, w, 3] fp16, 0 / 1 in every channel: get_canny_cond's [n, 3, h, w] tensor in the
+ *               channels_last layout, or NULL (not both NULL) */
+int64_t tf_canny_workspace(int64_t n, int h, int w);
+int tf_canny_u8(const void* frames, int64_t n, int h, int w, double low, double high, void* workspace,
+                int64_t workspace_bytes, void* edges_u8, void* cond_f16, tf_stream_t stream);
+
 /* ---- multi-GPU: all-gather of keyframe tensors along the pivotal-sample axis (SURVEY.md §8e) ----
  * NCCL (all-gather over NVLink 5 / NVSwitch) bound at run time; one communicator per process/GPU.
  * Rendezvous: rank 0 calls tf_comm_unique_id and ships the TF_COMM_ID_BYTES to the other ranks by any

@@ -1,6 +1,7 @@
 // C-ABI layer (include/tokenflow_b200.h): argument validation, per-frame tables, error plumbing.
 #include <algorithm>
 #include <atomic>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -114,13 +115,24 @@ static bool resize_sizes_ok(int in, int out, const char* who) {
   return true;
 }
 
+// Canny: every pixel index of the call is an int32 label of the hysteresis pass
+static bool canny_sizes_ok(int64_t n, int h, int w, const char* who) {
+  if (n < 0 || n > 65535 || h < 1 || w < 1 || h > 65536 || w > 65536 ||
+      (n > 0 && (int64_t)h * w > (INT32_MAX - 1) / n)) {
+    set_last_error("%s: bad size n=%lld h=%d w=%d (n <= 65535, 1 <= h, w <= 65536, n*h*w < 2^31)", who, (long long)n,
+                   h, w);
+    return false;
+  }
+  return true;
+}
+
 }  // namespace tf
 
 using namespace tf;
 
 extern "C" {
 
-int tf_version(void) { return 1002; }
+int tf_version(void) { return 1003; }
 
 const char* tf_last_error(void) { return g_err; }
 
@@ -317,6 +329,39 @@ int tf_resize_u8(const void* in, int64_t n, int h_in, int w_in, int h, int w, co
     g_launches += 1;
   }
   return TF_OK;
+}
+
+int64_t tf_canny_workspace(int64_t n, int h, int w) {
+  if (!canny_sizes_ok(n, h, w, "tf_canny_workspace")) return -1;
+  return (int64_t)canny_workspace(n, h, w);
+}
+
+int tf_canny_u8(const void* frames, int64_t n, int h, int w, double low, double high, void* workspace,
+                int64_t workspace_bytes, void* edges_u8, void* cond_f16, tf_stream_t stream) {
+  if (!canny_sizes_ok(n, h, w, "tf_canny_u8")) return TF_ERR_INVALID_ARGUMENT;
+  if (!(low == low) || !(high == high)) {
+    set_last_error("tf_canny_u8: NaN threshold");
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  if (low > high) std::swap(low, high);          // cv2.Canny swaps, then floors
+  const double lo = std::floor(low), hi = std::floor(high);
+  // magnitudes are in [0, 2040]: thresholds past either end act like the ends
+  const int ilo = (int)std::min(std::max(lo, -1.0), 2040.0), ihi = (int)std::min(std::max(hi, -1.0), 2040.0);
+  if (n == 0) return TF_OK;
+  const long long need = canny_workspace(n, h, w);
+  if (workspace_bytes < need) {
+    set_last_error("tf_canny_u8: workspace of %lld bytes, %lld needed", (long long)workspace_bytes, need);
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  if (!frames || !workspace || (!edges_u8 && !cond_f16) || !aligned16(workspace) ||
+      (cond_f16 && (reinterpret_cast<uintptr_t>(cond_f16) & 1u))) {
+    set_last_error("tf_canny_u8: NULL or misaligned pointer (frames, a 16-byte aligned workspace, and at least one "
+                   "output are needed)");
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  int e = launch_canny(frames, n, h, w, ilo, ihi, workspace, edges_u8, cond_f16, static_cast<cudaStream_t>(stream));
+  if (!e) g_launches += 5;
+  return e;
 }
 
 int tf_geglu(const void* xh, const void* gate, int64_t n, void* out, tf_stream_t stream) {

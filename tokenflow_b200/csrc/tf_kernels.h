@@ -50,6 +50,11 @@ int launch_resize_h(const void* in, long long n_rows, int w_in, int w, const int
 int launch_resize_v(const void* in, long long n, int h_in, int h, int w, const int32_t* bounds, const int32_t* coeffs,
                     int taps, void* out, cudaStream_t stream);
 
+// OpenCV's Canny of RGB uint8 frames (tf_canny.cu): a classify launch and four union-find hysteresis launches.
+long long canny_workspace(long long n, int h, int w);
+int launch_canny(const void* frames, long long n, int h, int w, int low, int high, void* workspace, void* edges,
+                 void* cond, cudaStream_t stream);
+
 int launch_propagate(const void* A, const int32_t* idx_a, const int32_t* idx_b, const FrameTable& tab, int F,
                      int S, int dim, int K, const void* residual, void* out, int out_is_f32, long long F_total,
                      cudaStream_t stream);

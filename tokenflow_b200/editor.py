@@ -13,6 +13,11 @@ Per denoising step (reference batched_denoise_step, :220-233):
      fills the per-block caches (pivot features, extended-attention outputs);
   3. frame passes: UNet over each batch of B frames; self-attention is replaced by NN propagation;
   4. classifier-free guidance + DDIM update per batch.
+
+With a ControlNet (controlnet.py) and the Canny conditioning of the frames (`preprocess.canny_cond`), every UNet call
+is preceded by the ControlNet on the same batch, each sample reading the conditioning of its own frame (a pivotal
+sample: its keyframe's), and the UNet adds the residuals: diffusers' ControlNet pipeline without guess_mode, applied
+to the source stream as well, as the reference's inversion does.  It composes with either mode.
 """
 from __future__ import annotations
 
@@ -29,11 +34,19 @@ from .ops import all_gather
 class TokenFlowEditor(nn.Module):
     def __init__(self, unet: nn.Module, scheduler, hooks, config: Dict, text_embeds: torch.Tensor,
                  pnp_guidance_embeds: torch.Tensor, source_latents: Optional[Callable[[int], torch.Tensor]] = None,
-                 world_size: int = 1, rank: int = 0, group=None):
+                 world_size: int = 1, rank: int = 0, group=None, controlnet: Optional[nn.Module] = None,
+                 controlnet_cond: Optional[torch.Tensor] = None):
         """config keys (names follow configs/config_pnp.yaml): n_frames, batch_size, n_timesteps,
-        guidance_scale, mode ('pnp' | 'sdedit'), pnp_attn_t, pnp_f_t, start (sdedit), latents_path.
-        text_embeds: [2, L, C] (uncond, cond);  pnp_guidance_embeds: [1, L, C] (inversion prompt)."""
+        guidance_scale, mode ('pnp' | 'sdedit'), pnp_attn_t, pnp_f_t, start (sdedit), latents_path,
+        controlnet_conditioning_scale (default 1.0).
+        text_embeds: [2, L, C] (uncond, cond);  pnp_guidance_embeds: [1, L, C] (inversion prompt).
+        controlnet, controlnet_cond: an optional ControlNet and the [N, 3, H, W] conditioning of all N frames."""
         super().__init__()
+        if (controlnet is None) != (controlnet_cond is None):
+            raise ValueError("TokenFlowEditor needs both controlnet and controlnet_cond, or neither")
+        # kept out of the module tree: the register_* hooks walk this module's submodules, and the ControlNet's
+        # attention must stay the plain one
+        object.__setattr__(self, "controlnet", controlnet)
         self.unet = unet
         self.scheduler = scheduler
         self.hooks = hooks
@@ -78,6 +91,17 @@ class TokenFlowEditor(nn.Module):
         self._g_static = None
         self._text_cache = {}
         self._shard_cache = {}
+        self._ccond = None
+        if controlnet is not None:
+            cl = next(controlnet.parameters()).is_contiguous(memory_format=torch.channels_last)
+            self._ccond = controlnet_cond.to(self.device, next(controlnet.parameters()).dtype).contiguous(
+                memory_format=torch.channels_last if cl else torch.contiguous_format)
+
+    def _residuals(self, latent_model_input, t, text, cond):
+        """UNet keyword arguments of one call: the ControlNet's residuals for `cond`, or {} without a ControlNet."""
+        from .controlnet import controlnet_residuals
+        return controlnet_residuals(self.controlnet, latent_model_input, t, text, cond,
+                                    float(self.config.get("controlnet_conditioning_scale", 1.0)))
 
     # ------------------------------------------------------------------------------------
     def init_method(self):
@@ -111,7 +135,11 @@ class TokenFlowEditor(nn.Module):
         self.hooks.register_time(self, int(t))
         text_embed_input = torch.cat([self.pnp_guidance_embeds.repeat(len(indices), 1, 1),
                                       torch.repeat_interleave(self.text_embeds, len(indices), dim=0)])
-        noise_pred = self.unet(latent_model_input, t, encoder_hidden_states=text_embed_input)['sample']
+        res = {}
+        if self.controlnet is not None:
+            c = self._ccond[indices.to(self._ccond.device)]
+            res = self._residuals(latent_model_input, t, text_embed_input, torch.cat([c, c, c]))
+        noise_pred = self.unet(latent_model_input, t, encoder_hidden_states=text_embed_input, **res)['sample']
         _, noise_pred_uncond, noise_pred_cond = noise_pred.chunk(3)
         noise_pred = noise_pred_uncond + self.config["guidance_scale"] * (noise_pred_cond - noise_pred_uncond)
         return self.scheduler.step(noise_pred, t, x)['prev_sample']
@@ -254,13 +282,19 @@ class TokenFlowEditor(nn.Module):
         xs, srcs = x[lo:lo + per], src_all[lo:lo + per]
         latent_model_input = torch.cat([piv_lat, srcs, xs, xs])
         text = self._fused_text(slots, per)
+        res = {}
+        if self.controlnet is not None:
+            # the same gather as the pivotal latents (index f or N + f: keyframe f), so a graph replay stays sync-free
+            c_piv = self._ccond.index_select(0, piv_idx.remainder(N))
+            c_loc = self._ccond[lo:lo + per]
+            res = self._residuals(latent_model_input, t_dev, text, torch.cat([c_piv, c_loc, c_loc, c_loc]))
         h.register_time(self, t_int)
         h.register_pivotal(self, False)
         h.register_shard(self, shard)
         h.register_frame_table(self, *self.frame_table(list(range(lo, lo + per))))
         h.register_fused(self, n_piv)
         try:
-            noise_pred = self.unet(latent_model_input, t_dev, encoder_hidden_states=text)['sample'][n_piv:]
+            noise_pred = self.unet(latent_model_input, t_dev, encoder_hidden_states=text, **res)['sample'][n_piv:]
         finally:
             h.register_fused(self, 0)
             h.register_shard(self, None)

@@ -69,6 +69,10 @@ _SIGNATURES = {
     "tf_resize_u8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                     ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
                                     ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "tf_canny_workspace": (ctypes.c_int64, [ctypes.c_int64, ctypes.c_int, ctypes.c_int]),
+    "tf_canny_u8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_double,
+                                   ctypes.c_double, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p,
+                                   ctypes.c_void_p]),
     "tf_geglu": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
 }
 
@@ -520,6 +524,36 @@ class CudaOps:
             frames.data_ptr(), n, h_in, w_in, h, w, ptr(hb), ptr(hk), ht, ptr(vb), ptr(vk), vt, ptr(tmp), out.data_ptr(),
             self._stream()), "tf_resize_u8"))
         return out
+
+    def canny(self, frames: torch.Tensor, low: float = 100, high: float = 200, edges: bool = True, cond: bool = True,
+              out_edges: Optional[torch.Tensor] = None, out_cond: Optional[torch.Tensor] = None):
+        """uint8 RGB frames [N, H, W, 3] (CUDA) -> (edges, cond): `cv2.Canny(frame, low, high)` of every frame as uint8
+        [N, H, W] (0 / 255) and the reference's `get_canny_cond` tensor, fp16 [N, 3, H, W] channels_last with 0 / 1 in
+        every channel.  Either output can be skipped (None is returned in its place) or given.  The workspace comes from
+        the caching allocator on this stream."""
+        assert frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[-1] == 3 and frames.is_cuda
+        assert edges or cond
+        frames = frames.contiguous()
+        n, h, w, _ = frames.shape
+        dev = frames.device
+        ws_bytes = int(self.lib.tf_canny_workspace(n, h, w))
+        if ws_bytes < 0:
+            self._check(1, "tf_canny_workspace")
+        ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=dev)
+        e = c = None
+        if edges:
+            e = out_edges if out_edges is not None else torch.empty((n, h, w), dtype=torch.uint8, device=dev)
+            assert e.shape == (n, h, w) and e.dtype == torch.uint8 and e.is_contiguous()
+        if cond:
+            c = out_cond if out_cond is not None else torch.empty((n, 3, h, w), dtype=torch.float16, device=dev,
+                                                                  memory_format=torch.channels_last)
+            assert c.shape == (n, 3, h, w) and c.dtype == torch.float16 and c.is_contiguous(memory_format=torch.channels_last)
+        work = 3.0 * n * h * w + (n * h * w if edges else 0) + (6.0 * n * h * w if cond else 0)
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        self._timed("tf_canny_u8", work, lambda: self._check(self.lib.tf_canny_u8(
+            frames.data_ptr(), n, h, w, float(low), float(high), ws.data_ptr(), ws.numel(), ptr(e), ptr(c),
+            self._stream()), "tf_canny_u8"))
+        return e, c
 
     def geglu(self, xh: torch.Tensor, gate: torch.Tensor) -> torch.Tensor:
         """xh * gelu(gate) of two fp16 tensors of one shape (the GEGLU GEMM outputs), bit-equal to the eager product."""

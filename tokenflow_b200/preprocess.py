@@ -8,9 +8,11 @@ run_tokenflow_pnp.py:145-163, on `vae.AutoencoderKL`), and the edit's starting n
     encode_imgs -> LatentInverter.ddim_inversion -> saved_latents() -> ddim_eps -> scheduler.add_noise ->
     TokenFlowEditor.sample_loop -> decode_latents
 
-The CLIP text encoder and the depth / ControlNet variants stay out of scope.  The latents directory is still written
-in the reference's format, so it can be read back by `TokenFlowEditor` / the reference drivers
-(`tokenflow_utils.load_source_latents_t`).  Frames are independent in this stage, so with several ranks each rank
+With a ControlNet (controlnet.py) and the Canny conditioning of the frames (`canny_cond`), every UNet call of both
+directions is the reference's `controlnet_pred` (preprocess.py:129-149): the ControlNet on the batch's frames of the
+conditioning, then the UNet with its residuals.  The CLIP text encoder and the depth variant stay out of scope.  The
+latents directory is still written in the reference's format, so it can be read back by `TokenFlowEditor` / the
+reference drivers (`tokenflow_utils.load_source_latents_t`).  Frames are independent in this stage, so with several ranks each rank
 inverts its own contiguous share and the saved tensors are all-gathered.
 
 Two paths compute the same steps:
@@ -67,10 +69,16 @@ def saved_timesteps(ts_up: List[int], timesteps_to_save: Optional[Iterable[int]]
 
 
 class LatentInverter:
-    def __init__(self, unet, scheduler, n_timesteps: int, world_size: int = 1, rank: int = 0, group=None):
+    def __init__(self, unet, scheduler, n_timesteps: int, world_size: int = 1, rank: int = 0, group=None,
+                 controlnet=None, controlnet_cond: Optional[torch.Tensor] = None):
         """`scheduler.set_timesteps(n_timesteps)` defines the inversion grid (reference default: 500 steps, of which
-        the 50 sampling timesteps are saved)."""
+        the 50 sampling timesteps are saved).  `controlnet` and `controlnet_cond` ([N, 3, H, W], the Canny
+        conditioning of all N frames, `canny_cond`) run every UNet call as the reference's `controlnet_pred`; each
+        rank reads the conditioning of its own frames."""
+        if (controlnet is None) != (controlnet_cond is None):
+            raise ValueError("LatentInverter needs both controlnet and controlnet_cond, or neither")
         self.unet, self.scheduler = unet, scheduler
+        self.controlnet, self.controlnet_cond = controlnet, controlnet_cond
         self.device = next(unet.parameters()).device
         self.scheduler.set_timesteps(n_timesteps, device=self.device)
         self.world_size, self.rank, self.group = world_size, rank, group
@@ -98,8 +106,16 @@ class LatentInverter:
         a_prev = float(self.scheduler.alphas_cumprod[t_prev]) if t_prev is not None else float(self.scheduler.final_alpha_cumprod)
         return a_t ** 0.5, (1 - a_t) ** 0.5, a_prev ** 0.5, (1 - a_prev) ** 0.5          # mu, sigma, mu_prev, sigma_prev
 
-    def _eps(self, x, t: int, cond):
-        out = self.unet(x, torch.tensor(t, device=x.device), encoder_hidden_states=cond.repeat(x.shape[0], 1, 1))
+    def _eps(self, x, t: int, cond, frame0: int = 0):
+        """The UNet's noise prediction for the frames [frame0, frame0 + len(x)) (reference preprocess.py:222-223)."""
+        from .controlnet import controlnet_residuals
+        t_dev = torch.tensor(t, device=x.device)
+        ctx = cond.repeat(x.shape[0], 1, 1)
+        ccond = None
+        if self.controlnet is not None:
+            ccond = self.controlnet_cond[frame0:frame0 + x.shape[0]].to(x.device)
+        res = controlnet_residuals(self.controlnet, x, t_dev, ctx, ccond)
+        out = self.unet(x, t_dev, encoder_hidden_states=ctx, **res)
         return out["sample"] if isinstance(out, dict) else out.sample
 
     def _local(self, n: int):
@@ -135,7 +151,7 @@ class LatentInverter:
             mu, sigma, mu_prev, sigma_prev = self._alphas(t, ts[i - 1] if i > 0 else None)
             for b in range(0, x.shape[0], batch_size):
                 xb = x[b:b + batch_size]
-                eps = self._eps(xb, t, cond)
+                eps = self._eps(xb, t, cond, lo + b)
                 pred_x0 = (xb - sigma_prev * eps) / mu_prev
                 x[b:b + batch_size] = mu * pred_x0 + sigma * eps
             if save_latents and save_path is not None and (t in keep or i == len(ts) - 1):
@@ -158,7 +174,7 @@ class LatentInverter:
             mu, sigma, mu_prev, sigma_prev = self._alphas(t, ts[i + 1] if i < len(ts) - 1 else None)
             for b in range(0, x.shape[0], batch_size):
                 xb = x[b:b + batch_size]
-                eps = self._eps(xb, t, cond)
+                eps = self._eps(xb, t, cond, lo + b)
                 pred_x0 = (xb - sigma * eps) / mu
                 x[b:b + batch_size] = mu_prev * pred_x0 + sigma_prev * eps
         return self._gathered(x, n)
@@ -180,12 +196,14 @@ class LatentInverter:
 
     def _step_runner(self, share: int, shape, batch_size: int, cond: torch.Tensor):
         """Static buffers and the step over a share of `share` frames: the UNet over the share in batches of
-        `batch_size`, then `tf_ddim` in place.  Captured once per share shape and replayed; `_use_graph = False` runs
-        the same function eagerly."""
+        `batch_size` (each call preceded by the ControlNet on the batch's conditioning when there is one), then
+        `tf_ddim` in place.  Captured once per share shape and replayed; `_use_graph = False` runs the same function
+        eagerly."""
         from . import tokenflow_utils as tfu
+        from .controlnet import controlnet_residuals
         ops = tfu._ops()                      # the library is required: raises without it or without an H100
         bs = max(1, min(batch_size, share))
-        key = (share, tuple(shape), bs, tuple(cond.shape[1:]), self._use_graph)
+        key = (share, tuple(shape), bs, tuple(cond.shape[1:]), self._use_graph, self.controlnet is not None)
         entry = self._graphs.get(key)
         if entry is not None:
             entry["cond"].copy_(cond.expand(bs, -1, -1))
@@ -195,13 +213,22 @@ class LatentInverter:
               "t": torch.zeros((), dtype=torch.int64, device=dev),
               "coef": torch.zeros(4, dtype=torch.float32, device=dev),
               "cond": cond.to(dev, torch.float16).repeat(bs, 1, 1)}
+        if self.controlnet is not None:
+            # the share's conditioning, refreshed per call by `_run_steps`, in the ControlNet's memory format
+            cl = next(self.controlnet.parameters()).is_contiguous(memory_format=torch.channels_last)
+            st["ccond"] = torch.zeros((share,) + tuple(self.controlnet_cond.shape[1:]), dtype=torch.float16,
+                                      device=dev).contiguous(memory_format=torch.channels_last if cl else
+                                                             torch.contiguous_format)
 
         def step():
             x = st["x"]
             outs = []
             for b in range(0, share, bs):
                 xb = x[b:b + bs]
-                out = self.unet(xb, st["t"], encoder_hidden_states=st["cond"][:xb.shape[0]])
+                ctx = st["cond"][:xb.shape[0]]
+                res = controlnet_residuals(self.controlnet, xb, st["t"], ctx, st["ccond"][b:b + bs]) \
+                    if self.controlnet is not None else {}
+                out = self.unet(xb, st["t"], encoder_hidden_states=ctx, **res)
                 outs.append(out["sample"] if isinstance(out, dict) else out.sample)
             eps = outs[0] if len(outs) == 1 else torch.cat(outs)
             ops.ddim(eps, x, st["coef"], out=x)
@@ -227,15 +254,19 @@ class LatentInverter:
         return entry
 
     def _run_steps(self, x_share: torch.Tensor, cond, batch_size: int, coef: torch.Tensor, ts: torch.Tensor,
-                   save_slots: Optional[Dict[int, int]] = None, saved: Optional[torch.Tensor] = None):
+                   save_slots: Optional[Dict[int, int]] = None, saved: Optional[torch.Tensor] = None,
+                   frame0: int = 0):
         """All steps of one direction over this rank's share: per step, refresh the timestep and the coefficient row,
-        replay, and copy the latents of a saved step into its slot of `saved`.  Returns the share's final latents."""
+        replay, and copy the latents of a saved step into its slot of `saved`.  Returns the share's final latents.
+        `frame0` is the share's first frame: the ControlNet conditioning is read from there."""
         share = x_share.shape[0]
         if share == 0:
             return x_share
         entry = self._step_runner(share, x_share.shape[1:], batch_size, cond)
         st = entry["st"]
         st["x"].copy_(x_share)
+        if "ccond" in st:
+            st["ccond"].copy_(self.controlnet_cond[frame0:frame0 + share])
         for i in range(coef.shape[0]):
             st["t"].copy_(ts[i])
             st["coef"].copy_(coef[i])
@@ -261,7 +292,7 @@ class LatentInverter:
         n = latent_frames.shape[0]
         x_share, per = self._share(latent_frames)
         saved = torch.zeros((len(plan), per) + tuple(latent_frames.shape[1:]), dtype=torch.float16, device=self.device)
-        self._run_steps(x_share, cond, batch_size, inv_coef, ts_up_dev, slots, saved)
+        self._run_steps(x_share, cond, batch_size, inv_coef, ts_up_dev, slots, saved, self._local(n)[0])
         # one collective after the last step: [G * n_saved, per, ...] -> per saved timestep, the N frames in order
         full = all_gather(saved, self.world_size, self.group, self.comm)
         full = full.view((self.world_size, len(plan), per) + tuple(latent_frames.shape[1:]))
@@ -278,7 +309,8 @@ class LatentInverter:
     def _device_sample(self, x, cond, batch_size):
         _, rec_coef, _, ts_dn_dev = self._device_tables()
         x_share, _ = self._share(x)
-        return self._gathered(self._run_steps(x_share, cond, batch_size, rec_coef, ts_dn_dev), x.shape[0])
+        return self._gathered(self._run_steps(x_share, cond, batch_size, rec_coef, ts_dn_dev,
+                                              frame0=self._local(x.shape[0])[0]), x.shape[0])
 
 
 def resize_frames(frames_u8: torch.Tensor, size) -> torch.Tensor:
@@ -300,6 +332,26 @@ def resize_frames(frames_u8: torch.Tensor, size) -> torch.Tensor:
     from PIL import Image
     return torch.from_numpy(np.stack([np.asarray(Image.fromarray(f).resize((w, h), Image.LANCZOS))
                                       for f in frames_u8.contiguous().numpy()]))
+
+
+def canny_cond(frames_u8: torch.Tensor, low: float = 100, high: float = 200) -> torch.Tensor:
+    """uint8 RGB frames [N, H, W, 3] -> the ControlNet conditioning [N, 3, H, W] fp16 of the reference's
+    `get_canny_cond` (preprocess.py:113-127): `cv2.Canny(frame, low, high)` of every frame, the edge map stacked
+    three times and divided by 255, so every value is 0 or 1.  The reference feeds Canny
+    `np.uint8(255 * fp16(ToTensor(frame)))`, which is the frame's own bytes, so the frames `resize_frames` returns
+    go in as they are.
+
+    CUDA frames go through `tf_canny_u8` on the device (bit for bit cv2's edges) and come back channels_last, the
+    layout the ControlNet's first convolution reads; CPU frames go through `cv2.Canny` itself."""
+    assert frames_u8.dtype == torch.uint8 and frames_u8.dim() == 4 and frames_u8.shape[-1] == 3
+    if frames_u8.is_cuda:
+        from . import ops as tf_ops
+        return tf_ops.default_ops().canny(frames_u8, low, high, edges=False)[1]
+    import cv2
+    import numpy as np
+    edges = np.stack([cv2.Canny(f, low, high) for f in frames_u8.contiguous().numpy()])
+    image = np.concatenate([edges[..., None]] * 3, axis=-1)
+    return torch.from_numpy(image.astype(np.float32) / 255.0).permute(0, 3, 1, 2).to(torch.float16)
 
 
 def _native_vae(vae) -> bool:

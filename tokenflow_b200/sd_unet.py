@@ -445,7 +445,12 @@ class UNet2DConditionModel(nn.Module):
         self.conv_act = nn.SiLU()
         self.conv_out = nn.Conv2d(ch[0], cfg.out_channels, 3, padding=1)
 
-    def forward(self, sample, timestep, encoder_hidden_states=None, **_):
+    def forward(self, sample, timestep, encoder_hidden_states=None, down_block_additional_residuals=None,
+                mid_block_additional_residual=None, return_dict: bool = True, **_):
+        """diffusers' UNet2DConditionModel.forward.  A ControlNet's outputs (controlnet.py) come in as
+        `down_block_additional_residuals`, one per skip, added to the skips before the up blocks read them, and
+        `mid_block_additional_residual`, added to the mid-block output.  `return_dict=False` returns `(sample,)`.
+        Other keyword arguments are accepted and ignored."""
         if not torch.is_tensor(timestep):
             timestep = torch.tensor([timestep], device=sample.device)
         timestep = timestep.reshape(-1).expand(sample.shape[0]).to(sample.device)
@@ -456,7 +461,13 @@ class UNet2DConditionModel(nn.Module):
         for blk in self.down_blocks:
             x, outs = blk(x, emb, encoder_hidden_states)
             skips.extend(outs)
+        if down_block_additional_residuals is not None:
+            if len(down_block_additional_residuals) != len(skips):
+                raise ValueError(f"{len(down_block_additional_residuals)} down-block residuals for {len(skips)} skips")
+            skips = [s + r for s, r in zip(skips, down_block_additional_residuals)]
         x = self.mid_block(x, emb, encoder_hidden_states)
+        if mid_block_additional_residual is not None:
+            x = x + mid_block_additional_residual
         # diffusers' rule for latents whose sides are not multiples of 2 ** (number of upsamplers): every up block but
         # the last upsamples to the size of the skip it will concatenate next (a plain doubling would give 22 rows
         # where the skip has 21); other latents keep the doubling
@@ -468,7 +479,7 @@ class UNet2DConditionModel(nn.Module):
                 size = skips[-len(blk.resnets) - 1].shape[-2:]
             x = blk(x, skips, emb, encoder_hidden_states, upsample_size=size)
         x = self.conv_out(norm_act(self.conv_norm_out, x))          # conv_norm_out + conv_act (SiLU)
-        return UNetOutput(sample=x)
+        return UNetOutput(sample=x) if return_dict else (x,)
 
 
 def build_unet(kind: str = "sd15", seed: int = 1, device="cpu", dtype=torch.float32,
