@@ -13,8 +13,11 @@
  *     enqueued on `stream` and the caller owns every buffer.
  *   - "host" pointers are read synchronously during the call (small per-frame tables passed to the
  *     kernels by value); "device" pointers must be valid on the current device.
- *   - fp16 activations, int32 indices.  dim and head_dim must be multiples of 8; device pointers
- *     16-byte aligned; tensors contiguous unless a stride argument says otherwise.
+ *   - fp16 activations, int32 indices.  dim and head_dim must be multiples of 8; device pointers to
+ *     activations, outputs and workspaces 16-byte aligned (a misaligned one is refused with
+ *     TF_ERR_INVALID_ARGUMENT before anything is enqueued); coefficient rows, index tables and the
+ *     buffers documented "any alignment" need only their element's alignment; tensors contiguous
+ *     unless a stride argument says otherwise.
  *   - compiled for sm_90a only; the kernels use wgmma / TMA / mbarrier.
  */
 #ifndef TOKENFLOW_B200_H_

@@ -175,8 +175,10 @@ class TokenFlowEditor(nn.Module):
         for t in self._t_host:
             a_t = float(sch._alpha(t))
             a_prev = float(sch._alpha(t - ratio))
-            s1, s2 = np.float32((1 - a_t) ** 0.5), np.float32(a_t ** 0.5)
-            rows.append([float(s1), float(np.float32(1.0) / s2), float(np.float32(a_prev ** 0.5)),
+            # the step divides the fp16 latents by the Python float sqrt(a_t): ATen multiplies by the reciprocal taken in
+            # double and rounded to fp32, which is not always the fp32 reciprocal of the fp32 sqrt (50 steps: 8 rows)
+            s1 = np.float32((1 - a_t) ** 0.5)
+            rows.append([float(s1), float(np.float32(1.0 / a_t ** 0.5)), float(np.float32(a_prev ** 0.5)),
                          float(np.float32((1 - a_prev) ** 0.5))])
         return torch.tensor(rows, dtype=torch.float32, device=self.device)
 

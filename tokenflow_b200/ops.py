@@ -131,6 +131,16 @@ def propagate_bytes(F_: int, S: int, dim: int, kf_a, kf_b, with_residual: bool, 
             + 3.0 * len(kfs) * S * dim * 2 + 4.0 * S * n_idx)
 
 
+def _dense(t: torch.Tensor, memory_format=torch.contiguous_format) -> torch.Tensor:
+    """`t` itself when it is dense in `memory_format` and starts on a 16-byte boundary (the C ABI refuses any other
+    pointer: the kernels load 16-byte vectors and address operands through TMA descriptors), else a copy that is both
+    (the caching allocator aligns every block).  An operand may start at any element offset: a slice along the first
+    dimension of an odd number of odd-sized latents, for one, starts 8 bytes off."""
+    if t.is_contiguous(memory_format=memory_format) and t.data_ptr() % 16 == 0:
+        return t
+    return t.clone(memory_format=memory_format)
+
+
 def _i32(vals: Sequence[int]):
     return (ctypes.c_int32 * len(vals))(*[int(v) for v in vals])
 
@@ -202,7 +212,8 @@ class CudaOps:
 
     # -- operators -------------------------------------------------------------------------
     def unit_rows(self, x: torch.Tensor) -> torch.Tensor:
-        """[..., dim] fp32/fp16 → fp16 unit rows (reference util.py:66-67 + autocast fp16 cast)."""
+        """[..., dim] fp32/fp16 → fp16 unit rows (reference util.py:66-67 + autocast fp16 cast); x may start at any
+        element offset."""
         if x.dtype not in (torch.float32, torch.float16):
             x = x.float()
         dim = x.shape[-1]
@@ -235,7 +246,8 @@ class CudaOps:
 
     def layernorm_unit_rows(self, x: torch.Tensor, norm: torch.nn.LayerNorm) -> torch.Tensor:
         """fp16 [..., dim] → fp16 unit rows of LayerNorm(x) (fp32 statistics): norm1 + unit_rows in one
-        pass over the source stream (reference tokenflow_utils.py:323 + util.py:66-67)."""
+        pass over the source stream (reference tokenflow_utils.py:323 + util.py:66-67); x may start at any element
+        offset."""
         dim = x.shape[-1]
         if not self._ln_fusable(x, norm):
             return self.unit_rows(norm(x))                       # shapes the fused kernel does not cover
@@ -256,7 +268,8 @@ class CudaOps:
         y = fp16(LN(x)) [b, S, dim] (the QKV GEMM operand) and unit = fp16 unit rows of LN(x) for the first
         `n_unit` samples [n_unit, S, dim] (the pivot features of the NN field) — one read of x
         (reference tokenflow_utils.py:323 -> :120-122, :326-327, util.py:66-67).  `y_out` / `unit_out` may be
-        views into packed buffers (last dim contiguous, row pitch a multiple of 8)."""
+        views into packed buffers (last dim contiguous, row pitch a multiple of 8); x and both outputs may start at
+        any element offset (a misaligned output is written through an aligned buffer and a copy)."""
         b, S, dim = x.shape
         if not self._ln_fusable(x, norm):
             y = norm(x)
@@ -270,6 +283,9 @@ class CudaOps:
         x2 = x.reshape(-1, dim)
         if x2.stride(-1) != 1 or x2.stride(0) % 8 or x2.data_ptr() % 16:
             x2 = x2.clone(memory_format=torch.contiguous_format)     # rows the kernel's 16-byte loads cannot address
+        y_dst, unit_dst = y_out, unit_out
+        y_out = y_out if y_out is not None and y_out.data_ptr() % 16 == 0 else None
+        unit_out = unit_out if unit_out is not None and unit_out.data_ptr() % 16 == 0 else None
         y = torch.empty((b, S, dim), dtype=torch.float16, device=x.device) if y_out is None else y_out
         unit = None
         if n_unit:
@@ -283,48 +299,60 @@ class CudaOps:
                                        unit.data_ptr() if unit is not None else None,
                                        pitch(unit) if unit is not None else dim, n_unit * S, self._stream()),
             "tf_layernorm_rows"))
+        if y_dst is not None and y_dst is not y:
+            y = y_dst.copy_(y)
+        if unit_dst is not None and unit is not None and unit_dst is not unit:
+            unit = unit_dst.copy_(unit)
         return y, unit
 
     def cfg_ddim(self, eps_uncond: torch.Tensor, eps_cond: torch.Tensor, x: torch.Tensor, coef: torch.Tensor,
                  guidance: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Classifier-free guidance + DDIM update (reference run_tokenflow_pnp.py:213-217) in one pass;
-        `coef` = device fp32 [4]: sqrt(1-a_t), 1/sqrt(a_t), sqrt(a_prev), sqrt(1-a_prev)."""
+        `coef` = device fp32 [4]: sqrt(1-a_t), 1/sqrt(a_t), sqrt(a_prev), sqrt(1-a_prev).  The operands may have any
+        layout and start at any element offset; `out` (contiguous, made here when None) too: a misaligned one is
+        written through an aligned buffer and a copy."""
         assert eps_uncond.dtype == eps_cond.dtype == x.dtype == torch.float16 and coef.dtype == torch.float32
-        eu, ec, xx = (t if t.is_contiguous() else t.contiguous() for t in (eps_uncond, eps_cond, x))
+        eu, ec, xx = (_dense(t) for t in (eps_uncond, eps_cond, x))
         assert eu.shape == ec.shape == xx.shape
         if out is None:
             out = torch.empty_like(xx)
+        assert out.shape == xx.shape and out.dtype == torch.float16 and out.is_contiguous()
+        dst = out if out.data_ptr() % 16 == 0 else torch.empty_like(xx)
         n = xx.numel()
         self._timed("tf_cfg_ddim", n * 8.0, lambda: self._check(
             self.lib.tf_cfg_ddim(eu.data_ptr(), ec.data_ptr(), xx.data_ptr(), coef.data_ptr(), float(guidance), n,
-                                 out.data_ptr(), self._stream()), "tf_cfg_ddim"))
-        return out
+                                 dst.data_ptr(), self._stream()), "tf_cfg_ddim"))
+        return out if dst is out else out.copy_(dst)
 
     def ddim(self, eps: torch.Tensor, x: torch.Tensor, coef: torch.Tensor,
              out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Guidance-free DDIM update of the inversion stage (reference preprocess.py:217-225 / :251-260);
-        `coef` = device fp32 [4] (s1, inv_s2, s3, s4), see include/tokenflow_b200.h.  `out` may be `x` (in place)."""
+        `coef` = device fp32 [4] (s1, inv_s2, s3, s4), see include/tokenflow_b200.h.  `out` may be `x` (in place).
+        eps may have any layout; x and `out` are contiguous.  All three may start at any element offset: a misaligned
+        operand is read from an aligned copy, a misaligned `out` (or `x`, in place) is written through an aligned
+        buffer and a copy back."""
         assert eps.dtype == x.dtype == torch.float16 and coef.dtype == torch.float32 and coef.is_cuda
         assert eps.shape == x.shape
-        e = eps if eps.is_contiguous() else eps.contiguous()
         if out is None:
             out = torch.empty_like(x, memory_format=torch.contiguous_format)
         assert out.shape == x.shape and out.dtype == torch.float16 and out.is_contiguous() and x.is_contiguous()
+        e, xx = _dense(eps), _dense(x)
+        dst = xx if out is x else (out if out.data_ptr() % 16 == 0 else torch.empty_like(out))
         n = x.numel()
         self._timed("tf_ddim", n * 6.0, lambda: self._check(
-            self.lib.tf_ddim(e.data_ptr(), x.data_ptr(), coef.data_ptr(), n, out.data_ptr(), self._stream()), "tf_ddim"))
-        return out
+            self.lib.tf_ddim(e.data_ptr(), xx.data_ptr(), coef.data_ptr(), n, dst.data_ptr(), self._stream()), "tf_ddim"))
+        return out if dst is out else out.copy_(dst)
 
     def nn_field(self, x_unit: torch.Tensor, piv_unit: torch.Tensor, kf_a: Sequence[int],
                  kf_b: Sequence[int]) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
         """x_unit [F,S,dim], piv_unit [K,S,dim] fp16 unit rows → int32 idx_a, idx_b [F,S]
         (reference tokenflow_utils.py:335-343).  The idx_b rows of frames with kf_b < 0 are left unwritten
-        (idx_b is None when no frame has a second keyframe)."""
+        (idx_b is None when no frame has a second keyframe).  Both operands may have any layout and start at any element
+        offset."""
         F_, S, dim = x_unit.shape
         K = piv_unit.shape[0]
         assert x_unit.dtype == torch.float16 and piv_unit.dtype == torch.float16
-        x_unit = x_unit.contiguous()
-        piv_unit = piv_unit.contiguous()
+        x_unit, piv_unit = _dense(x_unit), _dense(piv_unit)
         idx_a = torch.empty((F_, S), dtype=torch.int32, device=x_unit.device)
         any_b = any(int(b) >= 0 for b in kf_b)
         idx_b = torch.empty((F_, S), dtype=torch.int32, device=x_unit.device) if any_b else None
@@ -338,15 +366,15 @@ class CudaOps:
                   kf_a: Sequence[int], kf_b: Sequence[int], w: Sequence[float],
                   residual: Optional[torch.Tensor], out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
         """A [3,K,S,dim] fp16; idx [F,S] int32; residual [3F,S,dim] fp16 or None → [3F,S,dim]
-        (reference tokenflow_utils.py:361-397)."""
+        (reference tokenflow_utils.py:361-397).  A and residual may have any layout and start at any element offset,
+        the int32 indices at any element offset."""
         three, K, S, dim = A.shape
         out_dtype = torch.float16 if out_dtype is None else out_dtype
-        if A.dtype != torch.float16 or not A.is_contiguous():
-            A = A.to(torch.float16).contiguous()
+        A = _dense(A.to(torch.float16))
         assert three == 3
         F_ = idx_a.shape[0]
         if residual is not None:
-            residual = residual.to(torch.float16).contiguous().view(3, F_, S, dim)
+            residual = _dense(residual.to(torch.float16)).view(3, F_, S, dim)
         out = torch.empty((3, F_, S, dim), dtype=out_dtype, device=A.device)
         assert out_dtype in (torch.float16, torch.float32)
         self._timed("tf_propagate", propagate_bytes(F_, S, dim, kf_a, kf_b, residual is not None,
@@ -360,15 +388,16 @@ class CudaOps:
     def ext_attn(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, scale: float,
                  inject: bool) -> torch.Tensor:
         """q,k,v [3n,S,dim] fp16 (same token stride) → [3n,S,dim] fp16, before to_out
-        (reference tokenflow_utils.py:124-197 / :234-279)."""
+        (reference tokenflow_utils.py:124-197 / :234-279).  q, k and v may start at any element offset; views with
+        other strides are copied."""
         b, S, dim = q.shape
         n = b // 3
         d = dim // heads
         q, k, v = (t if t.dtype == torch.float16 else t.to(torch.float16) for t in (q, k, v))
         strides = {(t.stride(0), t.stride(1), t.stride(2)) for t in (q, k, v)}
         tok = q.stride(1)
-        if len(strides) != 1 or q.stride(2) != 1 or q.stride(0) != S * tok:
-            q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
+        if len(strides) != 1 or q.stride(2) != 1 or q.stride(0) != S * tok or any(t.data_ptr() % 16 for t in (q, k, v)):
+            q, k, v = _dense(q), _dense(k), _dense(v)
             tok = dim
         out = torch.empty((b, S, dim), dtype=torch.float16, device=q.device)
         flops = 4.0 * n * S * S * dim * (2 * n + 1)        # QK^T + PV; source: S keys, uncond+cond: n*S keys
@@ -381,13 +410,14 @@ class CudaOps:
     @staticmethod
     def _slab_view(t: torch.Tensor):
         """(tensor, token stride) of a [slabs, S, dim] fp16 operand the kernels can address in place: last dim
-        contiguous, slabs S tokens apart (a column slice of a packed [slabs, S, n*dim] buffer qualifies)."""
+        contiguous, slabs S tokens apart (a column slice of a packed [slabs, S, n*dim] buffer qualifies), 16-byte aligned;
+        anything else is copied."""
         if t.dtype != torch.float16:
             t = t.to(torch.float16)
         S = t.shape[1]
         if t.stride(2) != 1 or t.stride(1) % 8 or (t.shape[0] > 1 and t.stride(0) != S * t.stride(1)) \
                 or t.data_ptr() % 16:
-            t = t.contiguous()
+            t = _dense(t)
         return t, t.stride(1)
 
     def ext_attn_table(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, table, heads: int,
@@ -440,12 +470,13 @@ class CudaOps:
         out, with the eager fp16 rounding sequence.  `bias` is fp16 [N, C] or [1, C] (the resnet's time-embedding
         projection), and None at 4 channels per group.  Two launches, timed as "tf_group_norm_g4" at 4 channels per
         group (the VAE's 128-channel levels) and "tf_group_norm" otherwise; the statistics workspace comes from the
-        caching allocator on this stream."""
+        caching allocator on this stream.  x and bias may start at any element offset."""
         n, c, h, w = x.shape
+        x = _dense(x, torch.channels_last)
         if bias is not None:
             assert bias.dtype == torch.float16 and bias.dim() == 2 and bias.shape[1] == c and bias.shape[0] in (1, n)
             if bias.stride(1) != 1 or bias.stride(0) % 8 or bias.data_ptr() % 16:
-                bias = bias.contiguous()
+                bias = bias.clone(memory_format=torch.contiguous_format)
             bias_stride = 0 if bias.shape[0] == 1 else bias.stride(0)
         ws_bytes = int(self.lib.tf_group_norm_nhwc_workspace(n, h * w, c, norm.num_groups))
         if ws_bytes < 0:
@@ -462,10 +493,10 @@ class CudaOps:
 
     def frames_to_nhwc(self, frames: torch.Tensor) -> torch.Tensor:
         """uint8 RGB frames [N, H, W, 3] (CUDA) -> the encoder input 2 * ToTensor(frames) - 1 as a channels_last fp16
-        [N, 3, H, W] tensor, bit-equal to the reference's host conversion followed by the fp16 ops."""
+        [N, 3, H, W] tensor, bit-equal to the reference's host conversion followed by the fp16 ops.  `frames` may start
+        at any element offset."""
         assert frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[-1] == 3 and frames.is_cuda
-        if not frames.is_contiguous() or frames.data_ptr() % 16:
-            frames = frames.contiguous()
+        frames = _dense(frames)
         n, h, w, _ = frames.shape
         out = torch.empty((n, 3, h, w), dtype=torch.float16, device=frames.device, memory_format=torch.channels_last)
         self._timed("tf_frames_to_nhwc", 3.0 * n * h * w, lambda: self._check(self.lib.tf_frames_to_nhwc(
@@ -474,10 +505,9 @@ class CudaOps:
 
     def nhwc_to_frames(self, x: torch.Tensor) -> torch.Tensor:
         """fp16 decoder output [N, 3, H, W] -> uint8 frames [N, H, W, 3], bit-equal to
-        `((x / 2 + 0.5).clamp(0, 1) * 255).to(torch.uint8)` in fp16 (NaN -> 0)."""
+        `((x / 2 + 0.5).clamp(0, 1) * 255).to(torch.uint8)` in fp16 (NaN -> 0).  x may start at any element offset."""
         assert x.dtype == torch.float16 and x.dim() == 4 and x.shape[1] == 3 and x.is_cuda
-        if not x.is_contiguous(memory_format=torch.channels_last) or x.data_ptr() % 16:
-            x = x.contiguous(memory_format=torch.channels_last)
+        x = _dense(x, torch.channels_last)
         n, _, h, w = x.shape
         out = torch.empty((n, h, w, 3), dtype=torch.uint8, device=x.device)
         self._timed("tf_nhwc_to_frames", 3.0 * n * h * w, lambda: self._check(self.lib.tf_nhwc_to_frames(
@@ -502,7 +532,7 @@ class CudaOps:
                       out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """uint8 RGB frames [N, H_in, W_in, 3] (CUDA) -> [N, H, W, 3] for size = (H, W), bit-equal to PIL's
         `Image.resize((W, H), Image.LANCZOS)` of every frame.  `tmp` ([N, H_in, W, 3] uint8) and `out` may be given;
-        they are made here otherwise."""
+        they are made here otherwise.  Every buffer may start at any element offset (the kernels read and write bytes)."""
         assert frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[-1] == 3 and frames.is_cuda
         frames = frames.contiguous()
         n, h_in, w_in, _ = frames.shape
@@ -530,7 +560,7 @@ class CudaOps:
         """uint8 RGB frames [N, H, W, 3] (CUDA) -> (edges, cond): `cv2.Canny(frame, low, high)` of every frame as uint8
         [N, H, W] (0 / 255) and the reference's `get_canny_cond` tensor, fp16 [N, 3, H, W] channels_last with 0 / 1 in
         every channel.  Either output can be skipped (None is returned in its place) or given.  The workspace comes from
-        the caching allocator on this stream."""
+        the caching allocator on this stream.  Frames and outputs may start at any element offset."""
         assert frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[-1] == 3 and frames.is_cuda
         assert edges or cond
         frames = frames.contiguous()
@@ -556,9 +586,10 @@ class CudaOps:
         return e, c
 
     def geglu(self, xh: torch.Tensor, gate: torch.Tensor) -> torch.Tensor:
-        """xh * gelu(gate) of two fp16 tensors of one shape (the GEGLU GEMM outputs), bit-equal to the eager product."""
+        """xh * gelu(gate) of two fp16 tensors of one shape (the GEGLU GEMM outputs), bit-equal to the eager product.
+        Both may start at any element offset."""
         assert xh.dtype == gate.dtype == torch.float16 and xh.shape == gate.shape
-        xh, gate = (t if t.is_contiguous() and t.data_ptr() % 16 == 0 else t.contiguous() for t in (xh, gate))
+        xh, gate = _dense(xh), _dense(gate)
         out = torch.empty_like(xh)
         n = xh.numel()
         self._timed("tf_geglu", 3.0 * n * 2, lambda: self._check(
