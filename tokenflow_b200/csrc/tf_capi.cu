@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "../../include/tokenflow_b200.h"
+#include "../../include/tokenflow_b200_vpred.h"
 #include "tf_common.cuh"
 #include "tf_kernels.h"
 
@@ -132,7 +133,7 @@ using namespace tf;
 
 extern "C" {
 
-int tf_version(void) { return 1003; }
+int tf_version(void) { return 1004; }
 
 const char* tf_last_error(void) { return g_err; }
 
@@ -219,6 +220,32 @@ int tf_ddim(const void* eps, const void* x, const float* coef, int64_t n, void* 
     return TF_ERR_INVALID_ARGUMENT;
   }
   int e = launch_ddim(eps, x, coef, n, out, static_cast<cudaStream_t>(stream));
+  if (!e) g_launches += 1;
+  return e;
+}
+
+int tf_cfg_ddim_v(const void* v_uncond, const void* v_cond, const void* x, const float* coef, float guidance,
+                  int64_t n, void* out, tf_stream_t stream) {
+  if (n < 0) { set_last_error("tf_cfg_ddim_v: n=%lld", (long long)n); return TF_ERR_INVALID_ARGUMENT; }
+  if (n == 0) return TF_OK;
+  if (!v_uncond || !v_cond || !x || !coef || !out || !aligned16(v_uncond) || !aligned16(v_cond) || !aligned16(x) ||
+      !aligned16(out)) {
+    set_last_error("tf_cfg_ddim_v: NULL or misaligned pointer");
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  int e = launch_cfg_ddim_v(v_uncond, v_cond, x, coef, guidance, n, out, static_cast<cudaStream_t>(stream));
+  if (!e) g_launches += 1;
+  return e;
+}
+
+int tf_ddim_v(const void* v, const void* x, const float* coef, int64_t n, void* out, tf_stream_t stream) {
+  if (n < 0) { set_last_error("tf_ddim_v: n=%lld", (long long)n); return TF_ERR_INVALID_ARGUMENT; }
+  if (n == 0) return TF_OK;
+  if (!v || !x || !coef || !out || !aligned16(v) || !aligned16(x) || !aligned16(out)) {
+    set_last_error("tf_ddim_v: NULL or misaligned pointer");
+    return TF_ERR_INVALID_ARGUMENT;
+  }
+  int e = launch_ddim_v(v, x, coef, n, out, static_cast<cudaStream_t>(stream));
   if (!e) g_launches += 1;
   return e;
 }

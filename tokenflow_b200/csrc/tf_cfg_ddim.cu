@@ -18,6 +18,13 @@
 // tf_ddim is the same DDIM update without the guidance (the inversion stage's two directions), with the
 // coefficients of the direction it runs: inversion s1 = sigma_prev, inv_s2 = 1/mu_prev, s3 = mu, s4 = sigma;
 // reconstruction s1 = sigma, inv_s2 = 1/mu, s3 = mu_prev, s4 = sigma_prev.
+//
+// tf_cfg_ddim_v / tf_ddim_v are the same two kernels for a model that predicts the velocity
+// v = sqrt(alpha) * eps - sqrt(1 - alpha) * x0 (Stable Diffusion 2.x at 768^2), with diffusers' v-branch of
+// DDIMScheduler.step (eta = 0) as the DDIM half.  The coefficient row (a, b, c, d) is
+// (sqrt(alpha_t), sqrt(1 - alpha_t), sqrt(alpha_prev), sqrt(1 - alpha_prev)) for the edit, (mu_prev, sigma_prev,
+// mu, sigma) for the inversion and (mu, sigma, mu_prev, sigma_prev) for the reconstruction:
+//     p = h(h(a * x) - h(b * v))     e = h(h(a * v) + h(b * x))     out = h(h(c * p) + h(d * e))
 #include "tf_common.cuh"
 #include "tf_kernels.h"
 
@@ -26,20 +33,37 @@ namespace {
 
 __device__ __forceinline__ float rh(float x) { return __half2float(__float2half_rn(x)); }
 
-// The DDIM half of the step, shared by both kernels so the rounding sequence lives in one place:
-// out = h(h(s3 * h(h(x - h(s1 * e)) * inv_s2)) + h(s4 * e)).
-__device__ __forceinline__ float ddim_one(float e, float xv, float s1, float inv_s2, float s3, float s4) {
+// What the model predicts: the parameterisation selects the DDIM half of the step, nothing else.
+enum class Pred { kEps, kV };
+
+// The DDIM half of the step, shared by both kernels so each rounding sequence lives in one place.  `m` is the model
+// output (after guidance, for tf_cfg_ddim[_v]), `xv` the latent, (k0, k1, k2, k3) the coefficient row.
+template <Pred P>
+__device__ __forceinline__ float ddim_one(float m, float xv, float k0, float k1, float k2, float k3);
+
+// eps: out = h(h(s3 * h(h(x - h(s1 * e)) * inv_s2)) + h(s4 * e)).
+template <>
+__device__ __forceinline__ float ddim_one<Pred::kEps>(float e, float xv, float s1, float inv_s2, float s3, float s4) {
   const float p = rh(rh(xv - rh(s1 * e)) * inv_s2);
   return rh(rh(s3 * p) + rh(s4 * e));
 }
 
+// v: pred_x0 = h(h(a * x) - h(b * v)), pred_eps = h(h(a * v) + h(b * x)), out = h(h(c * pred_x0) + h(d * pred_eps)).
+template <>
+__device__ __forceinline__ float ddim_one<Pred::kV>(float v, float xv, float a, float b, float c, float d) {
+  const float p = rh(rh(a * xv) - rh(b * v));
+  const float e = rh(rh(a * v) + rh(b * xv));
+  return rh(rh(c * p) + rh(d * e));
+}
+
+template <Pred P>
 __global__ void __launch_bounds__(256)
 cfg_ddim_kernel(const __half* __restrict__ eu, const __half* __restrict__ ec, const __half* __restrict__ x,
                 const float* __restrict__ coef, float g, long long n_vec, long long n, __half* __restrict__ out) {
-  const float s1 = coef[0], inv_s2 = coef[1], s3 = coef[2], s4 = coef[3];
+  const float k0 = coef[0], k1 = coef[1], k2 = coef[2], k3 = coef[3];
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   auto one = [&](float u, float c, float xv) -> float {
-    return ddim_one(rh(u + rh(g * rh(c - u))), xv, s1, inv_s2, s3, s4);
+    return ddim_one<P>(rh(u + rh(g * rh(c - u))), xv, k0, k1, k2, k3);
   };
   if (i < n_vec) {
     const uint4 ru = reinterpret_cast<const uint4*>(eu)[i];
@@ -64,12 +88,13 @@ cfg_ddim_kernel(const __half* __restrict__ eu, const __half* __restrict__ ec, co
 }
 
 // Guidance-free DDIM update (both directions of the inversion stage, reference preprocess.py:217-225 and
-// :251-260): one read of eps and x, one write.  `out` may alias `x`: every element is read before it is
-// written by the same thread.
+// :251-260): one read of the model output and x, one write.  `out` may alias `x`: every element is read before it
+// is written by the same thread.
+template <Pred P>
 __global__ void __launch_bounds__(256)
 ddim_kernel(const __half* __restrict__ eps, const __half* x, const float* __restrict__ coef, long long n_vec,
             long long n, __half* out) {
-  const float s1 = coef[0], inv_s2 = coef[1], s3 = coef[2], s4 = coef[3];
+  const float k0 = coef[0], k1 = coef[1], k2 = coef[2], k3 = coef[3];
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n_vec) {
     const uint4 re = reinterpret_cast<const uint4*>(eps)[i];
@@ -81,38 +106,62 @@ ddim_kernel(const __half* __restrict__ eps, const __half* x, const float* __rest
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       const float2 ev = __half22float2(he[e]), xv = __half22float2(hx[e]);
-      ho[e] = __floats2half2_rn(ddim_one(ev.x, xv.x, s1, inv_s2, s3, s4), ddim_one(ev.y, xv.y, s1, inv_s2, s3, s4));
+      ho[e] = __floats2half2_rn(ddim_one<P>(ev.x, xv.x, k0, k1, k2, k3), ddim_one<P>(ev.y, xv.y, k0, k1, k2, k3));
     }
     reinterpret_cast<uint4*>(out)[i] = w;
   }
   if (i == 0) {                                   // tail (n not a multiple of 8)
     for (long long j = n_vec * 8; j < n; ++j)
-      out[j] = __float2half_rn(ddim_one(__half2float(eps[j]), __half2float(x[j]), s1, inv_s2, s3, s4));
+      out[j] = __float2half_rn(ddim_one<P>(__half2float(eps[j]), __half2float(x[j]), k0, k1, k2, k3));
   }
+}
+
+unsigned blocks_for(long long n_vec) {
+  const long long threads = n_vec > 0 ? n_vec : 1;
+  return (unsigned)((threads + 255) / 256);
+}
+
+template <Pred P>
+int launch_ddim_as(const void* eps, const void* x, const float* coef_dev, long long n, void* out, cudaStream_t stream,
+                   const char* what) {
+  if (n == 0) return TF_OK;
+  const long long n_vec = n / 8;
+  ddim_kernel<P><<<blocks_for(n_vec), 256, 0, stream>>>(static_cast<const __half*>(eps), static_cast<const __half*>(x),
+                                                        coef_dev, n_vec, n, static_cast<__half*>(out));
+  return check_cuda(cudaGetLastError(), what);
+}
+
+template <Pred P>
+int launch_cfg_ddim_as(const void* eps_uncond, const void* eps_cond, const void* x, const float* coef_dev,
+                       float guidance, long long n, void* out, cudaStream_t stream, const char* what) {
+  if (n == 0) return TF_OK;
+  const long long n_vec = n / 8;
+  cfg_ddim_kernel<P><<<blocks_for(n_vec), 256, 0, stream>>>(
+      static_cast<const __half*>(eps_uncond), static_cast<const __half*>(eps_cond), static_cast<const __half*>(x),
+      coef_dev, guidance, n_vec, n, static_cast<__half*>(out));
+  return check_cuda(cudaGetLastError(), what);
 }
 
 }  // namespace
 
 int launch_ddim(const void* eps, const void* x, const float* coef_dev, long long n, void* out, cudaStream_t stream) {
-  if (n == 0) return TF_OK;
-  const long long n_vec = n / 8;
-  const long long threads = n_vec > 0 ? n_vec : 1;
-  const unsigned blocks = (unsigned)((threads + 255) / 256);
-  ddim_kernel<<<blocks, 256, 0, stream>>>(static_cast<const __half*>(eps), static_cast<const __half*>(x), coef_dev,
-                                          n_vec, n, static_cast<__half*>(out));
-  return check_cuda(cudaGetLastError(), "tf_ddim launch");
+  return launch_ddim_as<Pred::kEps>(eps, x, coef_dev, n, out, stream, "tf_ddim launch");
+}
+
+int launch_ddim_v(const void* v, const void* x, const float* coef_dev, long long n, void* out, cudaStream_t stream) {
+  return launch_ddim_as<Pred::kV>(v, x, coef_dev, n, out, stream, "tf_ddim_v launch");
 }
 
 int launch_cfg_ddim(const void* eps_uncond, const void* eps_cond, const void* x, const float* coef_dev, float guidance,
                     long long n, void* out, cudaStream_t stream) {
-  if (n == 0) return TF_OK;
-  const long long n_vec = n / 8;
-  const long long threads = n_vec > 0 ? n_vec : 1;
-  const unsigned blocks = (unsigned)((threads + 255) / 256);
-  cfg_ddim_kernel<<<blocks, 256, 0, stream>>>(static_cast<const __half*>(eps_uncond), static_cast<const __half*>(eps_cond),
-                                             static_cast<const __half*>(x), coef_dev, guidance, n_vec, n,
-                                             static_cast<__half*>(out));
-  return check_cuda(cudaGetLastError(), "tf_cfg_ddim launch");
+  return launch_cfg_ddim_as<Pred::kEps>(eps_uncond, eps_cond, x, coef_dev, guidance, n, out, stream,
+                                        "tf_cfg_ddim launch");
+}
+
+int launch_cfg_ddim_v(const void* v_uncond, const void* v_cond, const void* x, const float* coef_dev, float guidance,
+                      long long n, void* out, cudaStream_t stream) {
+  return launch_cfg_ddim_as<Pred::kV>(v_uncond, v_cond, x, coef_dev, guidance, n, out, stream,
+                                      "tf_cfg_ddim_v launch");
 }
 
 }  // namespace tf

@@ -85,6 +85,7 @@ class TokenFlowEditor(nn.Module):
         self.comm = None                      # ops.Communicator (C-ABI NCCL all-gather), see attach_communicator
         # DDIM coefficients per schedule position, on the device, for the fused CFG+DDIM kernel:
         # sqrt(1-a_t), 1/sqrt(a_t), sqrt(a_prev), sqrt(1-a_prev) as the fp32 values the eager expression uses
+        # (a v-prediction scheduler: sqrt(a_t), sqrt(1-a_t), sqrt(a_prev), sqrt(1-a_prev))
         self._coef_table = self._make_coef_table()
         self._graphs = {}                     # injection variant -> captured step
         self._graph_pool = None
@@ -175,6 +176,11 @@ class TokenFlowEditor(nn.Module):
         for t in self._t_host:
             a_t = float(sch._alpha(t))
             a_prev = float(sch._alpha(t - ratio))
+            if sch.prediction_type == "v_prediction":
+                # tf_cfg_ddim_v: the step multiplies by the Python floats below, which ATen rounds to fp32
+                rows.append([float(np.float32(v)) for v in (a_t ** 0.5, (1 - a_t) ** 0.5, a_prev ** 0.5,
+                                                             (1 - a_prev) ** 0.5)])
+                continue
             # the step divides the fp16 latents by the Python float sqrt(a_t): ATen multiplies by the reciprocal taken in
             # double and rounded to fp32, which is not always the fp32 reciprocal of the fp32 sqrt (50 steps: 8 rows)
             s1 = np.float32((1 - a_t) ** 0.5)
@@ -304,7 +310,8 @@ class TokenFlowEditor(nn.Module):
         _, npu, npc = noise_pred.chunk(3)
         ops = self._cuda_ops()
         if ops is not None and coef is not None and npu.dtype == torch.float16 and xs.dtype == torch.float16:
-            x_local = ops.cfg_ddim(npu, npc, xs, coef, self.config["guidance_scale"])     # one kernel, same roundings
+            step = ops.cfg_ddim_v if self.scheduler.prediction_type == "v_prediction" else ops.cfg_ddim
+            x_local = step(npu, npc, xs, coef, self.config["guidance_scale"])     # one kernel, same roundings
         else:
             noise_pred = npu + self.config["guidance_scale"] * (npc - npu)
             x_local = self.scheduler.step(noise_pred, t_int, xs)['prev_sample'].contiguous()

@@ -76,6 +76,13 @@ _SIGNATURES = {
     "tf_geglu": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
 }
 
+# the v-prediction latent updates; mirrors include/tokenflow_b200_vpred.h one to one (same library, same signatures as
+# tf_cfg_ddim / tf_ddim)
+_VPRED_SIGNATURES = {
+    "tf_cfg_ddim_v": _SIGNATURES["tf_cfg_ddim"],
+    "tf_ddim_v": _SIGNATURES["tf_ddim"],
+}
+
 
 class TokenflowB200Error(RuntimeError):
     pass
@@ -99,7 +106,7 @@ def load_library() -> ctypes.CDLL:
             f"{path} is missing: build it with `python -m tokenflow_b200._build` "
             "(or __graft_entry__.build()).  tokenflow_b200 has no fallback path.")
     lib = ctypes.CDLL(str(path))
-    for name, (res, args) in _SIGNATURES.items():
+    for name, (res, args) in list(_SIGNATURES.items()) + list(_VPRED_SIGNATURES.items()):
         fn = getattr(lib, name)           # AttributeError here = header and library disagree
         fn.restype = res
         fn.argtypes = args
@@ -311,17 +318,28 @@ class CudaOps:
         `coef` = device fp32 [4]: sqrt(1-a_t), 1/sqrt(a_t), sqrt(a_prev), sqrt(1-a_prev).  The operands may have any
         layout and start at any element offset; `out` (contiguous, made here when None) too: a misaligned one is
         written through an aligned buffer and a copy."""
-        assert eps_uncond.dtype == eps_cond.dtype == x.dtype == torch.float16 and coef.dtype == torch.float32
-        eu, ec, xx = (_dense(t) for t in (eps_uncond, eps_cond, x))
+        return self._cfg_step("tf_cfg_ddim", eps_uncond, eps_cond, x, coef, guidance, out)
+
+    def cfg_ddim_v(self, v_uncond: torch.Tensor, v_cond: torch.Tensor, x: torch.Tensor, coef: torch.Tensor,
+                   guidance: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """`cfg_ddim` for a v-prediction model (include/tokenflow_b200_vpred.h): guidance on the two velocity
+        predictions, then diffusers' v-branch of the DDIM step; `coef` = device fp32 [4]: sqrt(a_t), sqrt(1-a_t),
+        sqrt(a_prev), sqrt(1-a_prev).  Operands and `out` as in `cfg_ddim`."""
+        return self._cfg_step("tf_cfg_ddim_v", v_uncond, v_cond, x, coef, guidance, out)
+
+    def _cfg_step(self, fn: str, u: torch.Tensor, c: torch.Tensor, x: torch.Tensor, coef: torch.Tensor,
+                  guidance: float, out: Optional[torch.Tensor]) -> torch.Tensor:
+        assert u.dtype == c.dtype == x.dtype == torch.float16 and coef.dtype == torch.float32
+        eu, ec, xx = (_dense(t) for t in (u, c, x))
         assert eu.shape == ec.shape == xx.shape
         if out is None:
             out = torch.empty_like(xx)
         assert out.shape == xx.shape and out.dtype == torch.float16 and out.is_contiguous()
         dst = out if out.data_ptr() % 16 == 0 else torch.empty_like(xx)
         n = xx.numel()
-        self._timed("tf_cfg_ddim", n * 8.0, lambda: self._check(
-            self.lib.tf_cfg_ddim(eu.data_ptr(), ec.data_ptr(), xx.data_ptr(), coef.data_ptr(), float(guidance), n,
-                                 dst.data_ptr(), self._stream()), "tf_cfg_ddim"))
+        self._timed(fn, n * 8.0, lambda: self._check(
+            getattr(self.lib, fn)(eu.data_ptr(), ec.data_ptr(), xx.data_ptr(), coef.data_ptr(), float(guidance), n,
+                                  dst.data_ptr(), self._stream()), fn))
         return out if dst is out else out.copy_(dst)
 
     def ddim(self, eps: torch.Tensor, x: torch.Tensor, coef: torch.Tensor,
@@ -331,16 +349,27 @@ class CudaOps:
         eps may have any layout; x and `out` are contiguous.  All three may start at any element offset: a misaligned
         operand is read from an aligned copy, a misaligned `out` (or `x`, in place) is written through an aligned
         buffer and a copy back."""
-        assert eps.dtype == x.dtype == torch.float16 and coef.dtype == torch.float32 and coef.is_cuda
-        assert eps.shape == x.shape
+        return self._step("tf_ddim", eps, x, coef, out)
+
+    def ddim_v(self, v: torch.Tensor, x: torch.Tensor, coef: torch.Tensor,
+               out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """`ddim` for a v-prediction model (include/tokenflow_b200_vpred.h), diffusers' DDIMInverseScheduler /
+        DDIMScheduler v-branch; `coef` = device fp32 [4]: inversion (mu_prev, sigma_prev, mu, sigma), reconstruction
+        (mu, sigma, mu_prev, sigma_prev).  Operands, `out` and in place as in `ddim`."""
+        return self._step("tf_ddim_v", v, x, coef, out)
+
+    def _step(self, fn: str, m: torch.Tensor, x: torch.Tensor, coef: torch.Tensor,
+              out: Optional[torch.Tensor]) -> torch.Tensor:
+        assert m.dtype == x.dtype == torch.float16 and coef.dtype == torch.float32 and coef.is_cuda
+        assert m.shape == x.shape
         if out is None:
             out = torch.empty_like(x, memory_format=torch.contiguous_format)
         assert out.shape == x.shape and out.dtype == torch.float16 and out.is_contiguous() and x.is_contiguous()
-        e, xx = _dense(eps), _dense(x)
+        e, xx = _dense(m), _dense(x)
         dst = xx if out is x else (out if out.data_ptr() % 16 == 0 else torch.empty_like(out))
         n = x.numel()
-        self._timed("tf_ddim", n * 6.0, lambda: self._check(
-            self.lib.tf_ddim(e.data_ptr(), xx.data_ptr(), coef.data_ptr(), n, dst.data_ptr(), self._stream()), "tf_ddim"))
+        self._timed(fn, n * 6.0, lambda: self._check(
+            getattr(self.lib, fn)(e.data_ptr(), xx.data_ptr(), coef.data_ptr(), n, dst.data_ptr(), self._stream()), fn))
         return out if dst is out else out.copy_(dst)
 
     def nn_field(self, x_unit: torch.Tensor, piv_unit: torch.Tensor, kf_a: Sequence[int],

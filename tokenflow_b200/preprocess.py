@@ -18,9 +18,9 @@ inverts its own contiguous share and the saved tensors are all-gathered.
 Two paths compute the same steps:
   * CPU / fp32 UNet: the eager loop below, step by step as the reference writes it;
   * CUDA fp16 UNet: one CUDA graph of a step over the rank's share (the UNet calls in batches of `batch_size`, then the
-    DDIM update `tf_ddim` in place), replayed for every step of both directions.  The step's timestep and its four
-    DDIM coefficients are read from device buffers the host refreshes per replay; saved timesteps are device-to-device
-    copies into one resident buffer, all-gathered once at the end.
+    DDIM update `tf_ddim` in place, `tf_ddim_v` for a v-prediction scheduler), replayed for every step of both
+    directions.  The step's timestep and its four DDIM coefficients are read from device buffers the host refreshes per
+    replay; saved timesteps are device-to-device copies into one resident buffer, all-gathered once at the end.
 """
 from __future__ import annotations
 
@@ -41,11 +41,16 @@ def inversion_coef_tables(scheduler) -> Tuple[torch.Tensor, torch.Tensor]:
     `mu` as a multiply by the fp32 reciprocal 1 / mu.  `final_alpha_cumprod` stands in for the missing neighbour at
     both ends of the grid.
     inversion step i (t = ts_up[i], prev = ts_up[i - 1]):     sigma_prev, 1 / mu_prev, mu, sigma
-    reconstruction step i (t = ts_dn[i], prev = ts_dn[i + 1]): sigma, 1 / mu, mu_prev, sigma_prev"""
+    reconstruction step i (t = ts_dn[i], prev = ts_dn[i + 1]): sigma, 1 / mu, mu_prev, sigma_prev
+
+    For a v-prediction scheduler the rows are those of `tf_ddim_v` (diffusers' DDIMInverseScheduler / DDIMScheduler
+    v-branch, which multiplies by every coefficient and divides by none), from the same 0-dim fp32 alphas:
+    inversion (mu_prev, sigma_prev, mu, sigma), reconstruction (mu, sigma, mu_prev, sigma_prev)."""
     a = scheduler.alphas_cumprod.cpu()
     final = scheduler.final_alpha_cumprod.cpu()
     ts_dn = [int(t) for t in scheduler.timesteps.tolist()]
     ts_up = ts_dn[::-1]
+    v = scheduler.prediction_type == "v_prediction"
     # 0-dim CPU tensor arithmetic, one step at a time, exactly as the reference evaluates it (the CPU's fp32 sqrt is
     # ATen's, which need not be the correctly rounded one)
     mu_sigma = lambda alpha: (alpha ** 0.5, (1 - alpha) ** 0.5)
@@ -53,11 +58,11 @@ def inversion_coef_tables(scheduler) -> Tuple[torch.Tensor, torch.Tensor]:
     for i, t in enumerate(ts_up):
         mu, sigma = mu_sigma(a[t])
         mu_p, sigma_p = mu_sigma(a[ts_up[i - 1]] if i > 0 else final)
-        inv.append(torch.stack([sigma_p, 1 / mu_p, mu, sigma]))
+        inv.append(torch.stack([mu_p, sigma_p, mu, sigma] if v else [sigma_p, 1 / mu_p, mu, sigma]))
     for i, t in enumerate(ts_dn):
         mu, sigma = mu_sigma(a[t])
         mu_p, sigma_p = mu_sigma(a[ts_dn[i + 1]] if i < len(ts_dn) - 1 else final)
-        rec.append(torch.stack([sigma, 1 / mu, mu_p, sigma_p]))
+        rec.append(torch.stack([mu, sigma, mu_p, sigma_p] if v else [sigma, 1 / mu, mu_p, sigma_p]))
     return torch.stack(inv), torch.stack(rec)
 
 
@@ -151,9 +156,7 @@ class LatentInverter:
             mu, sigma, mu_prev, sigma_prev = self._alphas(t, ts[i - 1] if i > 0 else None)
             for b in range(0, x.shape[0], batch_size):
                 xb = x[b:b + batch_size]
-                eps = self._eps(xb, t, cond, lo + b)
-                pred_x0 = (xb - sigma_prev * eps) / mu_prev
-                x[b:b + batch_size] = mu * pred_x0 + sigma * eps
+                x[b:b + batch_size] = self._update(xb, self._eps(xb, t, cond, lo + b), mu_prev, sigma_prev, mu, sigma)
             if save_latents and save_path is not None and (t in keep or i == len(ts) - 1):
                 full = self._gathered(x, n)
                 if self.rank == 0:
@@ -174,10 +177,19 @@ class LatentInverter:
             mu, sigma, mu_prev, sigma_prev = self._alphas(t, ts[i + 1] if i < len(ts) - 1 else None)
             for b in range(0, x.shape[0], batch_size):
                 xb = x[b:b + batch_size]
-                eps = self._eps(xb, t, cond, lo + b)
-                pred_x0 = (xb - sigma * eps) / mu
-                x[b:b + batch_size] = mu_prev * pred_x0 + sigma_prev * eps
+                x[b:b + batch_size] = self._update(xb, self._eps(xb, t, cond, lo + b), mu, sigma, mu_prev, sigma_prev)
         return self._gathered(x, n)
+
+    def _update(self, x, m, mu_from, sigma_from, mu_to, sigma_to):
+        """One DDIM step of the eager loop from the level of x (mu_from, sigma_from) to the next (mu_to, sigma_to), for
+        the model output m: the reference's eps update (preprocess.py:224-225 / :259-260), or for a v-prediction
+        scheduler diffusers' DDIMInverseScheduler / DDIMScheduler v-branch (the reference has none)."""
+        if self.scheduler.prediction_type == "v_prediction":
+            pred_x0 = mu_from * x - sigma_from * m
+            pred_eps = mu_from * m + sigma_from * x
+            return mu_to * pred_x0 + sigma_to * pred_eps
+        pred_x0 = (x - sigma_from * m) / mu_from
+        return mu_to * pred_x0 + sigma_to * m
 
     # -- CUDA fp16: graph-replayed steps ------------------------------------------------------------------------
     def _graphed_path(self) -> bool:
@@ -202,6 +214,7 @@ class LatentInverter:
         from . import tokenflow_utils as tfu
         from .controlnet import controlnet_residuals
         ops = tfu._ops()                      # the library is required: raises without it or without an H100
+        update = ops.ddim_v if self.scheduler.prediction_type == "v_prediction" else ops.ddim
         bs = max(1, min(batch_size, share))
         key = (share, tuple(shape), bs, tuple(cond.shape[1:]), self._use_graph, self.controlnet is not None)
         entry = self._graphs.get(key)
@@ -231,7 +244,7 @@ class LatentInverter:
                 out = self.unet(xb, st["t"], encoder_hidden_states=ctx, **res)
                 outs.append(out["sample"] if isinstance(out, dict) else out.sample)
             eps = outs[0] if len(outs) == 1 else torch.cat(outs)
-            ops.ddim(eps, x, st["coef"], out=x)
+            update(eps, x, st["coef"], out=x)
 
         entry = {"st": st, "cond": st["cond"], "step": step, "graph": None}
         if self._use_graph and share > 0:
