@@ -74,6 +74,8 @@ int tf_layernorm_rows(const void* x_f16, int64_t rows, int dim, int64_t x_row_st
  * fp16 output under autocast, and the two argmax reductions :340-343):
  *   idx_a[f,p] = argmax_c fp16( x_unit[f,p,:] . piv_unit[kf_a[f],c,:] )     first index on ties
  *   idx_b[f,p] = same against keyframe kf_b[f]            (skipped for frames with kf_b[f] < 0)
+ *   ordered as torch.argmax orders them: a NaN similarity (the unit row of a zero token is NaN) ranks above
+ *   every number and the first NaN wins, so a zero pivot token c gives c, a zero frame token 0
  *   x_unit    device [F, S, dim] fp16 unit rows (tf_unit_rows of the source-stream norm1 output)
  *   piv_unit  device [K, S, dim] fp16 unit rows of the cached source-stream pivot features
  *   kf_a,kf_b host   [F] keyframe ids in [0,K); reference batch i: kf_a = i, kf_b = i-1 (or -1)

@@ -41,9 +41,12 @@ maximum that arrives in the last tile far above everything before it) and return
 realise, so a test can assert that the band it meant was hit.
 
 `check_nn_field` is the one implementation of the NN-field rule: every index equals the argmax of the
-kernel's own fp16 operands (dot products accumulated in fp64, rounded to fp16, first index on ties), up to
-rows inside a 1-ulp fp16 tie class, whose winner depends on the GEMM's fp32 accumulation order.  Such
-rows are bounded and counted.
+kernel's own fp16 operands (dot products accumulated in fp64, rounded to fp16, first index on ties, a NaN
+similarity above every number as in torch.argmax: `nn_argmax`), up to rows inside a 1-ulp fp16 tie class,
+whose winner depends on the GEMM's fp32 accumulation order.  Such rows are bounded and counted.
+
+`propagate_exact` restates tf_propagate in numpy float32 from the reference expression, for bit-for-bit
+comparison (`bit_equal`); `every_fp16_propagate_inputs` builds a call that feeds it every fp16 bit pattern.
 
 `check_group_norm` compares a tf_group_norm_nhwc output with the eager ATen sequence it replaces and with
 an fp64 evaluation.  ATen stores the group mean and rstd in fp16, so those bounds cannot see a statistics
@@ -73,6 +76,7 @@ from __future__ import annotations
 import math
 from typing import Optional, Sequence
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -315,8 +319,19 @@ def check_ext_attn(got: torch.Tensor, q: torch.Tensor, k: torch.Tensor, v: torch
 
 
 def nn_similarity(x_unit: torch.Tensor, piv_unit: torch.Tensor) -> torch.Tensor:
-    """fp16 similarities of fp16 unit rows, dot products accumulated in fp64: [R, dim] x [C, dim] -> [R, C]."""
+    """fp16 similarities of fp16 unit rows, dot products accumulated in fp64: [R, dim] x [C, dim] -> [R, C].
+    The unit row of a zero token is NaN (0 / 0), so its similarity row or column is NaN."""
     return (x_unit.double() @ piv_unit.double().T).float().half()
+
+
+def nn_argmax(sim: torch.Tensor) -> torch.Tensor:
+    """Index of each row's maximum in the order of torch.argmax, which the reference takes over its similarities:
+    a NaN ranks above every number, and the first of equal values, or of several NaNs, wins.  A row that is all NaN
+    (a zero frame token) gives 0, a NaN column (a zero pivot token) wins every row it reaches."""
+    nan = torch.isnan(sim)
+    first_nan = nan.to(torch.uint8).argmax(dim=-1)
+    best = torch.where(nan, torch.full_like(sim, -math.inf), sim).argmax(dim=-1)
+    return torch.where(nan.any(dim=-1), first_nan, best)
 
 
 def tie_class(sim: torch.Tensor, rows: torch.Tensor, got: torch.Tensor, want: torch.Tensor,
@@ -353,16 +368,89 @@ def check_nn_field(idx_a: torch.Tensor, idx_b: Optional[torch.Tensor], x_unit: t
             assert got.min().item() >= 0 and got.max().item() < S, \
                 f"frame {f}, keyframe {kf}: index outside [0, {S}) ({got.min().item()}..{got.max().item()})"
             sim = nn_similarity(x_unit[f], piv_unit[kf])
-            want = sim.argmax(dim=-1)
+            want = nn_argmax(sim)
             bad = (got != want).nonzero().flatten()
             total += S
             ties += bad.numel()
             if bad.numel():
-                inside = tie_class(sim, bad, got[bad], want[bad])
+                # a NaN winner has no tie class: its index is exact
+                inside = tie_class(sim, bad, got[bad], want[bad]) & ~torch.isnan(sim[bad, want[bad]])
                 assert inside.all(), (f"frame {f}, keyframe {kf}: token {bad[~inside][0].item()} has an NN index "
                                       f"outside the fp16 tie class")
     assert ties <= max(2, int(max_tie_frac * total)), f"{ties}/{total} rows differ from the oracle"
     return {"ties": ties, "total": total}
+
+
+# ------------------------------------------------------------------------------------------------
+# NN-indexed propagation (tf_propagate)
+# ------------------------------------------------------------------------------------------------
+def propagate_exact(A: torch.Tensor, idx_a: torch.Tensor, idx_b: Optional[torch.Tensor], kf_a: Sequence[int],
+                    kf_b: Sequence[int], w: Sequence[float], residual: Optional[torch.Tensor],
+                    out_dtype: torch.dtype) -> torch.Tensor:
+    """tf_propagate restated in numpy float32 from the reference expression (tokenflow_utils.py:361-397).
+
+    A [3, K, S, dim] fp16, idx_a / idx_b [F, S], residual [3F, S, dim] fp16 or None.  For frame f and stream s the
+    gathered rows a = A[s, kf_a[f], idx_a[f]] and, when kf_b[f] >= 0, b = A[s, kf_b[f], idx_b[f]] give
+    fp32(w * a) + fp32((1 - w) * b): two fp32 products and one fp32 addition, with w and 1 - w in fp32 and no fused
+    multiply-add (the reference's `w1 * attn_output1 + (1 - w1) * attn_output2` on an fp32 weight tensor).  A frame
+    without a second keyframe is a.  The residual is added in fp32 and the sum rounded once to `out_dtype`
+    (float16 or float32).  Returns a CPU tensor [3F, S, dim]."""
+    a16 = A.detach().cpu().to(torch.float16).numpy()
+    _, K, S, dim = a16.shape
+    ia = idx_a.detach().cpu().long().numpy()
+    ib = idx_b.detach().cpu().long().numpy() if idx_b is not None else None
+    F_ = ia.shape[0]
+    out = np.empty((3, F_, S, dim), dtype=np.float32)
+    with np.errstate(all="ignore"):          # 0 * inf, inf - inf and overflow are part of the arithmetic
+        for f in range(F_):
+            a = a16[:, int(kf_a[f])][:, ia[f]].astype(np.float32)
+            if int(kf_b[f]) >= 0:
+                wf = np.float32(w[f])
+                b = a16[:, int(kf_b[f])][:, ib[f]].astype(np.float32)
+                a = wf * a + (np.float32(1.0) - wf) * b
+            out[:, f] = a
+        if residual is not None:
+            out += residual.detach().cpu().to(torch.float16).numpy().reshape(3, F_, S, dim).astype(np.float32)
+        res = out.reshape(3 * F_, S, dim).astype({torch.float16: np.float16, torch.float32: np.float32}[out_dtype])
+    return torch.from_numpy(res)
+
+
+def bit_equal(got: torch.Tensor, want: torch.Tensor) -> torch.Tensor:
+    """Elementwise: both NaN, or the same bit pattern (so +0 and -0 differ).  Both fp16 or both fp32."""
+    assert got.dtype == want.dtype and tuple(got.shape) == tuple(want.shape), (got.dtype, want.dtype, got.shape,
+                                                                              want.shape)
+    got, want = got.detach().cpu(), want.detach().cpu()
+    bits = {torch.float16: torch.int16, torch.float32: torch.int32}[got.dtype]
+    return (got.view(bits) == want.view(bits)) | (torch.isnan(got) & torch.isnan(want))
+
+
+FP16_PATTERN_SIDE = 256                # S = dim = 256: one [S, dim] slab holds all 65 536 fp16 bit patterns
+
+
+def every_fp16_propagate_inputs(weights: Sequence[float], generator=None) -> dict:
+    """A tf_propagate call whose operands hold every fp16 bit pattern: ±0, subnormals, ±inf, NaNs, the largest
+    finite values (whose sums overflow) and values whose blend lands on fp16 midpoints.  One keyframe slab is
+    S x dim = 256 x 256 = 65 536 elements.  Stream a (keyframe 1, identity indices) holds the patterns in order in
+    stream 0 and in two fixed permutations in streams 1 and 2; stream b (keyframe 0) holds another permutation per
+    stream, gathered through a different row permutation in every frame; the residual is an independent permutation
+    per frame and stream.  Frames: one per entry of `weights`, then w = 1 with a second keyframe (1 - w = 0, so
+    0 * inf gives NaN), then one frame without a second keyframe.  Returns CPU tensors, keyword arguments of
+    `propagate_exact` and `CudaOps.propagate` (without `out_dtype`)."""
+    S = dim = FP16_PATTERN_SIDE
+    pats = torch.arange(-32768, 32768, dtype=torch.int16).view(torch.float16)
+    perm = lambda: torch.randperm(S * dim, generator=generator)
+    kf_a = [1] * (len(weights) + 2)
+    kf_b = [0] * (len(weights) + 1) + [-1]
+    w = [float(x) for x in weights] + [1.0, 1.0]
+    F_ = len(kf_a)
+    A = torch.empty(3, 2, S, dim, dtype=torch.float16)
+    for s in range(3):
+        A[s, 1] = (pats if s == 0 else pats[perm()]).view(S, dim)
+        A[s, 0] = pats[perm()].view(S, dim)
+    idx_a = torch.arange(S, dtype=torch.int32).repeat(F_, 1)
+    idx_b = torch.stack([torch.randperm(S, generator=generator) for _ in range(F_)]).int()
+    residual = torch.stack([pats[perm()].view(S, dim) for _ in range(3 * F_)])
+    return dict(A=A, idx_a=idx_a, idx_b=idx_b, kf_a=kf_a, kf_b=kf_b, w=w, residual=residual)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -6,7 +6,8 @@ padding keys masked, online softmax with fp16 P and an fp32 normaliser, fp16 out
 (1 600 tiles) a thread-by-thread restatement of the normaliser shows that the kernel's earlier arithmetic
 (P <= 1, one fp32 addition per key) fails the error model on a subnormal-tail probe, that the current one
 (P <= 2^8, one addition per tile) meets it on every probe, and that one dropped or stale tile out of 1 600 is
-rejected.  Likewise for `check_nn_field` and the NN field's padding guard and first-index rule.  Everything
+rejected.  Likewise for `check_nn_field` and the NN field's padding guard, first-index rule and NaN order (torch's
+argmax, which the reference uses, ranks a NaN similarity above every number).  Everything
 here is CPU torch: no wrong computation is compiled into the library or run on a GPU."""
 import math
 
@@ -15,7 +16,7 @@ import torch
 
 from oracle.kernel_checks import (ATTN_P_OFFSET, TAIL_BANDS, attn_block_n, check_ext_attn, check_nn_field,
                                   ext_attn_samples, late_jump_probe, logit_shift_probe, negative_similarity_probe,
-                                  nn_similarity, staircase_probe, subnormal_tail_probe)
+                                  nn_argmax, nn_similarity, staircase_probe, subnormal_tail_probe)
 
 
 def _flash(q, k, v, table, heads, scale, row0=0, nrows=None, *, leak_pad=False, drop_last_key=False,
@@ -223,6 +224,63 @@ def test_check_nn_field_rejects_a_wrong_index_outside_the_tie_class():
     idx_a[0, 5] = (idx_a[0, 5] + 1) % 64
     with pytest.raises(AssertionError):
         check_nn_field(idx_a, None, xu, pu, [0], [-1])
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.float32])
+def test_torch_argmax_returns_the_first_nan_and_nn_argmax_agrees(dtype):
+    """The reference takes torch.argmax over its similarities: a NaN ranks above every number, +inf included, and
+    the first NaN of a row wins; `nn_argmax` states that order without relying on it."""
+    nan, inf = float("nan"), float("inf")
+    sim = torch.tensor([[0.1, nan, 0.9, nan], [nan, nan, nan, nan], [0.2, 0.7, 0.7, -0.1], [inf, 0.3, nan, 1.0],
+                        [-1.0, -2.0, -1.0, -3.0]], dtype=dtype)
+    want = [1, 0, 1, 2, 0]
+    assert sim.argmax(dim=-1).tolist() == want
+    assert nn_argmax(sim).tolist() == want
+    g = torch.Generator().manual_seed(5)
+    big = torch.randn(64, 700, generator=g).to(dtype)
+    big[torch.rand(64, 700, generator=g) < 0.004] = nan
+    big[3] = nan
+    big[7, 699] = nan
+    assert torch.isnan(big).any(dim=-1).sum() > 10
+    assert torch.equal(big.argmax(dim=-1), nn_argmax(big))
+
+
+def _zero_token_inputs(S=200, dim=64, seed=4):
+    """Unit rows of a video-like pair of frames with zero tokens: pivot token 150 of keyframe 1 and tokens 21 and
+    130 of keyframe 0 (NaN columns), and token 77 of frame 1 (a NaN row)."""
+    g = torch.Generator().manual_seed(seed)
+    piv = torch.nn.functional.layer_norm(torch.randn(2, S, dim, generator=g), (dim,))
+    x = piv[[1, 0]][:, torch.randperm(S, generator=g)] + 0.3 * torch.randn(2, S, dim, generator=g)
+    piv[1, 150] = 0
+    piv[0, [21, 130]] = 0
+    x[1, 77] = 0
+    return _unit(x), _unit(piv)
+
+
+def test_check_nn_field_requires_the_first_nan_column_and_index_0_for_a_nan_row():
+    xu, pu = _zero_token_inputs()
+    kf_a, kf_b = [1, 1], [-1, 0]
+    assert torch.isnan(pu[1, 150]).all() and torch.isnan(xu[1, 77]).all()
+    idx_a, idx_b = _nn(xu, pu, kf_a, kf_b)
+    assert idx_a[0].eq(150).all() and idx_b[1, :77].eq(21).all() and idx_b[1, 77] == 0
+    check_nn_field(idx_a, idx_b, xu, pu, kf_a, kf_b)
+    # a kernel that never picks a NaN similarity (`h > best` alone) gives the best finite candidate instead
+    skip_nan = [torch.where(torch.isnan(s), torch.full_like(s, -float("inf")), s).argmax(dim=-1).int()
+                for s in (nn_similarity(xu[0], pu[1]).float(), nn_similarity(xu[1], pu[0]).float())]
+    wrong_a = idx_a.clone()
+    wrong_a[0] = skip_nan[0]
+    with pytest.raises(AssertionError):
+        check_nn_field(wrong_a, idx_b, xu, pu, kf_a, kf_b)
+    # ... or, with two NaN columns, keeps the later one
+    wrong_b = idx_b.clone()
+    wrong_b[1, :77] = 130
+    with pytest.raises(AssertionError):
+        check_nn_field(idx_a, wrong_b, xu, pu, kf_a, kf_b)
+    # a NaN row must give index 0
+    wrong_row = idx_a.clone()
+    wrong_row[1, 77] = skip_nan[1][77] if skip_nan[1][77] != 0 else 1
+    with pytest.raises(AssertionError):
+        check_nn_field(wrong_row, idx_b, xu, pu, kf_a, kf_b)
 
 
 # ------------------------------------------------------------------------------------------------

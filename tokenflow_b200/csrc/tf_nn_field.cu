@@ -1,7 +1,7 @@
 // tf_nn_field — token nearest-neighbour field (reference tokenflow_utils.py:329-348 + util.py:61-69).
 //
 // For every token p of every frame f and each adjacent keyframe kf in {kf_a[f], kf_b[f]}:
-//     idx[f,p] = argmax_c  fp16( x̂[f,p,:] . ŷ[kf,c,:] )          first index wins ties
+//     idx[f,p] = argmax_c  fp16( x̂[f,p,:] . ŷ[kf,c,:] )          first index wins ties, NaN above every number
 // with x̂, ŷ the fp16 unit rows produced by tf_unit_rows.  This is the arithmetic of the reference's
 // GPU path (fp32 normalise -> fp16 operands -> fp32-accumulated GEMM -> *fp16 output* -> argmax),
 // but the [B*S, 2S] similarity matrix (512 MB fp16 per block per batch at the 40-frame SD1.5
@@ -163,7 +163,9 @@ nn_field_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
     reg_fence(acc);
     release(j - 1);
 
-    // epilogue: fp16-rounded similarities, strictly greater keeps the earlier index
+    // epilogue: fp16-rounded similarities in torch.argmax's order (a NaN ranks above every number; a zero
+    // token's unit row is NaN).  Each thread visits its columns in increasing order, so taking a value only
+    // when it is greater or NaN, and nothing once the best is NaN, keeps the first of equal values or NaNs.
     const int n0 = nt * kBlockN;
 #pragma unroll
     for (int jb = 0; jb < kBlockN / 8; ++jb) {
@@ -172,19 +174,24 @@ nn_field_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
         const int r = e >> 1;
         const int c = n0 + 8 * jb + qcol + (e & 1);
         const float h = __half2float(__float2half_rn(acc[4 * jb + e]));
-        if (c < S && h > best[r]) { best[r] = h; best_idx[r] = c; }
+        if (c < S && !(h <= best[r]) && best[r] == best[r]) { best[r] = h; best_idx[r] = c; }
       }
     }
   }
 
-  // merge the four threads of each row: larger value wins, equal values keep the smaller index
+  // merge the four threads of each row in the same order: NaN above every number, the smaller index among
+  // equal values or NaNs
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
 #pragma unroll
     for (int off = 1; off <= 2; off <<= 1) {
       const float ob = __shfl_xor_sync(0xffffffffu, best[r], off);
       const int oi = __shfl_xor_sync(0xffffffffu, best_idx[r], off);
-      if (ob > best[r] || (ob == best[r] && oi < best_idx[r])) { best[r] = ob; best_idx[r] = oi; }
+      const bool o_nan = ob != ob, b_nan = best[r] != best[r];
+      if ((!b_nan && !(ob <= best[r])) || ((ob == best[r] || (o_nan && b_nan)) && oi < best_idx[r])) {
+        best[r] = ob;
+        best_idx[r] = oi;
+      }
     }
     const int p = m0 + wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2) + 8 * r;
     if ((lane & 3) == 0 && p < S) out[(long long)f * S + p] = best_idx[r];
