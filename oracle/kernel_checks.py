@@ -40,10 +40,14 @@ offset from the row maximum (a dominant key over a tail in a band; a maximum tha
 maximum that arrives in the last tile far above everything before it) and return the offsets the fp16 q and k
 realise, so a test can assert that the band it meant was hit.
 
-`check_nn_field` is the one implementation of the NN-field rule: every index equals the argmax of the
-kernel's own fp16 operands (dot products accumulated in fp64, rounded to fp16, first index on ties, a NaN
-similarity above every number as in torch.argmax: `nn_argmax`), up to rows inside a 1-ulp fp16 tie class,
-whose winner depends on the GEMM's fp32 accumulation order.  Such rows are bounded and counted.
+`check_nn_field` is the one implementation of the NN-field rule for realistic inputs: every index must be a
+lawful winner of its row, given the kernel's own fp16 operands, the tensor core's fp32 accumulation error
+(`nn_dot_delta`), one rounding to fp16 and the first index among equal fp16 values, with a NaN similarity above
+every number as in torch.argmax (`nn_argmax`).  Rows with more than one lawful winner are counted.
+
+`exact_similarity_probe` and `every_fp16_similarity_probe` build operands whose similarities the tensor core
+computes exactly in any accumulation order, so that `nn_field_exact` states the one right index of every row;
+`assert_exact_similarities` checks the premise.  See `exact_similarity_probe` for the cases its rows hold.
 
 `propagate_exact` restates tf_propagate in numpy float32 from the reference expression, for bit-for-bit
 comparison (`bit_equal`); `every_fp16_propagate_inputs` builds a call that feeds it every fp16 bit pattern.
@@ -345,40 +349,339 @@ def tie_class(sim: torch.Tensor, rows: torch.Tensor, got: torch.Tensor, want: to
     return (s_want - s_got).abs() <= ulps * ulp * 1.001
 
 
+NN_BLOCK_N = 128                # tf_nn_field.cu kBlockN: key columns per tile
+NN_CHUNK = 64                   # kChunkK: channels per shared-memory chunk
+NN_KSTEP = 16                   # channels per wgmma k-step
+NN_GRID_BITS = 17               # exact probes: every partial sum of a dot stays below 2^17 steps of its grid
+
+
+def fp16_rn(v: torch.Tensor) -> torch.Tensor:
+    """fp64 -> fp16 with a single round-to-nearest-even (`.half()` of a double rounds through fp32, which can round
+    twice).  v = m 2^e with m in [0.5, 1) sits in an fp16 binade of spacing 2^(e - 11), 2^-24 below the normal range;
+    torch.round is round-half-even, and a result past 65504 becomes inf in the final conversion."""
+    _, e = torch.frexp(v)
+    q = torch.ldexp(torch.ones_like(v), e - 11).clamp_min(2.0 ** -24)
+    return (torch.round(v / q) * q).half()
+
+
+def nn_dot_delta(dim: int, abs_dot: torch.Tensor) -> torch.Tensor:
+    """Bound on |ŝ - s| of the kernel's fp32 similarity ŝ, s the exact dot product of fp16 rows, with
+    `abs_dot` = Σ|x_i y_i| (fp64).  The tensor-core model of `attn_accum_rel`: each wgmma k-step adds 16 products
+    to the running accumulator, every one of the 17 addends aligned to the largest of them and losing up to 2^-23
+    of it, and the sum is rounded to fp32 (2^-24).  Every addend, the accumulator included, is at most Σ|x_i y_i|,
+    so one k-step errs by at most (17 * 2^-23 + 2^-24) Σ|x_i y_i| = 35 * 2^-24 Σ|x_i y_i|, and ceil(dim / 16)
+    k-steps by ceil(dim / 16) times that.  δ is twice the sum: 2 * ceil(dim / 16) * 35 * 2^-24 * Σ|x_i y_i|.
+    (The fp16 rounding of the epilogue is not part of δ: `nn_lawful_winners` maps the interval through it.)"""
+    return (2 * -(-dim // NN_KSTEP) * 35 * 2.0 ** -24) * abs_dot
+
+
+def nn_lawful_winners(sim64: torch.Tensor, abs_dot: torch.Tensor, dim: int) -> torch.Tensor:
+    """[R, C] bool for rows without NaN: column c is a lawful winner when some fp32 similarities within δ
+    (`nn_dot_delta`) of the exact ones, each rounded to fp16, make c the first maximum.  With [lo16, hi16] the fp16
+    values an interval [s - δ, s + δ] can round to, that is hi16(c) > lo16(c') for every c' < c and
+    hi16(c) >= lo16(c') for every c' > c."""
+    d = nn_dot_delta(dim, abs_dot)
+    lo, hi = fp16_rn(sim64 - d).float(), fp16_rn(sim64 + d).float()
+    pad = torch.full_like(lo[:, :1], -math.inf)
+    before = torch.cat([pad, lo[:, :-1]], dim=1).cummax(dim=1).values
+    after = torch.cat([lo[:, 1:], pad], dim=1).flip(1).cummax(dim=1).values.flip(1)
+    return (hi > before) & (hi >= after)
+
+
 def check_nn_field(idx_a: torch.Tensor, idx_b: Optional[torch.Tensor], x_unit: torch.Tensor,
-                   piv_unit: torch.Tensor, kf_a: Sequence[int], kf_b: Sequence[int],
-                   max_tie_frac: float = 5e-3) -> dict:
+                   piv_unit: torch.Tensor, kf_a: Sequence[int], kf_b: Sequence[int], tag: str = "") -> dict:
     """Assert that (idx_a, idx_b) is `nn_field(x_unit, piv_unit, kf_a, kf_b)` computed correctly.
 
-    x_unit [F, S, dim], piv_unit [K, S, dim] are the fp16 unit rows the kernel read.  idx_b is read only for
-    frames with kf_b >= 0 (the kernel leaves the other rows unwritten).  Returns the tie-row count."""
-    F, S, _ = x_unit.shape
+    x_unit [F, S, dim], piv_unit [K, S, dim] are the fp16 rows the kernel read.  idx_b is read only for frames with
+    kf_b >= 0 (the kernel leaves the other rows unwritten).  Every index must be a lawful winner of its row
+    (`nn_lawful_winners`); a row with a NaN similarity (a zero token's unit row is NaN) is exact: its first NaN column
+    must win, index 0 for a row that is all NaN.  Returns {"ties": the number of rows with more than one lawful winner
+    (tie rows: the accumulation order may decide their index), "total": the number of rows}."""
+    F, S, dim = x_unit.shape
     assert idx_a.dtype == torch.int32 and tuple(idx_a.shape) == (F, S), (idx_a.dtype, tuple(idx_a.shape))
     any_b = any(int(b) >= 0 for b in kf_b)
     if any_b:
         assert idx_b is not None and idx_b.dtype == torch.int32 and tuple(idx_b.shape) == (F, S)
     else:
         assert idx_b is None
-    total = ties = 0
+    chunk = max(1, (1 << 24) // max(S, 1))              # rows per evaluation: a few [rows, S] fp64 matrices
+    total = multi = 0
     for f in range(F):
         for kf, idx in ((int(kf_a[f]), idx_a), (int(kf_b[f]), idx_b)):
             if kf < 0:
                 continue
-            got = idx[f].long()
+            got = idx[f].long().to(x_unit.device)
             assert got.min().item() >= 0 and got.max().item() < S, \
                 f"frame {f}, keyframe {kf}: index outside [0, {S}) ({got.min().item()}..{got.max().item()})"
-            sim = nn_similarity(x_unit[f], piv_unit[kf])
-            want = nn_argmax(sim)
-            bad = (got != want).nonzero().flatten()
+            y = piv_unit[kf].double()
+            for r0 in range(0, S, chunk):
+                xr = x_unit[f, r0:r0 + chunk].double()
+                s64 = xr @ y.T
+                lawful = nn_lawful_winners(s64, xr.abs() @ y.abs().T, dim)
+                nan_row = torch.isnan(s64).any(dim=1)
+                g = got[r0:r0 + chunk]
+                ok = torch.where(nan_row, g == nn_argmax(s64), lawful.gather(1, g[:, None]).squeeze(1))
+                if not ok.all():
+                    r = int((~ok).nonzero()[0])
+                    sim = fp16_rn(s64[r])
+                    want = int(nn_argmax(sim[None])[0])
+                    raise AssertionError(
+                        f"{tag} frame {f}, keyframe {kf}: {int((~ok).sum())} of the rows {r0}..{r0 + len(g) - 1} have "
+                        f"an index that is not a lawful winner; token {r0 + r} has {int(g[r])} (similarity "
+                        f"{s64[r, g[r]].item():.9g}, fp16 {sim[g[r]].item():.6g}); its first fp16 maximum is {want} "
+                        f"({s64[r, want].item():.9g}, fp16 {sim[want].item():.6g}), lawful winners "
+                        f"{lawful[r].nonzero().flatten()[:8].tolist()}")
+                multi += int(((lawful.sum(dim=1) > 1) & ~nan_row).sum())
             total += S
-            ties += bad.numel()
-            if bad.numel():
-                # a NaN winner has no tie class: its index is exact
-                inside = tie_class(sim, bad, got[bad], want[bad]) & ~torch.isnan(sim[bad, want[bad]])
-                assert inside.all(), (f"frame {f}, keyframe {kf}: token {bad[~inside][0].item()} has an NN index "
-                                      f"outside the fp16 tie class")
-    assert ties <= max(2, int(max_tie_frac * total)), f"{ties}/{total} rows differ from the oracle"
-    return {"ties": ties, "total": total}
+    print(f"{tag} nn_field: {multi} of {total} rows with more than one lawful winner")
+    return {"ties": multi, "total": total}
+
+
+# ------------------------------------------------------------------------------------------------
+# NN field: probes whose similarities are exact in every accumulation order
+# ------------------------------------------------------------------------------------------------
+def _token_grid(t: torch.Tensor) -> torch.Tensor:
+    """Per row of fp16 t [N, dim]: the largest power of two dividing every channel, in units of 2^-24 (int64; 2^62
+    for a zero row).  Every finite fp16 value is a multiple of 2^-24 below 2^16."""
+    n = (t.double() * 2.0 ** 24).long()
+    low = torch.where(n == 0, torch.full_like(n, 1 << 62), n & -n)
+    return low.min(dim=1).values
+
+
+def _unique_rows(t: torch.Tensor):
+    """(distinct rows by bit pattern, inverse map) of fp16 t [N, dim]."""
+    u, inv = torch.unique(t.contiguous().view(torch.int16), dim=0, return_inverse=True)
+    return u.view(torch.float16), inv
+
+
+def assert_exact_similarities(x: torch.Tensor, piv: torch.Tensor):
+    """Assert the premise of the exact probes for fp16 x [F, S, dim] and piv [K, S, dim]: for every frame token r and
+    keyframe token c, with g_r and g_c the power-of-two grids of their channels (`_token_grid`), every product
+    x_i y_i is a multiple of g_r g_c and Σ|x_i y_i| < 2^17 g_r g_c.  Every partial sum of the dot, in any order, is
+    then a multiple of g_r g_c below 2^17 of them: 17 significant bits, exact in an accumulator that keeps 24 bits of
+    its largest addend, and exact in fp32 and fp64."""
+    dim = x.shape[-1]
+    xs, _ = _unique_rows(x.reshape(-1, dim).cpu())
+    ys = piv.reshape(-1, dim).cpu()
+    assert torch.isfinite(xs).all() and torch.isfinite(ys).all(), "the exact premise needs finite operands"
+    gx, gy = _token_grid(xs).double() * 2.0 ** -24, _token_grid(ys).double() * 2.0 ** -24
+    a = xs.double().abs() @ ys.double().abs().T
+    bound = 2.0 ** NN_GRID_BITS * gx[:, None] * gy[None, :]
+    if not (a < bound).all():
+        r, c = (int(v) for v in (a >= bound).nonzero()[0])
+        raise AssertionError(f"exact-similarity premise: Σ|x_i y_i| = {a[r, c].item():.9g} for distinct frame row {r} "
+                             f"and keyframe token {c}, not below 2^{NN_GRID_BITS} grid steps ({bound[r, c].item():.3g})")
+
+
+def nn_field_exact(x: torch.Tensor, piv: torch.Tensor, kf_a: Sequence[int], kf_b: Sequence[int]):
+    """The NN field stated outright: per frame f and keyframe kf, the dot products in fp64, one rounding to fp16
+    (`fp16_rn`), then `nn_argmax`.  It is the kernel's one right answer where `assert_exact_similarities` holds, or
+    where every dot has a single nonzero product (`every_fp16_similarity_probe`).  Evaluated once per distinct frame
+    row.  Returns CPU int32 (idx_a, idx_b) [F, S]; idx_b is None when no frame has a second keyframe, and -1 in the
+    rows of frames without one."""
+    F, S, dim = x.shape
+    x, piv = x.cpu(), piv.cpu()
+    idx_a = torch.full((F, S), -1, dtype=torch.int32)
+    idx_b = idx_a.clone() if any(int(b) >= 0 for b in kf_b) else None
+    for f in range(F):
+        u, inv = _unique_rows(x[f])
+        for kf, idx in ((int(kf_a[f]), idx_a), (int(kf_b[f]), idx_b)):
+            if kf >= 0:
+                idx[f] = nn_argmax(fp16_rn(u.double() @ piv[kf].double().T))[inv].int()
+    return idx_a, idx_b
+
+
+# Each case: the similarities of its candidate columns, in grid steps of 2^-14 relative to a base b (an fp16 value
+# in [1, 2) with an even mantissa: b = 2^14 + 32 j, one fp16 ulp = 16 steps), in increasing column order, each
+# with a placement rule, and which candidate must win.  The fp16 value each rounds to is noted.
+#   first: in the first key tile          last: in the last key tile            end: the last column, S - 1
+#   pair: c_prev + 1, same thread         thread: same thread as candidate 0 (same c mod 8), a later tile
+#   other: same tile as c_prev, another thread of the row's 4-thread merge (another (c mod 8) // 2)
+#   any: anywhere after c_prev
+NN_PROBE_CASES = {
+    # an fp16 tie class inside one thread, within a tile and across tiles: the later exact values are larger
+    "tie_same_thread": ([(2, "first"), (4, "pair"), (7, "thread"), (-9, "any")], 0),          # b, b, b, b - 16
+    # an fp16 tie class across two threads of the merge; truncation would drop the first to b - 16
+    "tie_cross_threads": ([(-3, "any"), (3, "other"), (-23, "any")], 0),                     # b, b, b - 16
+    # a midpoint below an odd neighbour rounds down to the even b; rounding half up would pick it
+    "rne_midpoint_down": ([(-16, "any"), (1, "any"), (8, "other"), (7, "any")], 1),          # b - 16, b, b, b
+    # a midpoint above an odd value rounds up to the even b + 32; truncation leaves b + 16 everywhere
+    "rne_midpoint_up": ([(16, "any"), (23, "any"), (24, "any"), (25, "any")], 2),            # b + 16, b + 16, b + 32, b + 32
+    # every real similarity negative (near -0.3125, ulp 4 steps, b not used): a padding column (0) would win
+    "negative_last_tile": ([(-5124, "first"), (-5121, "any"), (-5116, "last")], 2),           # n - 4, n, n + 4
+    "first_tile_winner": ([(80, "first"), (87, "any")], 0),                                  # b + 80, b + 80
+    "last_column_winner": ([(0, "first"), (15, "end")], 1),                                  # b, b + 16
+}
+NN_PROBE_SMALL = ([(90, "any"), (113, "any"), (113, "other"), (112, "any"), (5, "any")], 1)  # exact below 2^-7
+NN_PROBE_ABSOLUTE = {"negative_last_tile"}
+_PROBE_SEL = 2048               # selector entry of a keyframe token (units 2^-7): -2^15 steps against other groups
+_PROBE_ROW_SEL = 16
+
+
+def _placement(rule: str, chosen: list, S: int, n_tiles: int) -> torch.Tensor:
+    """[S] bool: the columns where the next candidate of a case may go (see NN_PROBE_CASES)."""
+    c = torch.arange(S)
+    prev = chosen[-1] if chosen else -1
+    tile = c // NN_BLOCK_N
+    ok = c > prev
+    if rule == "first":
+        return ok & (tile == 0)
+    if rule == "last":
+        return ok & (tile == n_tiles - 1)
+    if rule == "end":
+        return ok & (c == S - 1)
+    if rule == "pair":
+        return ok & (c == prev + 1) & (prev % 2 == 0)
+    if rule == "thread":
+        return ok & (c % 8 == chosen[0] % 8) & (tile > chosen[0] // NN_BLOCK_N)
+    if rule == "other":
+        return ok & (tile == prev // NN_BLOCK_N) & ((c % 8) // 2 != (prev % 8) // 2)
+    assert rule == "any", rule
+    return ok
+
+
+def exact_similarity_probe(F: int, K: int, S: int, dim: int, generator=None) -> dict:
+    """fp16 frame tokens x [F, S, dim] and keyframe tokens piv [K, S, dim] whose similarities the kernel computes
+    exactly (`assert_exact_similarities`, asserted here), so every index has one right answer (`nn_field_exact`).
+
+    Layout, in integers times 2^-7 (products in grid steps of 2^-14): channels [0, G) select a group (G = 8, 6 at
+    dim 8), then mass channels up to dim - 3, a level channel dim - 2 and a fine channel dim - 1.  Frame tokens are
+    copies of G + 1 prototypes, permuted per frame: prototype g < G has 16 in selector channel g, random ±1 / ±2 in
+    every mass channel, 16 in the level channel and 1 in the fine channel; prototype G is prototype 0 times 2^-7.
+    A keyframe token of group g has -2048 in every selector channel but g (-2^15 steps against every other group),
+    random ±1 / ±2 mass, and a level ℓ and fine value t chosen so that its similarity with prototype g is the target
+    of its role: 16 ℓ + t = target - mass.  The fine channel holds the low 4 bits that settle ties and midpoints;
+    the mass spreads every similarity over every 64-channel chunk and 16-channel k-step, with different amounts for
+    the candidates of a case, so that skipping, repeating or misaddressing one changes some index.
+
+    In every keyframe, group 0 holds `NN_PROBE_SMALL`: exact similarities below 2^-7, fp16 subnormals for
+    prototype G.  Groups 1 .. G-1 hold the cases of `NN_PROBE_CASES`, rotated from keyframe to keyframe; a case that
+    does not fit S is left out.  Every other keyframe token is a filler well below its group's candidates.  Returns
+    {"x", "piv" (CPU fp16), "proto" [F, S] (each frame token's prototype), "groups" (G), "cases": [(keyframe,
+    prototype, name, candidate columns, winning column)]}."""
+    assert dim % 8 == 0 and dim >= 8 and S >= 1
+    g_ = generator
+    G = 6 if dim == 8 else 8
+    n_proto = G + 1
+    mass = slice(G, dim - 2)
+    n_mass = dim - 2 - G
+    n_tiles = -(-S // NN_BLOCK_N)
+
+    def pm12(*shape):
+        v = torch.randint(1, 3, shape, generator=g_) * (2 * torch.randint(0, 2, shape, generator=g_) - 1)
+        return v.long()
+
+    proto = torch.zeros(n_proto, dim, dtype=torch.long)
+    proto[torch.arange(G), torch.arange(G)] = _PROBE_ROW_SEL
+    proto[:G, mass] = pm12(G, n_mass)
+    proto[:G, dim - 2], proto[:G, dim - 1] = 16, 1
+    proto[G] = proto[0]
+    proto16 = (proto.double() * 2.0 ** -7).half()
+    proto16[G] = (proto[G].double() * 2.0 ** -14).half()
+    assert torch.equal(proto16[G].double() * 2 ** 7, proto16[0].double())
+
+    menu = sorted(NN_PROBE_CASES)
+    piv = torch.empty(K, S, dim, dtype=torch.float16)
+    cases = []
+    for k in range(K):
+        group = torch.randint(0, G, (S,), generator=g_)
+        target = torch.zeros(S, dtype=torch.long)
+        free = torch.ones(S, dtype=torch.bool)
+        floor = {}
+        plan = [(0, "small", NN_PROBE_SMALL)] + [
+            (gi, name, NN_PROBE_CASES[name])
+            for gi, name in ((gi, menu[((gi - 1) + k * (G - 1)) % len(menu)]) for gi in range(1, G))]
+        # place the cases with the tightest rules first
+        plan.sort(key=lambda p: (0 if any(r in ("end", "last", "thread") for _, r in p[2][0]) else 1))
+        for gi, name, (cands, win) in plan:
+            base = 0 if name == "small" or name in NN_PROBE_ABSOLUTE else 2 ** 14 + 32 * int(torch.randint(0, 64, (1,),
+                                                                                                             generator=g_))
+            chosen = []
+            for _, rule in cands:
+                options = (free & _placement(rule, chosen, S, n_tiles)).nonzero().flatten()
+                if rule == "first" and len(cands) > 1 and cands[1][1] == "pair":
+                    options = options[options % 2 == 0]
+                if not len(options):
+                    break
+                room = max(1, len(options) // (len(cands) - len(chosen) + 1))
+                chosen.append(int(options[int(torch.randint(0, room, (1,), generator=g_))]))
+                free[chosen[-1]] = False
+            if len(chosen) < len(cands):
+                free[chosen] = True
+                continue
+            for c, (t, _) in zip(chosen, cands):
+                group[c], target[c] = gi, base + t
+            floor[gi] = base + min(t for t, _ in cands)
+            cases.append((k, gi, name, chosen, chosen[win]))
+            if name == "small":
+                cases.append((k, G, "small_subnormal", chosen, chosen[win]))
+        rest = free.nonzero().flatten()
+        fg = group[rest]
+        fl = torch.tensor([floor.get(int(g), 2 ** 14 if g else 80) for g in fg], dtype=torch.long)
+        drop = torch.where(fg == 0, torch.randint(0, 208, (len(rest),), generator=g_),
+                           600 + torch.randint(0, 2000, (len(rest),), generator=g_))
+        target[rest] = fl - drop
+        target[rest[fg == 0]] = target[rest[fg == 0]].clamp_min(-127)
+
+        y = torch.zeros(S, dim, dtype=torch.long)
+        y[:, :G] = -_PROBE_SEL
+        y[torch.arange(S), group] = 0
+        y[:, mass] = pm12(S, n_mass)
+        r = target - (proto[group][:, mass] * y[:, mass]).sum(dim=1)
+        lvl = torch.div(r, 16, rounding_mode="floor")
+        y[:, dim - 2], y[:, dim - 1] = lvl, r - 16 * lvl
+        assert lvl.abs().max() <= 2047, "probe level channel out of fp16 integer range"
+        piv[k] = (y.double() * 2.0 ** -7).half()
+        assert torch.equal(piv[k].double() * 2 ** 7, y.double())
+
+    x = torch.empty(F, S, dim, dtype=torch.float16)
+    pmap = torch.empty(F, S, dtype=torch.long)
+    for f in range(F):
+        pmap[f] = torch.randperm(S, generator=g_) % n_proto
+        x[f] = proto16[pmap[f]]
+    assert_exact_similarities(x, piv)
+    # the cases decide as designed
+    for k, p, name, cols, win in cases:
+        got = int(nn_argmax(fp16_rn(proto16[p:p + 1].double() @ piv[k].double().T))[0])
+        assert got == win, f"probe case {name} in keyframe {k}: column {got} wins, not {win}"
+    return {"x": x, "piv": piv, "proto": pmap, "groups": G, "cases": cases}
+
+
+FP16_SIM_TOKENS = 65536                 # every fp16 bit pattern once
+FP16_SIM_DIM = 8
+FP16_SIM_SETS = ("all_patterns", "no_nan", "finite", "signed_zeros")
+
+
+def every_fp16_similarity_probe(generator=None) -> dict:
+    """Keyframes of S = 65 536 tokens whose channel 0 carries fp16 values (every other channel 0), against frame rows
+    ±2^k e0, k in [-24, 15]: every dot is a single exact product, so its fp16 rounding is the kernel's similarity in
+    any order.  Keyframe 0 holds every bit pattern once (a permutation); 1 the same with each NaN replaced by a
+    random non-NaN pattern; 2 with each NaN and ±inf replaced by a random finite one; 3 only ±0.  This pins the
+    kernel's total order: the first NaN above +inf, products that overflow fp16 to ±inf, products that round to
+    fp16 subnormals or to ±0 (RN-even), -0 equal to +0 so that the first index wins, and duplicates.  Every frame
+    holds all 80 multipliers, in its own order.  Returns {"x" [4, S, 8], "piv" [4, S, 8] (CPU fp16), "kf_a",
+    "kf_b"}."""
+    g_ = generator
+    S, dim = FP16_SIM_TOKENS, FP16_SIM_DIM
+    pats = torch.arange(-32768, 32768, dtype=torch.int32).to(torch.int16).view(torch.float16)
+    nan, inf = torch.isnan(pats), torch.isinf(pats)
+
+    def refill(bad):
+        v = pats.clone()
+        good = (~bad).nonzero().flatten()
+        v[bad] = pats[good[torch.randint(0, len(good), (int(bad.sum()),), generator=g_)]]
+        return v
+
+    sets = [pats, refill(nan), refill(nan | inf),
+            (torch.randint(0, 2, (S,), generator=g_, dtype=torch.int32) * -32768).to(torch.int16).view(torch.float16)]
+    piv = torch.zeros(len(sets), S, dim, dtype=torch.float16)
+    for k, v in enumerate(sets):
+        piv[k, :, 0] = v[torch.randperm(S, generator=g_)]
+    mult = torch.tensor([s * 2.0 ** e for e in range(-24, 16) for s in (1.0, -1.0)]).half()
+    x = torch.zeros(4, S, dim, dtype=torch.float16)
+    for f in range(4):
+        x[f, :, 0] = mult[torch.randperm(S, generator=g_) % len(mult)]
+    return {"x": x, "piv": piv, "kf_a": [0, 1, 2, 3], "kf_b": [1, -1, 3, 0]}
 
 
 # ------------------------------------------------------------------------------------------------

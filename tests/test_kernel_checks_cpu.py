@@ -6,8 +6,8 @@ padding keys masked, online softmax with fp16 P and an fp32 normaliser, fp16 out
 (1 600 tiles) a thread-by-thread restatement of the normaliser shows that the kernel's earlier arithmetic
 (P <= 1, one fp32 addition per key) fails the error model on a subnormal-tail probe, that the current one
 (P <= 2^8, one addition per tile) meets it on every probe, and that one dropped or stale tile out of 1 600 is
-rejected.  Likewise for `check_nn_field` and the NN field's padding guard, first-index rule and NaN order (torch's
-argmax, which the reference uses, ranks a NaN similarity above every number).  Everything
+rejected.  Likewise for `check_nn_field` and the NN field's padding guard, first-index rule, fp16 rounding and NaN
+order (torch's argmax, which the reference uses, ranks a NaN similarity above every number).  Everything
 here is CPU torch: no wrong computation is compiled into the library or run on a GPU."""
 import math
 
@@ -15,8 +15,9 @@ import pytest
 import torch
 
 from oracle.kernel_checks import (ATTN_P_OFFSET, TAIL_BANDS, attn_block_n, check_ext_attn, check_nn_field,
-                                  ext_attn_samples, late_jump_probe, logit_shift_probe, negative_similarity_probe,
-                                  nn_argmax, nn_similarity, staircase_probe, subnormal_tail_probe)
+                                  ext_attn_samples, fp16_rn, late_jump_probe, logit_shift_probe,
+                                  negative_similarity_probe, nn_argmax, nn_dot_delta, nn_similarity, staircase_probe,
+                                  subnormal_tail_probe, tie_class)
 
 
 def _flash(q, k, v, table, heads, scale, row0=0, nrows=None, *, leak_pad=False, drop_last_key=False,
@@ -160,8 +161,9 @@ def _unit(x):
     return (x / x.norm(dim=-1, keepdim=True)).half()
 
 
-def _nn(xu, pu, kf_a, kf_b, *, pad_leak=False, clamp_leak=False, last_on_ties=False):
-    """tf_nn_field's arithmetic on CPU (fp16 similarities, 128-column tiles, zero padding columns)."""
+def _nn(xu, pu, kf_a, kf_b, *, pad_leak=False, clamp_leak=False, last_on_ties=False, fp32_compare=False):
+    """tf_nn_field's arithmetic on CPU (fp16 similarities, 128-column tiles, zero padding columns); `fp32_compare`
+    takes the argmax of the fp32 similarities without rounding them to fp16."""
     F, S, _ = xu.shape
     S_pad = -(-S // 128) * 128
     idx_a = torch.full((F, S), -0x7f7f7f7f, dtype=torch.int32)
@@ -171,6 +173,8 @@ def _nn(xu, pu, kf_a, kf_b, *, pad_leak=False, clamp_leak=False, last_on_ties=Fa
             if kf < 0:
                 continue
             sim = nn_similarity(xu[f], pu[kf]).float()
+            if fp32_compare:
+                sim = (xu[f].double() @ pu[kf].double().T).float()
             if pad_leak or clamp_leak:
                 sim = torch.cat([sim, torch.zeros(S, S_pad - S)], dim=1)
             if last_on_ties:
@@ -224,6 +228,63 @@ def test_check_nn_field_rejects_a_wrong_index_outside_the_tie_class():
     idx_a[0, 5] = (idx_a[0, 5] + 1) % 64
     with pytest.raises(AssertionError):
         check_nn_field(idx_a, None, xu, pu, [0], [-1])
+
+
+def _tie_rows(S=256, dim=320, seed=6):
+    """Unit rows of video-like frames (keyframe tokens plus noise) at dim 320, and keyframe tokens c + S/2 that are
+    copies of tokens c with every other channel moved one fp16 ulp away from zero: for a frame token near token c the
+    copy's exact similarity is larger by about half an fp16 ulp, and often rounds to the same fp16 value."""
+    g = torch.Generator().manual_seed(seed)
+    base = torch.nn.functional.layer_norm(torch.randn(S // 2, dim, generator=g), (dim,))
+    b16 = _unit(base)
+    bump = (torch.arange(dim) % 2 == 0).to(torch.int16)                 # every other channel
+    away = (b16.view(torch.int16) + bump).view(torch.float16)          # sign and magnitude: one ulp away from 0
+    pu = torch.cat([b16, away]).unsqueeze(0)
+    x = base[torch.randperm(S // 2, generator=g)].repeat(2, 1) + 0.05 * torch.randn(S, dim, generator=g)
+    return _unit(x).unsqueeze(0), pu
+
+
+def test_check_nn_field_rejects_fp32_compare_on_unit_rows():
+    """A kernel that compares its fp32 similarities without rounding them to fp16 picks the later, exactly larger
+    column of an fp16 tie.  The old rule (a 1-ulp tie class and a 0.5 % allowance) excused such rows; every one of
+    them whose two exact values lie more than 2δ apart is a violation now."""
+    xu, pu = _tie_rows()
+    S, dim = xu.shape[1:]
+    check_nn_field(*_nn(xu, pu, [0], [-1]), xu, pu, [0], [-1])
+    got, _ = _nn(xu, pu, [0], [-1], fp32_compare=True)
+    want, _ = _nn(xu, pu, [0], [-1])
+    s64 = xu[0].double() @ pu[0].double().T
+    d = nn_dot_delta(dim, xu[0].double().abs() @ pu[0].double().abs().T)
+    rows = (got[0] != want[0]).nonzero().flatten()
+    g, w = got[0, rows].long(), want[0, rows].long()
+    # every such row is an fp16 tie whose later column is larger by more than both intervals
+    s16 = fp16_rn(s64)
+    assert (s16[rows, g] == s16[rows, w]).all() and (g > w).all()
+    outside = (s64[rows, g] - d[rows, g]) - (s64[rows, w] + d[rows, w])
+    clear = int((outside > 0).sum())
+    print(f"fp32-compare mutant: {len(rows)} of {S} rows differ, {clear} of them outside the δ band")
+    assert clear >= 5
+    assert tie_class(s16.float(), rows, g, w).all()                    # the old rule's tie class excuses them all
+    with pytest.raises(AssertionError, match="not a lawful winner"):
+        check_nn_field(got, None, xu, pu, [0], [-1])
+
+
+def test_video_like_unit_rows_and_the_delta_band():
+    """How many fp16 tie rows video-like data at dim 320 has, and how wide δ is against an fp16 ulp: printed, and δ
+    stays below 1/4 ulp of a similarity near 1."""
+    g = torch.Generator().manual_seed(8)
+    S, dim = 1024, 320
+    piv = torch.nn.functional.layer_norm(torch.randn(S, dim, generator=g), (dim,))
+    x = piv[torch.randperm(S, generator=g)] + 0.3 * torch.randn(S, dim, generator=g)
+    xu, pu = _unit(x), _unit(piv)
+    s64 = xu.double() @ pu.double().T
+    s16 = fp16_rn(s64).float()
+    top = s16.max(dim=1, keepdim=True).values
+    ties = int(((s16 == top).sum(dim=1) > 1).sum())
+    d = nn_dot_delta(dim, xu.double().abs() @ pu.double().abs().T)
+    print(f"video-like dim {dim}: {ties} of {S} rows with an fp16 tie at the maximum; δ at most {d.max().item():.3g}")
+    assert d.max().item() < 2.0 ** -11 / 4
+    assert check_nn_field(nn_argmax(s16).int()[None], None, xu[None], pu[None], [0], [-1])["total"] == S
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.float32])
