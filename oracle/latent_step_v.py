@@ -1,5 +1,5 @@
 """ORACLE (test infrastructure) — the two latent updates for a v-prediction model, restated in numpy from a coefficient
-row: `tf_cfg_ddim_v` and `tf_ddim_v` (include/tokenflow_b200_vpred.h, tokenflow_b200/csrc/tf_cfg_ddim.cu).
+row: `tf_cfg_ddim_v` and `tf_ddim_v` (include/tokenflow_b200.h, tokenflow_b200/csrc/tf_cfg_ddim.cu).
 
 The same guidance as `tf_cfg_ddim` (oracle/latent_step.py), then diffusers' v-branch of the DDIM step (eta = 0) with the
 fp32 coefficient row (a, b, c, d), each operation in fp32 on fp16 operands and rounded to fp16 (h):

@@ -1,14 +1,11 @@
 """CPU tier: the numpy restatement of the latent updates (oracle/latent_step.py) can tell plausible wrong kernels
-apart, and the C ABI refuses device pointers the kernels cannot address before it touches CUDA.
+apart.
 
 * Planted variants.  A thread-by-thread restatement of tf_cfg_ddim with one deliberate change each (an FMA-contracted
   final sum, a true division by sqrt(alpha_t), the fp32 reciprocal of the fp32 sqrt(alpha_t), an unrounded c - u or
   g * d, guidance written as (1 - g) u + g c, fp64 coefficients, s3 and s4 swapped) must differ from the restatement on the GPU sweep's inputs (every fp16 value of u
   against the structured values of c and x) at a named step of the 50-step schedule.  Unchanged, it must agree.
-* Alignment contract.  Every pointer the header requires to be 16-byte aligned, passed one element off, is refused
-  with "misaligned": the misaligned-operand tests of the GPU tier rely on this refusal happening on the host.
 """
-import ctypes
 import functools
 import types
 
@@ -16,7 +13,6 @@ import numpy as np
 import pytest
 
 from oracle import latent_step as LS
-from tokenflow_b200 import ops as tf_ops
 from tokenflow_b200.editor import TokenFlowEditor
 from tokenflow_b200.scheduler import DDIMScheduler
 
@@ -137,106 +133,3 @@ VARIANTS = {
 def test_sweep_tells_the_planted_variant_apart(name):
     variant, row = VARIANTS[name]
     assert _differs(row, GUIDANCE, **variant), f"{name} is indistinguishable at step {row}"
-
-
-# ------------------------------------------------------------------------------------------------
-# alignment contract of the C ABI
-# ------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def lib():
-    from tokenflow_b200 import _build
-    if not tf_ops.library_path().exists():
-        _build.build()
-    return tf_ops.load_library()
-
-
-_BUF = (ctypes.c_uint8 * (1 << 20))()
-_P = (ctypes.addressof(_BUF) + 255) & ~255
-
-
-def _i32(*v):
-    return (ctypes.c_int32 * len(v))(*v)
-
-
-# entry point -> {pointer: element bytes} for every pointer the header requires to be 16-byte aligned (the canny
-# conditioning output only 2-byte aligned); coefficient rows, index tables and the frames of tf_resize_u8 / tf_canny_u8
-# need only their element's alignment and are not listed
-POINTERS = {
-    "tf_unit_rows[f16]": {"x": 2, "out": 2},
-    "tf_unit_rows[f32]": {"x": 4, "out": 2},
-    "tf_layernorm_unit_rows": {"x": 2, "gamma": 4, "beta": 4, "out": 2},
-    "tf_layernorm_rows": {"x": 2, "gamma": 4, "beta": 4, "y": 2, "unit": 2},
-    "tf_cfg_ddim": {"u": 2, "c": 2, "x": 2, "out": 2},
-    "tf_ddim": {"eps": 2, "x": 2, "out": 2},
-    "tf_nn_field": {"x_unit": 2, "piv_unit": 2},
-    "tf_propagate[f16]": {"A": 2, "residual": 2, "out": 2},
-    "tf_propagate[f32]": {"out": 4},
-    "tf_ext_attn_fwd": {"q": 2, "k": 2, "v": 2, "out": 2},
-    "tf_ext_attn_fwd_rows": {"q": 2, "k": 2, "v": 2, "out": 2},
-    "tf_group_norm_nhwc": {"x": 2, "bias": 2, "workspace": 1, "out": 2},
-    "tf_geglu": {"xh": 2, "gate": 2, "out": 2},
-    "tf_frames_to_nhwc": {"frames": 1, "out": 2},
-    "tf_nhwc_to_frames": {"x": 2, "frames": 1},
-    "tf_canny_u8": {"workspace": 1, "cond": 1},
-}
-
-
-def _calls(lib):
-    """entry point -> call(p): `p(name)` is the address of pointer `name`.  The shapes are valid, so the alignment
-    check is the only one that can refuse the call."""
-    kf = _i32(0, 0)
-    kfb = _i32(-1, 0)
-    w = (ctypes.c_float * 2)(1.0, 0.5)
-    one = _i32(1)
-    zero = _i32(0)
-    canny_ws = lib.tf_canny_workspace(1, 8, 8)
-    gn_ws = lib.tf_group_norm_nhwc_workspace(2, 16, 64, 8)
-    return {
-        "tf_unit_rows[f16]": lambda p: lib.tf_unit_rows(p("x"), 0, 4, 8, 8, p("out"), None),
-        "tf_unit_rows[f32]": lambda p: lib.tf_unit_rows(p("x"), 1, 4, 8, 8, p("out"), None),
-        "tf_layernorm_unit_rows": lambda p: lib.tf_layernorm_unit_rows(
-            p("x"), 4, 8, 8, p("gamma"), p("beta"), 1e-5, p("out"), None),
-        "tf_layernorm_rows": lambda p: lib.tf_layernorm_rows(
-            p("x"), 4, 8, 8, p("gamma"), p("beta"), 1e-5, p("y"), 8, p("unit"), 8, 2, None),
-        "tf_cfg_ddim": lambda p: lib.tf_cfg_ddim(p("u"), p("c"), p("x"), _P, 7.5, 64, p("out"), None),
-        "tf_ddim": lambda p: lib.tf_ddim(p("eps"), p("x"), _P, 64, p("out"), None),
-        "tf_nn_field": lambda p: lib.tf_nn_field(p("x_unit"), p("piv_unit"), kf, kfb, 2, 16, 8, 1, _P, _P, None),
-        "tf_propagate[f16]": lambda p: lib.tf_propagate(
-            p("A"), _P, _P, kf, kfb, w, 2, 16, 8, 1, p("residual"), p("out"), 0, None),
-        "tf_propagate[f32]": lambda p: lib.tf_propagate(p("A"), _P, _P, kf, kfb, w, 2, 16, 8, 1, None, p("out"), 1, None),
-        "tf_ext_attn_fwd": lambda p: lib.tf_ext_attn_fwd(p("q"), p("k"), p("v"), 16, 1, 16, 1, 16, 0.25, 0, p("out"),
-                                                         None),
-        "tf_ext_attn_fwd_rows": lambda p: lib.tf_ext_attn_fwd_rows(
-            p("q"), 1, 16, p("k"), p("v"), 1, 16, 1, zero, zero, zero, zero, one, 16, 1, 16, 0.25, 0, 16, p("out"), None),
-        "tf_group_norm_nhwc": lambda p: lib.tf_group_norm_nhwc(
-            p("x"), p("bias"), 64, _P, _P, 2, 16, 64, 8, 1e-5, 1, p("workspace"), gn_ws, p("out"), None),
-        "tf_geglu": lambda p: lib.tf_geglu(p("xh"), p("gate"), 64, p("out"), None),
-        "tf_frames_to_nhwc": lambda p: lib.tf_frames_to_nhwc(p("frames"), 16, p("out"), None),
-        "tf_nhwc_to_frames": lambda p: lib.tf_nhwc_to_frames(p("x"), 16, p("frames"), None),
-        "tf_canny_u8": lambda p: lib.tf_canny_u8(_P, 1, 8, 8, 100.0, 200.0, p("workspace"), canny_ws, None, p("cond"),
-                                                 None),
-    }
-
-
-# entry points with device pointers that need no more than element alignment: the resize tables and frames, NCCL's
-# buffers
-ANY_ALIGNMENT = {"tf_resize_u8", "tf_allgather"}
-
-
-def test_every_entry_point_with_device_pointers_is_covered():
-    with_pointers = {name for name, (_, args) in tf_ops._SIGNATURES.items()
-                     if any(a is ctypes.c_void_p for a in args) and not name.startswith(("tf_comm_", "tf_resize_coeffs"))}
-    covered = {entry.split("[")[0] for entry in POINTERS}
-    assert with_pointers - ANY_ALIGNMENT == covered
-
-
-_CASES = [(entry, ptr) for entry, ptrs in POINTERS.items() for ptr in ptrs]
-
-
-@pytest.mark.parametrize("entry,ptr", _CASES, ids=[f"{e}-{p}" for e, p in _CASES])
-def test_pointer_one_element_off_is_refused_on_the_host(lib, entry, ptr):
-    ptrs = POINTERS[entry]
-    slot = {name: i * 4096 for i, name in enumerate(ptrs)}          # disjoint 4 KB regions of one host buffer
-    addr = lambda name: _P + 65536 + slot.get(name, 0) + (ptrs[ptr] if name == ptr else 0)
-    status = _calls(lib)[entry](addr)
-    assert status == 1 and b"misaligned" in lib.tf_last_error(), (entry, ptr, status, lib.tf_last_error())

@@ -9,11 +9,8 @@ editor.
   oracle/latent_step_v.py's `cfg_ddim_v` on the GPU sweep's inputs; unchanged, it must agree.
 * `DDIMScheduler.from_config` on the shapes of the SD 1.5, SD 2.1-base and SD 2.1 (768-v) scheduler configs, and its
   refusals.
-* The v header (include/tokenflow_b200_vpred.h): header and binding table agree, every symbol is exported, every
-  device pointer passed one element off is refused on the host.
 * A tiny-UNet v edit: the fused step equals the reference's per-batch schedule, and two gloo ranks equal one.
 """
-import ctypes
 import functools
 import os
 import re
@@ -28,13 +25,11 @@ import torch.multiprocessing as mp
 
 from oracle import latent_step as LS
 from oracle import latent_step_v as LSV
-from tokenflow_b200 import ops as tf_ops
 from tokenflow_b200 import tokenflow_utils as tfu
 from tokenflow_b200.editor import TokenFlowEditor
 from tokenflow_b200.preprocess import LatentInverter, inversion_coef_tables
 from tokenflow_b200.scheduler import DDIMScheduler
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 V = "v_prediction"
 
 
@@ -306,66 +301,6 @@ def test_constructor_defaults_and_refusals():
     assert DDIMScheduler().prediction_type == "epsilon"
     with pytest.raises(ValueError, match="sample"):
         DDIMScheduler(prediction_type="sample")
-
-
-# ------------------------------------------------------------------------------------------------
-# d. the v header: binding, symbols, alignment
-# ------------------------------------------------------------------------------------------------
-def _header_functions():
-    text = open(os.path.join(REPO, "include", "tokenflow_b200_vpred.h")).read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    return sorted(set(re.findall(r"\b(tf_[a-z0-9_]+)\s*\(", text)))
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from tokenflow_b200 import _build
-    if not tf_ops.library_path().exists():
-        _build.build()
-    return tf_ops.load_library()
-
-
-def test_header_and_binding_agree():
-    assert _header_functions() == sorted(tf_ops._VPRED_SIGNATURES) == ["tf_cfg_ddim_v", "tf_ddim_v"]
-    assert not set(tf_ops._VPRED_SIGNATURES) & set(tf_ops._SIGNATURES)
-
-
-def test_library_exports_every_declared_symbol(lib):
-    for name in _header_functions():
-        fn = getattr(lib, name)
-        assert fn.argtypes == tf_ops._VPRED_SIGNATURES[name][1], name
-    assert lib.tf_version() == 1004
-
-
-_BUF = (ctypes.c_uint8 * (1 << 20))()
-_P = (ctypes.addressof(_BUF) + 255) & ~255
-POINTERS = {"tf_cfg_ddim_v": ("u", "c", "x", "out"), "tf_ddim_v": ("v", "x", "out")}
-
-
-def _call(lib, entry, p):
-    if entry == "tf_cfg_ddim_v":
-        return lib.tf_cfg_ddim_v(p("u"), p("c"), p("x"), _P, 7.5, 64, p("out"), None)
-    return lib.tf_ddim_v(p("v"), p("x"), _P, 64, p("out"), None)
-
-
-_CASES = [(entry, ptr) for entry, ptrs in POINTERS.items() for ptr in ptrs]
-
-
-@pytest.mark.parametrize("entry,ptr", _CASES, ids=[f"{e}-{p}" for e, p in _CASES])
-def test_pointer_one_element_off_is_refused_on_the_host(lib, entry, ptr):
-    slot = {name: i * 4096 for i, name in enumerate(POINTERS[entry])}
-    addr = lambda name: _P + 65536 + slot[name] + (2 if name == ptr else 0)
-    status = _call(lib, entry, addr)
-    assert status == 1 and b"misaligned" in lib.tf_last_error(), (entry, ptr, status, lib.tf_last_error())
-
-
-@pytest.mark.parametrize("entry", sorted(POINTERS))
-def test_null_pointers_and_negative_lengths_are_refused(lib, entry):
-    for name in POINTERS[entry]:
-        addr = lambda n: None if n == name else _P + 65536
-        assert _call(lib, entry, addr) == 1 and b"NULL" in lib.tf_last_error()
-    assert getattr(lib, entry)(*([None] * (3 if entry == "tf_ddim_v" else 4)),
-                               *((7.5,) if entry == "tf_cfg_ddim_v" else ()), -1, None, None) == 1
 
 
 # ------------------------------------------------------------------------------------------------

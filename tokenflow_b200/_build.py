@@ -21,8 +21,7 @@ STAMP = PKG_DIR / ".libtokenflow_b200.stamp"
 SOURCES = ["tf_capi.cu", "tf_unit_rows.cu", "tf_propagate.cu", "tf_nn_field.cu", "tf_ext_attn.cu", "tf_cfg_ddim.cu",
            "tf_comm.cu", "tf_body.cu", "tf_pixels.cu", "tf_resize.cu",
            "tf_canny.cu"]
-HEADERS = ["tf_common.cuh", "tf_kernels.h", "tf_wgmma.cuh", "../../include/tokenflow_b200.h",
-           "../../include/tokenflow_b200_vpred.h"]
+HEADERS = ["tf_common.cuh", "tf_kernels.h", "tf_wgmma.cuh", "../../include/tokenflow_b200.h"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -5,10 +5,10 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <vector>
 
 #include "../../include/tokenflow_b200.h"
-#include "../../include/tokenflow_b200_vpred.h"
 #include "tf_common.cuh"
 #include "tf_kernels.h"
 
@@ -73,21 +73,63 @@ CUresult encode_tiled(CUtensorMap* map, CUtensorMapDataType dtype, uint32_t rank
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-static int fill_table(FrameTable& tab, const int32_t* kf_a, const int32_t* kf_b, const float* w, int F, int K,
-                      const char* who) {
-  if (F < 0 || F > kMaxFrames) { set_last_error("%s: F=%d outside [0,%d]", who, F, kMaxFrames); return TF_ERR_INVALID_ARGUMENT; }
+// The pointer rule of every entry point that enqueues work: each `required` pointer non-NULL and 16-byte aligned (the
+// kernels move 16-byte vectors and address operands through TMA), each `optional` one NULL or 16-byte aligned, and
+// `others_ok` the caller's verdict on the pointers that need less (coefficient rows, index and host tables).
+static int check_pointers(const char* who, std::initializer_list<const void*> required,
+                          std::initializer_list<const void*> optional = {}, bool others_ok = true) {
+  bool ok = others_ok;
+  for (const void* p : required) ok = ok && p && aligned16(p);
+  for (const void* p : optional) ok = ok && aligned16(p);
+  if (ok) return TF_OK;
+  set_last_error("%s: NULL or misaligned pointer", who);
+  return TF_ERR_INVALID_ARGUMENT;
+}
+
+// The status of `n_launches` kernel launches, counted for tf_launch_count when they were enqueued.
+static int launched(int e, long long n_launches = 1) {
+  if (!e) g_launches += n_launches;
+  return e;
+}
+
+// An element-wise entry point: a length outside [0, max_n] is refused, an empty call succeeds without looking at a
+// pointer, and `launch()` enqueues one kernel once the pointers pass check_pointers(who, ptrs, {}, others_ok).
+template <class Launch>
+static int elementwise(const char* who, int64_t n, int64_t max_n, std::initializer_list<const void*> ptrs,
+                       bool others_ok, Launch launch) {
+  if (n < 0 || n > max_n) { set_last_error("%s: n=%lld", who, (long long)n); return TF_ERR_INVALID_ARGUMENT; }
+  if (n == 0) return TF_OK;
+  if (int e = check_pointers(who, ptrs, {}, others_ok)) return e;
+  return launched(launch());
+}
+
+// Frames [f0, f0 + n) of one tf_nn_field / tf_propagate launch.
+struct FrameChunk {
+  int f0, n;
+  FrameTable tab;
+};
+
+// The launches of F frames, kMaxFrames per launch, every one validated before the caller enqueues the first.
+// need_b: some frame has a second keyframe.
+static int frame_chunks(std::vector<FrameChunk>& chunks, bool& need_b, const int32_t* kf_a, const int32_t* kf_b,
+                        const float* w, int F, int K, const char* who) {
   if (F > 0 && !kf_a) { set_last_error("%s: kf_a is NULL", who); return TF_ERR_INVALID_ARGUMENT; }
-  memset(&tab, 0, sizeof(tab));
-  for (int f = 0; f < F; ++f) {
-    const int a = kf_a[f];
-    const int b = kf_b ? kf_b[f] : -1;
-    if (a < 0 || a >= K || b >= K) {
-      set_last_error("%s: frame %d has keyframe ids (%d,%d) outside [0,%d)", who, f, a, b, K);
-      return TF_ERR_INVALID_ARGUMENT;
+  need_b = false;
+  for (int f0 = 0; f0 < F; f0 += kMaxFrames) {
+    chunks.push_back({f0, std::min(F - f0, kMaxFrames), {}});
+    FrameTable& tab = chunks.back().tab;
+    for (int f = 0; f < chunks.back().n; ++f) {
+      const int a = kf_a[f0 + f];
+      const int b = kf_b ? kf_b[f0 + f] : -1;
+      if (a < 0 || a >= K || b >= K) {
+        set_last_error("%s: frame %d has keyframe ids (%d,%d) outside [0,%d)", who, f, a, b, K);
+        return TF_ERR_INVALID_ARGUMENT;
+      }
+      tab.kf_a[f] = a;
+      tab.kf_b[f] = b < 0 ? -1 : b;
+      tab.w[f] = w ? w[f0 + f] : 1.0f;
+      need_b |= b >= 0;
     }
-    tab.kf_a[f] = a;
-    tab.kf_b[f] = b < 0 ? -1 : b;
-    tab.w[f] = w ? w[f] : 1.0f;
   }
   return TF_OK;
 }
@@ -147,13 +189,8 @@ int tf_unit_rows(const void* x, int x_is_f32, int64_t rows, int dim, int64_t x_r
     return TF_ERR_INVALID_ARGUMENT;
   }
   if (rows == 0) return TF_OK;
-  if (!x || !out_f16 || !aligned16(x) || !aligned16(out_f16)) {
-    set_last_error("tf_unit_rows: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  int e = launch_unit_rows(x, x_is_f32, rows, dim, x_row_stride, out_f16, static_cast<cudaStream_t>(stream));
-  if (!e) g_launches += 1;
-  return e;
+  if (int e = check_pointers("tf_unit_rows", {x, out_f16})) return e;
+  return launched(launch_unit_rows(x, x_is_f32, rows, dim, x_row_stride, out_f16, static_cast<cudaStream_t>(stream)));
 }
 
 int tf_layernorm_unit_rows(const void* x_f16, int64_t rows, int dim, int64_t x_row_stride, const float* gamma,
@@ -164,15 +201,9 @@ int tf_layernorm_unit_rows(const void* x_f16, int64_t rows, int dim, int64_t x_r
     return TF_ERR_INVALID_ARGUMENT;
   }
   if (rows == 0) return TF_OK;
-  if (!x_f16 || !gamma || !beta || !out_f16 || !aligned16(x_f16) || !aligned16(out_f16) || !aligned16(gamma) ||
-      !aligned16(beta)) {
-    set_last_error("tf_layernorm_unit_rows: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  int e = launch_layernorm_unit_rows(x_f16, rows, dim, x_row_stride, gamma, beta, eps, out_f16,
-                                     static_cast<cudaStream_t>(stream));
-  if (!e) g_launches += 1;
-  return e;
+  if (int e = check_pointers("tf_layernorm_unit_rows", {x_f16, gamma, beta, out_f16})) return e;
+  return launched(launch_layernorm_unit_rows(x_f16, rows, dim, x_row_stride, gamma, beta, eps, out_f16,
+                                             static_cast<cudaStream_t>(stream)));
 }
 
 int tf_layernorm_rows(const void* x_f16, int64_t rows, int dim, int64_t x_row_stride, const float* gamma,
@@ -186,68 +217,36 @@ int tf_layernorm_rows(const void* x_f16, int64_t rows, int dim, int64_t x_row_st
     return TF_ERR_INVALID_ARGUMENT;
   }
   if (rows == 0) return TF_OK;
-  if (!x_f16 || !gamma || !beta || !aligned16(x_f16) || !aligned16(gamma) || !aligned16(beta) ||
-      (y_out_f16 && !aligned16(y_out_f16)) || (unit_out_f16 && !aligned16(unit_out_f16))) {
-    set_last_error("tf_layernorm_rows: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
+  if (int e = check_pointers("tf_layernorm_rows", {x_f16, gamma, beta}, {y_out_f16, unit_out_f16})) return e;
   if (!y_out_f16 && (!unit_out_f16 || unit_rows == 0)) return TF_OK;
-  int e = launch_layernorm_rows(x_f16, rows, dim, x_row_stride, gamma, beta, eps, y_out_f16, y_row_stride,
-                                unit_out_f16, unit_row_stride, unit_rows, static_cast<cudaStream_t>(stream));
-  if (!e) g_launches += 1;
-  return e;
+  return launched(launch_layernorm_rows(x_f16, rows, dim, x_row_stride, gamma, beta, eps, y_out_f16, y_row_stride,
+                                        unit_out_f16, unit_row_stride, unit_rows, static_cast<cudaStream_t>(stream)));
 }
 
 int tf_cfg_ddim(const void* eps_uncond, const void* eps_cond, const void* x, const float* coef, float guidance,
                 int64_t n, void* out, tf_stream_t stream) {
-  if (n < 0) { set_last_error("tf_cfg_ddim: n=%lld", (long long)n); return TF_ERR_INVALID_ARGUMENT; }
-  if (n == 0) return TF_OK;
-  if (!eps_uncond || !eps_cond || !x || !coef || !out || !aligned16(eps_uncond) || !aligned16(eps_cond) ||
-      !aligned16(x) || !aligned16(out)) {
-    set_last_error("tf_cfg_ddim: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  int e = launch_cfg_ddim(eps_uncond, eps_cond, x, coef, guidance, n, out, static_cast<cudaStream_t>(stream));
-  if (!e) g_launches += 1;
-  return e;
+  return elementwise("tf_cfg_ddim", n, INT64_MAX, {eps_uncond, eps_cond, x, out}, coef != nullptr, [&] {
+    return launch_cfg_ddim(eps_uncond, eps_cond, x, coef, guidance, n, out, static_cast<cudaStream_t>(stream));
+  });
 }
 
 int tf_ddim(const void* eps, const void* x, const float* coef, int64_t n, void* out, tf_stream_t stream) {
-  if (n < 0) { set_last_error("tf_ddim: n=%lld", (long long)n); return TF_ERR_INVALID_ARGUMENT; }
-  if (n == 0) return TF_OK;
-  if (!eps || !x || !coef || !out || !aligned16(eps) || !aligned16(x) || !aligned16(out)) {
-    set_last_error("tf_ddim: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  int e = launch_ddim(eps, x, coef, n, out, static_cast<cudaStream_t>(stream));
-  if (!e) g_launches += 1;
-  return e;
+  return elementwise("tf_ddim", n, INT64_MAX, {eps, x, out}, coef != nullptr, [&] {
+    return launch_ddim(eps, x, coef, n, out, static_cast<cudaStream_t>(stream));
+  });
 }
 
 int tf_cfg_ddim_v(const void* v_uncond, const void* v_cond, const void* x, const float* coef, float guidance,
                   int64_t n, void* out, tf_stream_t stream) {
-  if (n < 0) { set_last_error("tf_cfg_ddim_v: n=%lld", (long long)n); return TF_ERR_INVALID_ARGUMENT; }
-  if (n == 0) return TF_OK;
-  if (!v_uncond || !v_cond || !x || !coef || !out || !aligned16(v_uncond) || !aligned16(v_cond) || !aligned16(x) ||
-      !aligned16(out)) {
-    set_last_error("tf_cfg_ddim_v: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  int e = launch_cfg_ddim_v(v_uncond, v_cond, x, coef, guidance, n, out, static_cast<cudaStream_t>(stream));
-  if (!e) g_launches += 1;
-  return e;
+  return elementwise("tf_cfg_ddim_v", n, INT64_MAX, {v_uncond, v_cond, x, out}, coef != nullptr, [&] {
+    return launch_cfg_ddim_v(v_uncond, v_cond, x, coef, guidance, n, out, static_cast<cudaStream_t>(stream));
+  });
 }
 
 int tf_ddim_v(const void* v, const void* x, const float* coef, int64_t n, void* out, tf_stream_t stream) {
-  if (n < 0) { set_last_error("tf_ddim_v: n=%lld", (long long)n); return TF_ERR_INVALID_ARGUMENT; }
-  if (n == 0) return TF_OK;
-  if (!v || !x || !coef || !out || !aligned16(v) || !aligned16(x) || !aligned16(out)) {
-    set_last_error("tf_ddim_v: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  int e = launch_ddim_v(v, x, coef, n, out, static_cast<cudaStream_t>(stream));
-  if (!e) g_launches += 1;
-  return e;
+  return elementwise("tf_ddim_v", n, INT64_MAX, {v, x, out}, coef != nullptr, [&] {
+    return launch_ddim_v(v, x, coef, n, out, static_cast<cudaStream_t>(stream));
+  });
 }
 
 int64_t tf_group_norm_nhwc_workspace(int64_t n, int64_t hw, int c, int groups) {
@@ -273,39 +272,22 @@ int tf_group_norm_nhwc(const void* x, const void* bias, int64_t bias_stride, con
     set_last_error("tf_group_norm_nhwc: workspace of %lld bytes, %lld needed", (long long)workspace_bytes, need);
     return TF_ERR_INVALID_ARGUMENT;
   }
-  if (!x || !gamma || !beta || !workspace || !out || !aligned16(x) || !aligned16(out) || !aligned16(workspace) ||
-      (bias && !aligned16(bias))) {
-    set_last_error("tf_group_norm_nhwc: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  int e = launch_group_norm_nhwc(x, bias, bias_stride, gamma, beta, n, hw, c, groups, eps, silu, workspace, out,
-                                 static_cast<cudaStream_t>(stream));
-  if (!e) g_launches += 2 * ((n + 65534) / 65535);
-  return e;
+  if (int e = check_pointers("tf_group_norm_nhwc", {x, workspace, out}, {bias}, gamma && beta)) return e;
+  return launched(launch_group_norm_nhwc(x, bias, bias_stride, gamma, beta, n, hw, c, groups, eps, silu, workspace,
+                                         out, static_cast<cudaStream_t>(stream)),
+                  2 * ((n + 65534) / 65535));
 }
 
 int tf_frames_to_nhwc(const void* frames_u8, int64_t n_px, void* out_f16, tf_stream_t stream) {
-  if (n_px < 0 || n_px > INT64_MAX / 3) { set_last_error("tf_frames_to_nhwc: n_px=%lld", (long long)n_px); return TF_ERR_INVALID_ARGUMENT; }
-  if (n_px == 0) return TF_OK;
-  if (!frames_u8 || !out_f16 || !aligned16(frames_u8) || !aligned16(out_f16)) {
-    set_last_error("tf_frames_to_nhwc: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  int e = launch_frames_to_nhwc(frames_u8, 3 * n_px, out_f16, static_cast<cudaStream_t>(stream));
-  if (!e) g_launches += 1;
-  return e;
+  return elementwise("tf_frames_to_nhwc", n_px, INT64_MAX / 3, {frames_u8, out_f16}, true, [&] {
+    return launch_frames_to_nhwc(frames_u8, 3 * n_px, out_f16, static_cast<cudaStream_t>(stream));
+  });
 }
 
 int tf_nhwc_to_frames(const void* x_f16, int64_t n_px, void* frames_u8, tf_stream_t stream) {
-  if (n_px < 0 || n_px > INT64_MAX / 3) { set_last_error("tf_nhwc_to_frames: n_px=%lld", (long long)n_px); return TF_ERR_INVALID_ARGUMENT; }
-  if (n_px == 0) return TF_OK;
-  if (!x_f16 || !frames_u8 || !aligned16(x_f16) || !aligned16(frames_u8)) {
-    set_last_error("tf_nhwc_to_frames: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  int e = launch_nhwc_to_frames(x_f16, 3 * n_px, frames_u8, static_cast<cudaStream_t>(stream));
-  if (!e) g_launches += 1;
-  return e;
+  return elementwise("tf_nhwc_to_frames", n_px, INT64_MAX / 3, {x_f16, frames_u8}, true, [&] {
+    return launch_nhwc_to_frames(x_f16, 3 * n_px, frames_u8, static_cast<cudaStream_t>(stream));
+  });
 }
 
 int tf_resize_taps(int in, int out) {
@@ -345,16 +327,10 @@ int tf_resize_u8(const void* in, int64_t n, int h_in, int w_in, int h, int w, co
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!need_h && !need_v)          // Pillow returns a copy when the size is unchanged
     return check_cuda(cudaMemcpyAsync(out, in, (size_t)n * h * w * 3, cudaMemcpyDeviceToDevice, st), "tf_resize_u8 copy");
-  if (need_h) {
-    int e = launch_resize_h(in, n * h_in, w_in, w, h_bounds, h_coeffs, h_taps, need_v ? tmp : out, st);
-    if (e) return e;
-    g_launches += 1;
-  }
-  if (need_v) {
-    int e = launch_resize_v(need_h ? tmp : in, n, h_in, h, w, v_bounds, v_coeffs, v_taps, out, st);
-    if (e) return e;
-    g_launches += 1;
-  }
+  if (need_h)
+    if (int e = launched(launch_resize_h(in, n * h_in, w_in, w, h_bounds, h_coeffs, h_taps, need_v ? tmp : out, st)))
+      return e;
+  if (need_v) return launched(launch_resize_v(need_h ? tmp : in, n, h_in, h, w, v_bounds, v_coeffs, v_taps, out, st));
   return TF_OK;
 }
 
@@ -380,27 +356,16 @@ int tf_canny_u8(const void* frames, int64_t n, int h, int w, double low, double 
     set_last_error("tf_canny_u8: workspace of %lld bytes, %lld needed", (long long)workspace_bytes, need);
     return TF_ERR_INVALID_ARGUMENT;
   }
-  if (!frames || !workspace || (!edges_u8 && !cond_f16) || !aligned16(workspace) ||
-      (cond_f16 && (reinterpret_cast<uintptr_t>(cond_f16) & 1u))) {
-    set_last_error("tf_canny_u8: NULL or misaligned pointer (frames, a 16-byte aligned workspace, and at least one "
-                   "output are needed)");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  int e = launch_canny(frames, n, h, w, ilo, ihi, workspace, edges_u8, cond_f16, static_cast<cudaStream_t>(stream));
-  if (!e) g_launches += 5;
-  return e;
+  // the fp16 conditioning output is written element by element: 2-byte alignment is enough
+  const bool cond_ok = !(reinterpret_cast<uintptr_t>(cond_f16) & 1u);
+  if (int e = check_pointers("tf_canny_u8", {workspace}, {}, frames && (edges_u8 || cond_f16) && cond_ok)) return e;
+  return launched(
+      launch_canny(frames, n, h, w, ilo, ihi, workspace, edges_u8, cond_f16, static_cast<cudaStream_t>(stream)), 5);
 }
 
 int tf_geglu(const void* xh, const void* gate, int64_t n, void* out, tf_stream_t stream) {
-  if (n < 0) { set_last_error("tf_geglu: n=%lld", (long long)n); return TF_ERR_INVALID_ARGUMENT; }
-  if (n == 0) return TF_OK;
-  if (!xh || !gate || !out || !aligned16(xh) || !aligned16(gate) || !aligned16(out)) {
-    set_last_error("tf_geglu: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
-  int e = launch_geglu(xh, gate, n, out, static_cast<cudaStream_t>(stream));
-  if (!e) g_launches += 1;
-  return e;
+  return elementwise("tf_geglu", n, INT64_MAX, {xh, gate, out}, true,
+                     [&] { return launch_geglu(xh, gate, n, out, static_cast<cudaStream_t>(stream)); });
 }
 
 int tf_nn_field(const void* x_unit, const void* piv_unit, const int32_t* kf_a, const int32_t* kf_b, int F, int S,
@@ -409,30 +374,17 @@ int tf_nn_field(const void* x_unit, const void* piv_unit, const int32_t* kf_a, c
     set_last_error("tf_nn_field: bad shape F=%d S=%d dim=%d K=%d", F, S, dim, K);
     return TF_ERR_INVALID_ARGUMENT;
   }
-  if (F > 0 && !kf_a) { set_last_error("tf_nn_field: kf_a is NULL"); return TF_ERR_INVALID_ARGUMENT; }
-  // validate every chunk before the first launch
-  for (int f0 = 0; f0 < F; f0 += kMaxFrames) {
-    FrameTable tab;
-    const int fc = F - f0 < kMaxFrames ? F - f0 : kMaxFrames;
-    if (int e = fill_table(tab, kf_a + f0, kf_b ? kf_b + f0 : nullptr, nullptr, fc, K, "tf_nn_field")) return e;
-  }
+  std::vector<FrameChunk> chunks;
+  bool need_b;
+  if (int e = frame_chunks(chunks, need_b, kf_a, kf_b, nullptr, F, K, "tf_nn_field")) return e;
   if (F == 0 || S == 0) return TF_OK;
-  bool need_b = false;
-  if (kf_b) for (int f = 0; f < F; ++f) need_b |= kf_b[f] >= 0;
-  if (!x_unit || !piv_unit || !idx_a || (need_b && !idx_b) || !aligned16(x_unit) || !aligned16(piv_unit)) {
-    set_last_error("tf_nn_field: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
+  if (int e = check_pointers("tf_nn_field", {x_unit, piv_unit}, {}, idx_a && (!need_b || idx_b))) return e;
   const __half* xu = static_cast<const __half*>(x_unit);
-  for (int f0 = 0; f0 < F; f0 += kMaxFrames) {         // any number of frames: kMaxFrames per launch
-    FrameTable tab;
-    const int fc = F - f0 < kMaxFrames ? F - f0 : kMaxFrames;
-    fill_table(tab, kf_a + f0, kf_b ? kf_b + f0 : nullptr, nullptr, fc, K, "tf_nn_field");
-    const long long off = (long long)f0 * S;
-    int e = launch_nn_field(xu + off * dim, piv_unit, tab, fc, S, dim, K, idx_a + off, idx_b ? idx_b + off : nullptr,
-                            static_cast<cudaStream_t>(stream));
-    if (e) return e;
-    g_launches += 1;
+  for (const FrameChunk& c : chunks) {                  // any number of frames: kMaxFrames per launch
+    const long long off = (long long)c.f0 * S;
+    if (int e = launched(launch_nn_field(xu + off * dim, piv_unit, c.tab, c.n, S, dim, K, idx_a + off,
+                                         idx_b ? idx_b + off : nullptr, static_cast<cudaStream_t>(stream))))
+      return e;
   }
   return TF_OK;
 }
@@ -444,33 +396,19 @@ int tf_propagate(const void* A, const int32_t* idx_a, const int32_t* idx_b, cons
     set_last_error("tf_propagate: bad shape F=%d S=%d dim=%d K=%d", F, S, dim, K);
     return TF_ERR_INVALID_ARGUMENT;
   }
-  if (F > 0 && !kf_a) { set_last_error("tf_propagate: kf_a is NULL"); return TF_ERR_INVALID_ARGUMENT; }
-  bool need_b = false;
-  for (int f0 = 0; f0 < F; f0 += kMaxFrames) {
-    FrameTable tab;
-    const int fc = F - f0 < kMaxFrames ? F - f0 : kMaxFrames;
-    if (int e = fill_table(tab, kf_a + f0, kf_b ? kf_b + f0 : nullptr, w ? w + f0 : nullptr, fc, K, "tf_propagate"))
-      return e;
-    for (int f = 0; f < fc; ++f) need_b |= tab.kf_b[f] >= 0;
-  }
+  std::vector<FrameChunk> chunks;
+  bool need_b;
+  if (int e = frame_chunks(chunks, need_b, kf_a, kf_b, w, F, K, "tf_propagate")) return e;
   if (F == 0 || S == 0) return TF_OK;
-  if (!A || !idx_a || !out || (need_b && (!idx_b || !w)) || !aligned16(A) || !aligned16(out) ||
-      (residual && !aligned16(residual))) {
-    set_last_error("tf_propagate: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
+  if (int e = check_pointers("tf_propagate", {A, out}, {residual}, idx_a && (!need_b || (idx_b && w)))) return e;
   const size_t out_esz = out_is_f32 ? 4 : 2;
-  for (int f0 = 0; f0 < F; f0 += kMaxFrames) {         // any number of frames: kMaxFrames per launch, no copies
-    FrameTable tab;
-    const int fc = F - f0 < kMaxFrames ? F - f0 : kMaxFrames;
-    fill_table(tab, kf_a + f0, kf_b ? kf_b + f0 : nullptr, w ? w + f0 : nullptr, fc, K, "tf_propagate");
-    const long long off = (long long)f0 * S;
-    int e = launch_propagate(A, idx_a + off, idx_b ? idx_b + off : nullptr, tab, fc, S, dim, K,
-                             residual ? static_cast<const __half*>(residual) + off * dim : nullptr,
-                             static_cast<char*>(out) + (size_t)off * dim * out_esz, out_is_f32, F,
-                             static_cast<cudaStream_t>(stream));
-    if (e) return e;
-    g_launches += 1;
+  for (const FrameChunk& c : chunks) {                  // any number of frames: kMaxFrames per launch, no copies
+    const long long off = (long long)c.f0 * S;
+    if (int e = launched(launch_propagate(A, idx_a + off, idx_b ? idx_b + off : nullptr, c.tab, c.n, S, dim, K,
+                                          residual ? static_cast<const __half*>(residual) + off * dim : nullptr,
+                                          static_cast<char*>(out) + (size_t)off * dim * out_esz, out_is_f32, F,
+                                          static_cast<cudaStream_t>(stream))))
+      return e;
   }
   return TF_OK;
 }
@@ -492,11 +430,8 @@ int tf_ext_attn_fwd_rows(const void* q, int q_slabs, int64_t q_tok_stride, const
     return TF_ERR_INVALID_ARGUMENT;
   }
   if (n_out == 0 || S == 0 || q_nrows == 0 || q_row0 >= S) return TF_OK;
-  if (!q || !k || !v || !out || !out_slab || !q_slab || !k_slab0 || !v_slab0 || !n_kv || !aligned16(q) ||
-      !aligned16(k) || !aligned16(v) || !aligned16(out)) {
-    set_last_error("tf_ext_attn: NULL or misaligned pointer");
-    return TF_ERR_INVALID_ARGUMENT;
-  }
+  if (int e = check_pointers("tf_ext_attn", {q, k, v, out}, {}, out_slab && q_slab && k_slab0 && v_slab0 && n_kv))
+    return e;
   for (int i = 0; i < n_out; ++i) {
     if (q_slab[i] < 0 || q_slab[i] >= q_slabs || n_kv[i] <= 0 || k_slab0[i] < 0 || v_slab0[i] < 0 ||
         k_slab0[i] + n_kv[i] > kv_slabs || v_slab0[i] + n_kv[i] > kv_slabs || out_slab[i] < 0) {
@@ -542,10 +477,10 @@ int tf_ext_attn_fwd_rows(const void* q, int q_slabs, int64_t q_tok_stride, const
         ptab.p[slot].v_c0 = v_slab0[j];
         ptab.p[slot].n_kv = n_kv[i];
       }
-      int e = launch_ext_attn_pairs(q, k, v, q_tok_stride, kv_tok_stride, q_slabs, kv_slabs, ptab, nc, S, heads, d, scale,
-                                    out, q_row0, q_nrows, static_cast<cudaStream_t>(stream));
-      if (e) return e;
-      g_launches += 1;
+      if (int e = launched(launch_ext_attn_pairs(q, k, v, q_tok_stride, kv_tok_stride, q_slabs, kv_slabs, ptab, nc, S,
+                                                 heads, d, scale, out, q_row0, q_nrows,
+                                                 static_cast<cudaStream_t>(stream))))
+        return e;
     }
   }
   // heavy samples (most key slabs) first: the hardware block scheduler then fills the tail of the
@@ -567,10 +502,9 @@ int tf_ext_attn_fwd_rows(const void* q, int q_slabs, int64_t q_tok_stride, const
       tab.s[slot].v_sample0 = v_slab0[i];
       tab.s[slot].n_kv = n_kv[i];
     }
-    int e = launch_ext_attn(q, k, v, q_tok_stride, kv_tok_stride, q_slabs, kv_slabs, tab, nc, S, heads, d, scale, out,
-                            q_row0, q_nrows, static_cast<cudaStream_t>(stream));
-    if (e) return e;
-    g_launches += 1;
+    if (int e = launched(launch_ext_attn(q, k, v, q_tok_stride, kv_tok_stride, q_slabs, kv_slabs, tab, nc, S, heads, d,
+                                         scale, out, q_row0, q_nrows, static_cast<cudaStream_t>(stream))))
+      return e;
   }
   return TF_OK;
 }

@@ -29,7 +29,7 @@ int launch_layernorm_rows(const void* x_f16, long long rows, int dim, long long 
 int launch_cfg_ddim(const void* eps_uncond, const void* eps_cond, const void* x, const float* coef_dev, float guidance,
                     long long n, void* out, cudaStream_t stream);
 int launch_ddim(const void* eps, const void* x, const float* coef_dev, long long n, void* out, cudaStream_t stream);
-// The same two updates for a v-prediction model (include/tokenflow_b200_vpred.h).
+// The same two updates for a v-prediction model (tf_cfg_ddim_v / tf_ddim_v).
 int launch_cfg_ddim_v(const void* v_uncond, const void* v_cond, const void* x, const float* coef_dev, float guidance,
                       long long n, void* out, cudaStream_t stream);
 int launch_ddim_v(const void* v, const void* x, const float* coef_dev, long long n, void* out, cudaStream_t stream);

@@ -39,6 +39,10 @@ _SIGNATURES = {
                                    ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
     "tf_ddim": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
                                ctypes.c_void_p]),
+    "tf_cfg_ddim_v": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                     ctypes.c_float, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
+    "tf_ddim_v": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
+                                 ctypes.c_void_p]),
     "tf_comm_nccl_version": (ctypes.c_int, []),
     "tf_comm_unique_id": (ctypes.c_int, [ctypes.c_void_p]),
     "tf_comm_init": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_void_p)]),
@@ -76,13 +80,6 @@ _SIGNATURES = {
     "tf_geglu": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
 }
 
-# the v-prediction latent updates; mirrors include/tokenflow_b200_vpred.h one to one (same library, same signatures as
-# tf_cfg_ddim / tf_ddim)
-_VPRED_SIGNATURES = {
-    "tf_cfg_ddim_v": _SIGNATURES["tf_cfg_ddim"],
-    "tf_ddim_v": _SIGNATURES["tf_ddim"],
-}
-
 
 class TokenflowB200Error(RuntimeError):
     pass
@@ -106,7 +103,7 @@ def load_library() -> ctypes.CDLL:
             f"{path} is missing: build it with `python -m tokenflow_b200._build` "
             "(or __graft_entry__.build()).  tokenflow_b200 has no fallback path.")
     lib = ctypes.CDLL(str(path))
-    for name, (res, args) in list(_SIGNATURES.items()) + list(_VPRED_SIGNATURES.items()):
+    for name, (res, args) in _SIGNATURES.items():
         fn = getattr(lib, name)           # AttributeError here = header and library disagree
         fn.restype = res
         fn.argtypes = args
@@ -148,6 +145,35 @@ def _dense(t: torch.Tensor, memory_format=torch.contiguous_format) -> torch.Tens
     return t.clone(memory_format=memory_format)
 
 
+def _rows(t: torch.Tensor, multiple: int) -> torch.Tensor:
+    """`t` itself when the kernels can address its rows (its last dimension) in place: last dimension contiguous, rows
+    equally spaced by a pitch of a multiple of `multiple` elements, the first one on a 16-byte boundary (a column slice
+    of a packed buffer qualifies); else a dense copy, as in `_dense`."""
+    spaced = all(t.stride(i) == t.shape[i + 1] * t.stride(i + 1) for i in range(t.dim() - 2) if t.shape[i] > 1)
+    if t.stride(-1) == 1 and t.stride(-2) % multiple == 0 and spaced and t.data_ptr() % 16 == 0:
+        return t
+    return t.clone(memory_format=torch.contiguous_format)
+
+
+def _out_buffer(out: Optional[torch.Tensor], shape, device, scratch: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Where a kernel writes the fp16 output `out`: `out` itself when it starts on a 16-byte boundary, else `scratch`
+    or a new dense buffer of `shape` (also when `out` is None), which `_written` copies back."""
+    if out is not None and out.data_ptr() % 16 == 0:
+        return out
+    return scratch if scratch is not None else torch.empty(shape, dtype=torch.float16, device=device)
+
+
+def _written(out: Optional[torch.Tensor], buf: torch.Tensor) -> torch.Tensor:
+    """The output `out` (or `buf` when there is none) holding what the kernel wrote into `_out_buffer`'s `buf`."""
+    return buf if out is None or out is buf else out.copy_(buf)
+
+
+def _check(lib: ctypes.CDLL, status: int, what: str):
+    if status != 0:
+        msg = lib.tf_last_error().decode(errors="replace")
+        raise TokenflowB200Error(f"{what} failed (status {status}): {msg}")
+
+
 def _i32(vals: Sequence[int]):
     return (ctypes.c_int32 * len(vals))(*[int(v) for v in vals])
 
@@ -171,11 +197,6 @@ class CudaOps:
             raise TokenflowB200Error(f"tokenflow_b200 kernels are compiled for sm_90a only (got sm_{major}{minor})")
 
     # -- helpers ---------------------------------------------------------------------------
-    def _check(self, status: int, what: str):
-        if status != 0:
-            msg = self.lib.tf_last_error().decode(errors="replace")
-            raise TokenflowB200Error(f"{what} failed (status {status}): {msg}")
-
     @staticmethod
     def _stream() -> int:
         return torch.cuda.current_stream().cuda_stream
@@ -191,17 +212,19 @@ class CudaOps:
         (current) stream; `timing_summary()` synchronises and aggregates them per kernel."""
         self._timing = [] if on else None
 
-    def _timed(self, name: str, work: float, fn):
+    def _launch(self, timer: str, work: float, fn: str, *args):
+        """Enqueue the C entry point `fn`(*args, stream) on the current stream, timed as `timer` with `work` when timing
+        is on, and raise on a nonzero status."""
+        entry = getattr(self.lib, fn)
         if self._timing is None:
-            return fn()
+            return _check(self.lib, entry(*args, self._stream()), fn)
         ext = torch.cuda.is_current_stream_capturing()    # inside a CUDA-graph capture: event-record NODES
         start = torch.cuda.Event(enable_timing=True, external=ext)
         end = torch.cuda.Event(enable_timing=True, external=ext)
         start.record()
-        out = fn()
+        _check(self.lib, entry(*args, self._stream()), fn)
         end.record()
-        self._timing.append((name, float(work), start, end))
-        return out
+        self._timing.append((timer, float(work), start, end))
 
     def timing_summary(self):
         """{kernel: {"launches", "ms", "work"}}; `work` = algorithmic flops (tensor-bound kernels)
@@ -224,14 +247,11 @@ class CudaOps:
         if x.dtype not in (torch.float32, torch.float16):
             x = x.float()
         dim = x.shape[-1]
-        x2 = x.reshape(-1, dim)
-        if x2.stride(-1) != 1 or x2.stride(0) % 4 or x2.data_ptr() % 16:
-            x2 = x2.clone(memory_format=torch.contiguous_format)     # rows the kernel's loads cannot address
+        x2 = _rows(x.reshape(-1, dim), 4)
         out = torch.empty(x2.shape, dtype=torch.float16, device=x.device)
         nbytes = x2.shape[0] * dim * (x2.element_size() + 2)
-        self._timed("tf_unit_rows", nbytes, lambda: self._check(
-            self.lib.tf_unit_rows(x2.data_ptr(), int(x2.dtype == torch.float32), x2.shape[0], dim,
-                                  x2.stride(0), out.data_ptr(), self._stream()), "tf_unit_rows"))
+        self._launch("tf_unit_rows", nbytes, "tf_unit_rows", x2.data_ptr(), int(x2.dtype == torch.float32), x2.shape[0],
+                     dim, x2.stride(0), out.data_ptr())
         return out.view(*x.shape)
 
     @staticmethod
@@ -259,14 +279,10 @@ class CudaOps:
         if not self._ln_fusable(x, norm):
             return self.unit_rows(norm(x))                       # shapes the fused kernel does not cover
         gamma, beta = self._affine_f32(norm, x.device)
-        x2 = x.reshape(-1, dim)
-        if x2.stride(-1) != 1 or x2.stride(0) % 8 or x2.data_ptr() % 16:
-            x2 = x2.clone(memory_format=torch.contiguous_format)     # rows the kernel's 16-byte loads cannot address
+        x2 = _rows(x.reshape(-1, dim), 8)
         out = torch.empty(x2.shape, dtype=torch.float16, device=x.device)
-        self._timed("tf_layernorm_unit_rows", x2.shape[0] * dim * 4, lambda: self._check(
-            self.lib.tf_layernorm_unit_rows(x2.data_ptr(), x2.shape[0], dim, x2.stride(0), gamma.data_ptr(),
-                                            beta.data_ptr(), float(norm.eps), out.data_ptr(), self._stream()),
-            "tf_layernorm_unit_rows"))
+        self._launch("tf_layernorm_unit_rows", x2.shape[0] * dim * 4, "tf_layernorm_unit_rows", x2.data_ptr(),
+                     x2.shape[0], dim, x2.stride(0), gamma.data_ptr(), beta.data_ptr(), float(norm.eps), out.data_ptr())
         return out.view(*x.shape)
 
     def layernorm_rows(self, x: torch.Tensor, norm: torch.nn.LayerNorm, n_unit: int,
@@ -287,30 +303,17 @@ class CudaOps:
                 unit_out.copy_(unit); unit = unit_out
             return y, unit
         gamma, beta = self._affine_f32(norm, x.device)
-        x2 = x.reshape(-1, dim)
-        if x2.stride(-1) != 1 or x2.stride(0) % 8 or x2.data_ptr() % 16:
-            x2 = x2.clone(memory_format=torch.contiguous_format)     # rows the kernel's 16-byte loads cannot address
-        y_dst, unit_dst = y_out, unit_out
-        y_out = y_out if y_out is not None and y_out.data_ptr() % 16 == 0 else None
-        unit_out = unit_out if unit_out is not None and unit_out.data_ptr() % 16 == 0 else None
-        y = torch.empty((b, S, dim), dtype=torch.float16, device=x.device) if y_out is None else y_out
-        unit = None
-        if n_unit:
-            unit = torch.empty((n_unit, S, dim), dtype=torch.float16, device=x.device) if unit_out is None else unit_out
+        x2 = _rows(x.reshape(-1, dim), 8)
+        y = _out_buffer(y_out, (b, S, dim), x.device)
+        unit = _out_buffer(unit_out, (n_unit, S, dim), x.device) if n_unit else None
         def pitch(t):      # row pitch of a [.., S, dim] view whose rows are equally spaced
             assert t.stride(-1) == 1 and t.stride(-2) % 8 == 0 and (t.shape[0] <= 1 or t.stride(0) == S * t.stride(-2))
             return t.stride(-2)
-        self._timed("tf_layernorm_rows", x2.shape[0] * dim * 4 + n_unit * S * dim * 2, lambda: self._check(
-            self.lib.tf_layernorm_rows(x2.data_ptr(), x2.shape[0], dim, x2.stride(0), gamma.data_ptr(), beta.data_ptr(),
-                                       float(norm.eps), y.data_ptr(), pitch(y),
-                                       unit.data_ptr() if unit is not None else None,
-                                       pitch(unit) if unit is not None else dim, n_unit * S, self._stream()),
-            "tf_layernorm_rows"))
-        if y_dst is not None and y_dst is not y:
-            y = y_dst.copy_(y)
-        if unit_dst is not None and unit is not None and unit_dst is not unit:
-            unit = unit_dst.copy_(unit)
-        return y, unit
+        self._launch("tf_layernorm_rows", x2.shape[0] * dim * 4 + n_unit * S * dim * 2, "tf_layernorm_rows",
+                     x2.data_ptr(), x2.shape[0], dim, x2.stride(0), gamma.data_ptr(), beta.data_ptr(), float(norm.eps),
+                     y.data_ptr(), pitch(y), unit.data_ptr() if unit is not None else None,
+                     pitch(unit) if unit is not None else dim, n_unit * S)
+        return _written(y_out, y), _written(unit_out, unit) if unit is not None else None
 
     def cfg_ddim(self, eps_uncond: torch.Tensor, eps_cond: torch.Tensor, x: torch.Tensor, coef: torch.Tensor,
                  guidance: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -322,7 +325,7 @@ class CudaOps:
 
     def cfg_ddim_v(self, v_uncond: torch.Tensor, v_cond: torch.Tensor, x: torch.Tensor, coef: torch.Tensor,
                    guidance: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """`cfg_ddim` for a v-prediction model (include/tokenflow_b200_vpred.h): guidance on the two velocity
+        """`cfg_ddim` for a v-prediction model (include/tokenflow_b200.h): guidance on the two velocity
         predictions, then diffusers' v-branch of the DDIM step; `coef` = device fp32 [4]: sqrt(a_t), sqrt(1-a_t),
         sqrt(a_prev), sqrt(1-a_prev).  Operands and `out` as in `cfg_ddim`."""
         return self._cfg_step("tf_cfg_ddim_v", v_uncond, v_cond, x, coef, guidance, out)
@@ -332,15 +335,12 @@ class CudaOps:
         assert u.dtype == c.dtype == x.dtype == torch.float16 and coef.dtype == torch.float32
         eu, ec, xx = (_dense(t) for t in (u, c, x))
         assert eu.shape == ec.shape == xx.shape
-        if out is None:
-            out = torch.empty_like(xx)
-        assert out.shape == xx.shape and out.dtype == torch.float16 and out.is_contiguous()
-        dst = out if out.data_ptr() % 16 == 0 else torch.empty_like(xx)
+        assert out is None or (out.shape == xx.shape and out.dtype == torch.float16 and out.is_contiguous())
+        dst = _out_buffer(out, xx.shape, xx.device)
         n = xx.numel()
-        self._timed(fn, n * 8.0, lambda: self._check(
-            getattr(self.lib, fn)(eu.data_ptr(), ec.data_ptr(), xx.data_ptr(), coef.data_ptr(), float(guidance), n,
-                                  dst.data_ptr(), self._stream()), fn))
-        return out if dst is out else out.copy_(dst)
+        self._launch(fn, n * 8.0, fn, eu.data_ptr(), ec.data_ptr(), xx.data_ptr(), coef.data_ptr(), float(guidance), n,
+                     dst.data_ptr())
+        return _written(out, dst)
 
     def ddim(self, eps: torch.Tensor, x: torch.Tensor, coef: torch.Tensor,
              out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -353,7 +353,7 @@ class CudaOps:
 
     def ddim_v(self, v: torch.Tensor, x: torch.Tensor, coef: torch.Tensor,
                out: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """`ddim` for a v-prediction model (include/tokenflow_b200_vpred.h), diffusers' DDIMInverseScheduler /
+        """`ddim` for a v-prediction model (include/tokenflow_b200.h), diffusers' DDIMInverseScheduler /
         DDIMScheduler v-branch; `coef` = device fp32 [4]: inversion (mu_prev, sigma_prev, mu, sigma), reconstruction
         (mu, sigma, mu_prev, sigma_prev).  Operands, `out` and in place as in `ddim`."""
         return self._step("tf_ddim_v", v, x, coef, out)
@@ -361,16 +361,13 @@ class CudaOps:
     def _step(self, fn: str, m: torch.Tensor, x: torch.Tensor, coef: torch.Tensor,
               out: Optional[torch.Tensor]) -> torch.Tensor:
         assert m.dtype == x.dtype == torch.float16 and coef.dtype == torch.float32 and coef.is_cuda
-        assert m.shape == x.shape
-        if out is None:
-            out = torch.empty_like(x, memory_format=torch.contiguous_format)
-        assert out.shape == x.shape and out.dtype == torch.float16 and out.is_contiguous() and x.is_contiguous()
+        assert m.shape == x.shape and x.is_contiguous()
+        assert out is None or (out.shape == x.shape and out.dtype == torch.float16 and out.is_contiguous())
         e, xx = _dense(m), _dense(x)
-        dst = xx if out is x else (out if out.data_ptr() % 16 == 0 else torch.empty_like(out))
+        dst = _out_buffer(out, x.shape, x.device, scratch=xx if out is x else None)     # in place: x's aligned copy
         n = x.numel()
-        self._timed(fn, n * 6.0, lambda: self._check(
-            getattr(self.lib, fn)(e.data_ptr(), xx.data_ptr(), coef.data_ptr(), n, dst.data_ptr(), self._stream()), fn))
-        return out if dst is out else out.copy_(dst)
+        self._launch(fn, n * 6.0, fn, e.data_ptr(), xx.data_ptr(), coef.data_ptr(), n, dst.data_ptr())
+        return _written(out, dst)
 
     def nn_field(self, x_unit: torch.Tensor, piv_unit: torch.Tensor, kf_a: Sequence[int],
                  kf_b: Sequence[int]) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
@@ -386,9 +383,9 @@ class CudaOps:
         any_b = any(int(b) >= 0 for b in kf_b)
         idx_b = torch.empty((F_, S), dtype=torch.int32, device=x_unit.device) if any_b else None
         pairs = F_ + sum(1 for b in kf_b if int(b) >= 0)
-        self._timed("tf_nn_field", 2.0 * pairs * S * S * dim, lambda: self._check(self.lib.tf_nn_field(
-            x_unit.data_ptr(), piv_unit.data_ptr(), _i32(kf_a), _i32(kf_b), F_, S, dim, K, idx_a.data_ptr(),
-            idx_b.data_ptr() if idx_b is not None else None, self._stream()), "tf_nn_field"))
+        self._launch("tf_nn_field", 2.0 * pairs * S * S * dim, "tf_nn_field", x_unit.data_ptr(), piv_unit.data_ptr(),
+                     _i32(kf_a), _i32(kf_b), F_, S, dim, K, idx_a.data_ptr(),
+                     idx_b.data_ptr() if idx_b is not None else None)
         return idx_a, idx_b
 
     def propagate(self, A: torch.Tensor, idx_a: torch.Tensor, idx_b: Optional[torch.Tensor],
@@ -406,12 +403,11 @@ class CudaOps:
             residual = _dense(residual.to(torch.float16)).view(3, F_, S, dim)
         out = torch.empty((3, F_, S, dim), dtype=out_dtype, device=A.device)
         assert out_dtype in (torch.float16, torch.float32)
-        self._timed("tf_propagate", propagate_bytes(F_, S, dim, kf_a, kf_b, residual is not None,
-                                                    out.element_size()), lambda: self._check(
-            self.lib.tf_propagate(
-                A.data_ptr(), idx_a.data_ptr(), idx_b.data_ptr() if idx_b is not None else None, _i32(kf_a),
-                _i32(kf_b), _f32(w), F_, S, dim, K, residual.data_ptr() if residual is not None else None,
-                out.data_ptr(), int(out_dtype == torch.float32), self._stream()), "tf_propagate"))
+        self._launch("tf_propagate", propagate_bytes(F_, S, dim, kf_a, kf_b, residual is not None, out.element_size()),
+                     "tf_propagate", A.data_ptr(), idx_a.data_ptr(), idx_b.data_ptr() if idx_b is not None else None,
+                     _i32(kf_a), _i32(kf_b), _f32(w), F_, S, dim, K,
+                     residual.data_ptr() if residual is not None else None, out.data_ptr(),
+                     int(out_dtype == torch.float32))
         return out.view(3 * F_, S, dim)
 
     def ext_attn(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, scale: float,
@@ -422,32 +418,14 @@ class CudaOps:
         b, S, dim = q.shape
         n = b // 3
         d = dim // heads
-        q, k, v = (t if t.dtype == torch.float16 else t.to(torch.float16) for t in (q, k, v))
-        strides = {(t.stride(0), t.stride(1), t.stride(2)) for t in (q, k, v)}
-        tok = q.stride(1)
-        if len(strides) != 1 or q.stride(2) != 1 or q.stride(0) != S * tok or any(t.data_ptr() % 16 for t in (q, k, v)):
-            q, k, v = _dense(q), _dense(k), _dense(v)
-            tok = dim
+        q, k, v = (_rows(t.to(torch.float16), 8) for t in (q, k, v))
+        if len({t.stride() for t in (q, k, v)}) != 1:         # one token stride for all three
+            q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
         out = torch.empty((b, S, dim), dtype=torch.float16, device=q.device)
         flops = 4.0 * n * S * S * dim * (2 * n + 1)        # QK^T + PV; source: S keys, uncond+cond: n*S keys
-        self._timed("tf_ext_attn", flops, lambda: self._check(
-            self.lib.tf_ext_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), tok, n, S, heads, d,
-                                     float(scale), int(bool(inject)), out.data_ptr(), self._stream()),
-            "tf_ext_attn_fwd"))
+        self._launch("tf_ext_attn", flops, "tf_ext_attn_fwd", q.data_ptr(), k.data_ptr(), v.data_ptr(), q.stride(1),
+                     n, S, heads, d, float(scale), int(bool(inject)), out.data_ptr())
         return out
-
-    @staticmethod
-    def _slab_view(t: torch.Tensor):
-        """(tensor, token stride) of a [slabs, S, dim] fp16 operand the kernels can address in place: last dim
-        contiguous, slabs S tokens apart (a column slice of a packed [slabs, S, n*dim] buffer qualifies), 16-byte aligned;
-        anything else is copied."""
-        if t.dtype != torch.float16:
-            t = t.to(torch.float16)
-        S = t.shape[1]
-        if t.stride(2) != 1 or t.stride(1) % 8 or (t.shape[0] > 1 and t.stride(0) != S * t.stride(1)) \
-                or t.data_ptr() % 16:
-            t = _dense(t)
-        return t, t.stride(1)
 
     def ext_attn_table(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, table, heads: int,
                        scale: float, row0: int = 0, nrows: Optional[int] = None) -> torch.Tensor:
@@ -459,19 +437,17 @@ class CudaOps:
         _, S, dim = q.shape
         d = dim // heads
         nrows = S if nrows is None else int(nrows)
-        (q, q_tok), (k, k_tok), (v, v_tok) = self._slab_view(q), self._slab_view(k), self._slab_view(v)
-        if k_tok != v_tok:
+        q, k, v = (_rows(t.to(torch.float16), 8) for t in (q, k, v))
+        if k.stride(1) != v.stride(1):
             k, v = k.contiguous(), v.contiguous()
-            k_tok = v_tok = dim
         n_out = len(table)
         out = torch.empty((n_out, nrows, dim), dtype=torch.float16, device=q.device)
         rows_eff = max(0, min(S, row0 + nrows) - row0)
         flops = sum(4.0 * rows_eff * (nkv * S) * dim for (_, _, _, nkv) in table)
-        self._timed("tf_ext_attn", flops, lambda: self._check(self.lib.tf_ext_attn_fwd_rows(
-            q.data_ptr(), q.shape[0], q_tok, k.data_ptr(), v.data_ptr(), k.shape[0], k_tok, n_out,
-            _i32(range(n_out)), _i32([t[0] for t in table]), _i32([t[1] for t in table]),
-            _i32([t[2] for t in table]), _i32([t[3] for t in table]), S, heads, d, float(scale), int(row0), nrows,
-            out.data_ptr(), self._stream()), "tf_ext_attn_fwd_rows"))
+        self._launch("tf_ext_attn", flops, "tf_ext_attn_fwd_rows", q.data_ptr(), q.shape[0], q.stride(1), k.data_ptr(),
+                     v.data_ptr(), k.shape[0], k.stride(1), n_out, _i32(range(n_out)), _i32([t[0] for t in table]),
+                     _i32([t[1] for t in table]), _i32([t[2] for t in table]), _i32([t[3] for t in table]), S, heads,
+                     d, float(scale), int(row0), nrows, out.data_ptr())
         return out
 
     # -- UNet body ----------------------------------------------------------------------------
@@ -504,20 +480,18 @@ class CudaOps:
         x = _dense(x, torch.channels_last)
         if bias is not None:
             assert bias.dtype == torch.float16 and bias.dim() == 2 and bias.shape[1] == c and bias.shape[0] in (1, n)
-            if bias.stride(1) != 1 or bias.stride(0) % 8 or bias.data_ptr() % 16:
-                bias = bias.clone(memory_format=torch.contiguous_format)
+            bias = _rows(bias, 8)
             bias_stride = 0 if bias.shape[0] == 1 else bias.stride(0)
         ws_bytes = int(self.lib.tf_group_norm_nhwc_workspace(n, h * w, c, norm.num_groups))
         if ws_bytes < 0:
-            self._check(3, "tf_group_norm_nhwc_workspace")
+            _check(self.lib, 3, "tf_group_norm_nhwc_workspace")
         ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=x.device)
         out = torch.empty_like(x, memory_format=torch.channels_last)
         work = 3.0 * x.numel() * 2 + (n * c * 2 if bias is not None else 0)
         name = "tf_group_norm_g4" if c == 4 * norm.num_groups else "tf_group_norm"
-        self._timed(name, work, lambda: self._check(self.lib.tf_group_norm_nhwc(
-            x.data_ptr(), bias.data_ptr() if bias is not None else None, bias_stride if bias is not None else 0,
-            norm.weight.data_ptr(), norm.bias.data_ptr(), n, h * w, c, norm.num_groups, float(norm.eps), int(bool(silu)),
-            ws.data_ptr(), ws.numel(), out.data_ptr(), self._stream()), "tf_group_norm_nhwc"))
+        self._launch(name, work, "tf_group_norm_nhwc", x.data_ptr(), bias.data_ptr() if bias is not None else None,
+                     bias_stride if bias is not None else 0, norm.weight.data_ptr(), norm.bias.data_ptr(), n, h * w, c,
+                     norm.num_groups, float(norm.eps), int(bool(silu)), ws.data_ptr(), ws.numel(), out.data_ptr())
         return out
 
     def frames_to_nhwc(self, frames: torch.Tensor) -> torch.Tensor:
@@ -528,8 +502,8 @@ class CudaOps:
         frames = _dense(frames)
         n, h, w, _ = frames.shape
         out = torch.empty((n, 3, h, w), dtype=torch.float16, device=frames.device, memory_format=torch.channels_last)
-        self._timed("tf_frames_to_nhwc", 3.0 * n * h * w, lambda: self._check(self.lib.tf_frames_to_nhwc(
-            frames.data_ptr(), n * h * w, out.data_ptr(), self._stream()), "tf_frames_to_nhwc"))
+        self._launch("tf_frames_to_nhwc", 3.0 * n * h * w, "tf_frames_to_nhwc", frames.data_ptr(), n * h * w,
+                     out.data_ptr())
         return out
 
     def nhwc_to_frames(self, x: torch.Tensor) -> torch.Tensor:
@@ -539,8 +513,7 @@ class CudaOps:
         x = _dense(x, torch.channels_last)
         n, _, h, w = x.shape
         out = torch.empty((n, h, w, 3), dtype=torch.uint8, device=x.device)
-        self._timed("tf_nhwc_to_frames", 3.0 * n * h * w, lambda: self._check(self.lib.tf_nhwc_to_frames(
-            x.data_ptr(), n * h * w, out.data_ptr(), self._stream()), "tf_nhwc_to_frames"))
+        self._launch("tf_nhwc_to_frames", 3.0 * n * h * w, "tf_nhwc_to_frames", x.data_ptr(), n * h * w, out.data_ptr())
         return out
 
     def _resize_tables(self, n_in: int, n_out: int, device):
@@ -550,10 +523,10 @@ class CudaOps:
         if key not in cache:
             taps = int(self.lib.tf_resize_taps(n_in, n_out))
             if taps < 0:
-                self._check(1, "tf_resize_taps")
+                _check(self.lib, 1, "tf_resize_taps")
             bounds = torch.empty((n_out, 2), dtype=torch.int32)
             coeffs = torch.empty((n_out, taps), dtype=torch.int32)
-            self._check(self.lib.tf_resize_coeffs(n_in, n_out, bounds.data_ptr(), coeffs.data_ptr()), "tf_resize_coeffs")
+            _check(self.lib, self.lib.tf_resize_coeffs(n_in, n_out, bounds.data_ptr(), coeffs.data_ptr()), "tf_resize_coeffs")
             cache[key] = (bounds.to(device), coeffs.to(device), taps)
         return cache[key]
 
@@ -579,9 +552,8 @@ class CudaOps:
             assert tmp.numel() >= n * h_in * w * 3 and tmp.dtype == torch.uint8 and tmp.is_contiguous()
         work = 3.0 * n * (h_in * w_in + (2 * h_in * w if need_h and need_v else 0) + h * w)
         ptr = lambda t: t.data_ptr() if t is not None else None
-        self._timed("tf_resize_u8", work, lambda: self._check(self.lib.tf_resize_u8(
-            frames.data_ptr(), n, h_in, w_in, h, w, ptr(hb), ptr(hk), ht, ptr(vb), ptr(vk), vt, ptr(tmp), out.data_ptr(),
-            self._stream()), "tf_resize_u8"))
+        self._launch("tf_resize_u8", work, "tf_resize_u8", frames.data_ptr(), n, h_in, w_in, h, w, ptr(hb), ptr(hk), ht,
+                     ptr(vb), ptr(vk), vt, ptr(tmp), out.data_ptr())
         return out
 
     def canny(self, frames: torch.Tensor, low: float = 100, high: float = 200, edges: bool = True, cond: bool = True,
@@ -597,7 +569,7 @@ class CudaOps:
         dev = frames.device
         ws_bytes = int(self.lib.tf_canny_workspace(n, h, w))
         if ws_bytes < 0:
-            self._check(1, "tf_canny_workspace")
+            _check(self.lib, 1, "tf_canny_workspace")
         ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=dev)
         e = c = None
         if edges:
@@ -609,9 +581,8 @@ class CudaOps:
             assert c.shape == (n, 3, h, w) and c.dtype == torch.float16 and c.is_contiguous(memory_format=torch.channels_last)
         work = 3.0 * n * h * w + (n * h * w if edges else 0) + (6.0 * n * h * w if cond else 0)
         ptr = lambda t: t.data_ptr() if t is not None else None
-        self._timed("tf_canny_u8", work, lambda: self._check(self.lib.tf_canny_u8(
-            frames.data_ptr(), n, h, w, float(low), float(high), ws.data_ptr(), ws.numel(), ptr(e), ptr(c),
-            self._stream()), "tf_canny_u8"))
+        self._launch("tf_canny_u8", work, "tf_canny_u8", frames.data_ptr(), n, h, w, float(low), float(high),
+                     ws.data_ptr(), ws.numel(), ptr(e), ptr(c))
         return e, c
 
     def geglu(self, xh: torch.Tensor, gate: torch.Tensor) -> torch.Tensor:
@@ -621,8 +592,7 @@ class CudaOps:
         xh, gate = _dense(xh), _dense(gate)
         out = torch.empty_like(xh)
         n = xh.numel()
-        self._timed("tf_geglu", 3.0 * n * 2, lambda: self._check(
-            self.lib.tf_geglu(xh.data_ptr(), gate.data_ptr(), n, out.data_ptr(), self._stream()), "tf_geglu"))
+        self._launch("tf_geglu", 3.0 * n * 2, "tf_geglu", xh.data_ptr(), gate.data_ptr(), n, out.data_ptr())
         return out
 
 
@@ -679,21 +649,16 @@ class Communicator:
         self.world_size, self.rank = world_size, rank
         idbuf = (ctypes.c_uint8 * TF_COMM_ID_BYTES)()
         if rank == 0:
-            self._check(self.lib.tf_comm_unique_id(idbuf), "tf_comm_unique_id")
+            _check(self.lib, self.lib.tf_comm_unique_id(idbuf), "tf_comm_unique_id")
         t = torch.tensor(list(idbuf), dtype=torch.uint8)
         if dist.get_backend(group) == "nccl":
             t = t.cuda()
         dist.broadcast(t, src=0, group=group)
         raw = bytes(t.cpu().tolist())
         handle = ctypes.c_void_p()
-        self._check(self.lib.tf_comm_init(ctypes.create_string_buffer(raw, TF_COMM_ID_BYTES), world_size, rank,
-                                          ctypes.byref(handle)), "tf_comm_init")
+        _check(self.lib, self.lib.tf_comm_init(ctypes.create_string_buffer(raw, TF_COMM_ID_BYTES), world_size, rank,
+                                               ctypes.byref(handle)), "tf_comm_init")
         self.handle = handle
-
-    def _check(self, status, what):
-        if status != 0:
-            raise TokenflowB200Error(f"{what} failed (status {status}): "
-                                     f"{self.lib.tf_last_error().decode(errors='replace')}")
 
     def all_gather(self, t: torch.Tensor) -> torch.Tensor:
         # tf_allgather reads numel * esz bytes from the pointer: it must be device memory of this rank's GPU, dense
@@ -702,8 +667,8 @@ class Communicator:
                                      f"{t.device}")
         t = t.contiguous()
         out = torch.empty((self.world_size * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
-        self._check(self.lib.tf_allgather(self.handle, t.data_ptr(), out.data_ptr(), t.numel() * t.element_size(),
-                                          torch.cuda.current_stream().cuda_stream), "tf_allgather")
+        _check(self.lib, self.lib.tf_allgather(self.handle, t.data_ptr(), out.data_ptr(), t.numel() * t.element_size(),
+                                               torch.cuda.current_stream().cuda_stream), "tf_allgather")
         return out
 
     def destroy(self):
