@@ -28,7 +28,7 @@ from typing import Callable, Dict, Optional
 import torch
 import torch.nn as nn
 
-from .ops import all_gather
+from .ops import frame_share, gather_frames
 
 
 class TokenFlowEditor(nn.Module):
@@ -151,13 +151,16 @@ class TokenFlowEditor(nn.Module):
         return contextlib.nullcontext()
 
     def draw_keyframes(self, n: int) -> torch.Tensor:
-        """run_tokenflow_pnp.py:224 — one uniformly random frame inside every batch (CPU RNG)."""
+        """run_tokenflow_pnp.py:224 — one uniformly random frame inside every batch (CPU RNG).  A last batch of
+        r = n mod B frames gets its keyframe from one more draw, randint(r), after the full batches' draws: when B
+        divides n the draws are the reference's, and no frame is dropped when it does not (the reference truncates
+        n to a multiple of B, run_tokenflow_pnp.py:121-123)."""
         batch_size = self.config["batch_size"]
-        if self._kf_gen is None:
-            r = torch.randint(batch_size, (n // batch_size,))
-        else:
-            r = torch.randint(batch_size, (n // batch_size,), generator=self._kf_gen)
-        idx = r + torch.arange(0, n, batch_size)
+        full, rest = divmod(n, batch_size)
+        gen = {} if self._kf_gen is None else {"generator": self._kf_gen}
+        idx = torch.randint(batch_size, (full,), **gen) + torch.arange(0, full * batch_size, batch_size)
+        if rest:
+            idx = torch.cat([idx, torch.randint(rest, (1,), **gen) + full * batch_size])
         if self.world_size > 1 and self.config.get("check_keyframes", False):
             import torch.distributed as dist
             mine = idx.to(self.device if dist.get_backend(self.group) == "nccl" else "cpu")
@@ -213,7 +216,12 @@ class TokenFlowEditor(nn.Module):
             if per_pass == batch_size:                                   # the reference's schedule (:229-231)
                 denoised = []
                 for i, b in enumerate(range(0, len(x), batch_size)):
-                    h.register_batch_idx(self, i)
+                    if b + batch_size <= len(x):
+                        h.register_batch_idx(self, i)
+                    else:
+                        # a short last batch: the reference's per-batch weights would place its frames as if the
+                        # batch had len(x) - b frames (tokenflow_utils.py:375-378); the table keeps the stride B
+                        h.register_frame_table(self, *self.frame_table(list(range(b, len(x)))))
                     denoised.append(self.denoise_step(x[b:b + batch_size], t, indices[b:b + batch_size]))
                 return torch.cat(denoised)
             # same arithmetic, fewer and larger UNet passes: frames of several batches in one pass, each frame
@@ -227,7 +235,9 @@ class TokenFlowEditor(nn.Module):
 
     def frame_table(self, frames):
         """Per-frame (keyframe, previous keyframe, blend weight) for global frame ids — the reference's
-        batch_idx arithmetic (tokenflow_utils.py:331-333, :375-383) evaluated per frame."""
+        batch_idx arithmetic (tokenflow_utils.py:331-333, :375-383) evaluated per frame.  The frames of a short last
+        batch keep the nominal stride B, so frame g blends with weight blend_weights(B)[g % B]; the reference's hooks,
+        given a short batch of r frames, would compute their positions with n_frames = r (:312, :375-378)."""
         from .ops import blend_weights
         B = self.config["batch_size"]
         w = blend_weights(B)
@@ -268,54 +278,86 @@ class TokenFlowEditor(nn.Module):
         return [divmod(min(i, 3 * K - 1), K) for i in shard.slots], shard
 
     def _fused_text(self, slots, per):
+        """Text embeddings of a call over the pivotal `slots` (none for a later frame chunk) and `per` frames."""
         key = (tuple(slots), per)
         text = self._text_cache.get(key)
         if text is None:
             emb = [self.pnp_guidance_embeds[0] if s_ == 0 else self.text_embeds[s_ - 1] for s_, _ in slots]
-            text = torch.cat([torch.stack(emb), self.pnp_guidance_embeds.repeat(per, 1, 1),
-                              torch.repeat_interleave(self.text_embeds, per, dim=0)])
-            self._text_cache = {key: text}
+            text = torch.cat(([torch.stack(emb)] if emb else []) + [self.pnp_guidance_embeds.repeat(per, 1, 1),
+                             torch.repeat_interleave(self.text_embeds, per, dim=0)])
+            if len(self._text_cache) >= 3:        # a step makes at most three: pivotal + chunk 0, chunk, last chunk
+                self._text_cache = {}
+            self._text_cache[key] = text
         return text
+
+    def _rank_frames(self, N: int):
+        """Frames [lo, hi) this rank edits (`ops.frame_share`, the inversion stage's split)."""
+        G, per = self.world_size, -(-N // self.world_size)
+        if (G - 1) * per >= N:
+            raise ValueError(f"{N} frames in shares of {per} leave rank {G - 1} of {G} without frames: use fewer "
+                             "ranks or more frames")
+        return frame_share(N, G, self.rank)
+
+    def _frame_chunks(self, lo: int, hi: int):
+        """[a, b) frame ranges of the rank's UNet calls: chunks of at most config["frames_per_pass"] frames, or one."""
+        c = int(self.config.get("frames_per_pass", hi - lo))
+        if c < 1:
+            raise ValueError(f"config['frames_per_pass'] = {c}: a UNet call needs at least one frame")
+        return [(a, min(hi, a + c)) for a in range(lo, hi, c)]
 
     def _fused_compute(self, x, src_all, piv_idx, t_dev, t_int, coef, slots, shard):
         """Device work of one fused step.  Everything that varies from step to step arrives in device tensors
         (`piv_idx`: which latents are the pivotal samples, `t_dev`, `coef`: the DDIM coefficients), so the same
         function body can be captured once into a CUDA graph and replayed (run_tokenflow_pnp.py:195-233)."""
-        h, G, r = self.hooks, self.world_size, self.rank
+        h, G = self.hooks, self.world_size
         N = x.shape[0]
-        per = N // G
-        lo = r * per
-        n_piv = len(slots)
+        lo, hi = self._rank_frames(N)
+        chunks = self._frame_chunks(lo, hi)
         piv_lat = torch.cat([src_all, x]).index_select(0, piv_idx)       # slot (s, f): src[kf_f] if s == 0 else x[kf_f]
-        xs, srcs = x[lo:lo + per], src_all[lo:lo + per]
-        latent_model_input = torch.cat([piv_lat, srcs, xs, xs])
-        text = self._fused_text(slots, per)
-        res = {}
+        c_piv = None
         if self.controlnet is not None:
             # the same gather as the pivotal latents (index f or N + f: keyframe f), so a graph replay stays sync-free
             c_piv = self._ccond.index_select(0, piv_idx.remainder(N))
-            c_loc = self._ccond[lo:lo + per]
-            res = self._residuals(latent_model_input, t_dev, text, torch.cat([c_piv, c_loc, c_loc, c_loc]))
         h.register_time(self, t_int)
         h.register_pivotal(self, False)
-        h.register_shard(self, shard)
-        h.register_frame_table(self, *self.frame_table(list(range(lo, lo + per))))
-        h.register_fused(self, n_piv)
-        try:
-            noise_pred = self.unet(latent_model_input, t_dev, encoder_hidden_states=text, **res)['sample'][n_piv:]
-        finally:
-            h.register_fused(self, 0)
-            h.register_shard(self, None)
-        # classifier-free guidance + DDIM update of this rank's frames, then the all-gather of every rank's frames
-        _, npu, npc = noise_pred.chunk(3)
-        ops = self._cuda_ops()
-        if ops is not None and coef is not None and npu.dtype == torch.float16 and xs.dtype == torch.float16:
-            step = ops.cfg_ddim_v if self.scheduler.prediction_type == "v_prediction" else ops.cfg_ddim
-            x_local = step(npu, npc, xs, coef, self.config["guidance_scale"])     # one kernel, same roundings
-        else:
-            noise_pred = npu + self.config["guidance_scale"] * (npc - npu)
-            x_local = self.scheduler.step(noise_pred, t_int, xs)['prev_sample'].contiguous()
-        return all_gather(x_local, G, self.group, self.comm)
+        x_local = None if len(chunks) == 1 else x.new_empty((hi - lo,) + tuple(x.shape[1:]))
+        for j, (a, b) in enumerate(chunks):
+            # the first call also carries the pivotal samples and fills every block's keyframe caches; a later chunk is
+            # a plain frame pass over [a, b) that reads them from the modules (kf_attn_output, _tf_pivot_unit)
+            piv = (piv_lat,) if j == 0 else ()
+            n_piv = len(slots) if j == 0 else 0
+            xs, srcs = x[a:b], src_all[a:b]
+            latent_model_input = torch.cat(piv + (srcs, xs, xs))
+            text = self._fused_text(slots if j == 0 else (), b - a)
+            res = {}
+            if c_piv is not None:
+                c_loc = self._ccond[a:b]
+                res = self._residuals(latent_model_input, t_dev, text,
+                                      torch.cat(((c_piv,) if j == 0 else ()) + (c_loc, c_loc, c_loc)))
+            h.register_shard(self, shard if j == 0 else None)
+            h.register_frame_table(self, *self.frame_table(list(range(a, b))))
+            h.register_fused(self, n_piv)
+            try:
+                noise_pred = self.unet(latent_model_input, t_dev, encoder_hidden_states=text, **res)['sample'][n_piv:]
+            finally:
+                h.register_fused(self, 0)
+                h.register_shard(self, None)
+            # classifier-free guidance + DDIM update of the chunk's frames, into its slice of this rank's output
+            out = None if x_local is None else x_local[a - lo:b - lo]
+            _, npu, npc = noise_pred.chunk(3)
+            ops = self._cuda_ops()
+            if ops is not None and coef is not None and npu.dtype == torch.float16 and xs.dtype == torch.float16:
+                step = ops.cfg_ddim_v if self.scheduler.prediction_type == "v_prediction" else ops.cfg_ddim
+                y = step(npu, npc, xs, coef, self.config["guidance_scale"], out=out)    # one kernel, same roundings
+            else:
+                noise_pred = npu + self.config["guidance_scale"] * (npc - npu)
+                y = self.scheduler.step(noise_pred, t_int, xs)['prev_sample'].contiguous()
+                if out is not None:
+                    out.copy_(y)
+            if x_local is None:
+                x_local = y
+        # one all-gather of every rank's frames
+        return gather_frames(x_local, N, G, self.group, self.comm)
 
     def _cuda_ops(self):
         """The CUDA op object if the hooks run on it (None under the oracle test seam / on CPU)."""
@@ -341,8 +383,8 @@ class TokenFlowEditor(nn.Module):
     def _fused_step(self, x, t, indices):
         """One UNet call per denoising step and rank: [pivotal samples | this rank's frames x 3 streams]."""
         N, B = len(x), self.config["batch_size"]
-        K = N // B
-        assert N % self.world_size == 0, "frames must divide evenly over the ranks"
+        K = -(-N // B)                                        # a last keyframe group may be short
+        self._rank_frames(N)                                  # refuses a split that leaves a rank without frames
         t_int, t_dev = self._timestep_pair(t)
         pivotal_idx = self.draw_keyframes(N)
         kf_list = pivotal_idx.tolist()

@@ -638,6 +638,24 @@ def all_gather(t: torch.Tensor, world_size: int, group=None, comm=None) -> torch
     return out
 
 
+def frame_share(n: int, world_size: int, rank: int) -> Tuple[int, int]:
+    """Frames [lo, hi) of `rank` when n frames are dealt to `world_size` ranks in contiguous shares of ceil(n / G):
+    the split of the inversion stage and of the edit.  The last shares may be short, or empty (hi <= lo)."""
+    per = -(-n // world_size)
+    return rank * per, min(n, (rank + 1) * per)
+
+
+def gather_frames(x_local: torch.Tensor, n: int, world_size: int, group=None, comm=None) -> torch.Tensor:
+    """All n frames in order from every rank's `frame_share`: each share is padded to ceil(n / G) frames for the
+    all-gather and the padding is sliced off.  One rank returns `x_local` itself."""
+    if world_size == 1:
+        return x_local
+    pad = -(-n // world_size) - x_local.shape[0]
+    if pad:
+        x_local = torch.cat([x_local, x_local.new_zeros((pad,) + tuple(x_local.shape[1:]))])
+    return all_gather(x_local, world_size, group, comm)[:n]
+
+
 class Communicator:
     """NCCL all-gather through the C ABI (tf_comm_init / tf_allgather, include/tokenflow_b200.h): the data
     plane of the multi-GPU pivotal pass.  The 128-byte NCCL id travels over torch.distributed (control

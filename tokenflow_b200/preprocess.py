@@ -29,7 +29,7 @@ from typing import Dict, Iterable, List, Optional, Tuple
 
 import torch
 
-from .ops import all_gather
+from .ops import all_gather, frame_share, gather_frames
 
 
 def inversion_coef_tables(scheduler) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -124,18 +124,10 @@ class LatentInverter:
         return out["sample"] if isinstance(out, dict) else out.sample
 
     def _local(self, n: int):
-        per = -(-n // self.world_size)
-        return self.rank * per, min(n, (self.rank + 1) * per)
+        return frame_share(n, self.world_size, self.rank)
 
     def _gathered(self, x_local, n: int):
-        """All N frames from every rank's share (the last shares may be short: padded to equal size)."""
-        if self.world_size == 1:
-            return x_local
-        per = -(-n // self.world_size)
-        pad = per - x_local.shape[0]
-        if pad:
-            x_local = torch.cat([x_local, x_local.new_zeros((pad,) + tuple(x_local.shape[1:]))])
-        return all_gather(x_local, self.world_size, self.group, self.comm)[:n]
+        return gather_frames(x_local, n, self.world_size, self.group, self.comm)
 
     @torch.no_grad()
     def ddim_inversion(self, cond: torch.Tensor, latent_frames: torch.Tensor, save_path: Optional[str], batch_size: int,
