@@ -216,7 +216,9 @@ int tf_nhwc_to_frames(const void* x_f16, int64_t n_px, void* frames_u8, tf_strea
  * reference's frame resize (util.py:28 to (W, H); run_tokenflow_pnp.py:174-175, run_tokenflow_sdedit.py:136-137,
  * preprocess.py:191-192 square frames to 512x512).  Per axis, Lanczos-3 weights in double, normalised and rounded to
  * int32 with 22 fractional bits; a horizontal pass into a uint8 intermediate, then a vertical pass, each value
- * clamp((2^21 + sum v * k) >> 22, 0, 255).  A pass whose axis keeps its size is skipped; equal sizes are a copy.
+ * clamp((2^21 + sum v * k) >> 22, 0, 255).  A frame more than 100 times taller than wide (h_in > 100 * w_in) whose
+ * height shrinks goes through the vertical pass first, as Pillow 12 takes it.  A pass whose axis keeps its size is
+ * skipped; equal sizes are a copy.
  * Sizes are in [1, 65536].
  *
  * tf_resize_taps      taps per output pixel of the table for one axis `in` -> `out` (-1 for bad sizes)
@@ -227,7 +229,12 @@ int tf_nhwc_to_frames(const void* x_f16, int64_t n_px, void* frames_u8, tf_strea
  *   h_bounds, h_coeffs, h_taps   device copies of the tables for w_in -> w (unused, may be NULL, when w == w_in)
  *   v_bounds, v_coeffs, v_taps   the same for h_in -> h (unused when h == h_in)
  *   tmp                          device [n, h_in, w, 3] uint8 intermediate, used only when both axes change
- * The device tables are trusted: they must be what tf_resize_coeffs wrote for the same sizes. */
+ *                                ([n, h, w_in, 3] when the vertical pass goes first)
+ * The device tables are trusted: they must be what tf_resize_coeffs wrote for the same sizes.  Each pass is one launch
+ * of at most 2^31 - 1 blocks: the horizontal pass takes n*h_in / rows blocks (n*h / rows when it goes second; rows = 4
+ * up to w_in = 4090, 3, 2, then 1 from w_in = 8187), the vertical one n*h*ceil(3w / 2048) (w_in for w when it goes
+ * first; ceil(3w / 512) unless w % 16 == 0 and its input and output are 16-byte aligned); a call past either is
+ * refused (TF_ERR_UNSUPPORTED) before anything is enqueued. */
 int tf_resize_taps(int in, int out);
 int tf_resize_coeffs(int in, int out, int32_t* bounds, int32_t* coeffs);
 int tf_resize_u8(const void* in, int64_t n, int h_in, int w_in, int h, int w, const int32_t* h_bounds,

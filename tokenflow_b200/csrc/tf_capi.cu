@@ -318,6 +318,37 @@ int tf_resize_u8(const void* in, int64_t n, int h_in, int w_in, int h, int w, co
     set_last_error("tf_resize_u8: vertical table of %d taps, %d -> %d has %d", v_taps, h_in, h, resize_taps(h_in, h));
     return TF_ERR_INVALID_ARGUMENT;
   }
+  // Pillow's Image.resize takes a frame more than 100 times taller than wide through the vertical pass first when its
+  // height shrinks (a vertical-only resize to (w_in, h), then a horizontal-only one); every other frame goes through
+  // the horizontal pass first.  The two orders round the intermediate differently.
+  const bool v_first = need_h && need_v && h_in > 100LL * w_in && h < h_in;
+  const long long h_rows = v_first ? h : h_in;           // input rows per frame of the horizontal pass
+  const int v_w = v_first ? w_in : w;                    // row width of the vertical pass
+  const void* v_in = need_h && !v_first ? tmp : in;
+  void* v_out = v_first ? tmp : out;
+  // Both passes' grids (at most 2^31 - 1 blocks) are checked before the first launch, so that a refused call enqueues
+  // nothing.  The horizontal pass runs one block per `rows` input rows, the vertical pass one per output row and
+  // column block of 128 threads of 16 bytes (4 unless the row pitch and both pointers are 16-byte aligned):
+  // launch_resize_h / launch_resize_v.  Written as divisions, so that no product overflows.
+  constexpr long long kMaxBlocks = 0x7fffffffLL;
+  if (need_h) {
+    const long long rows = std::min(std::max(48LL * 1024 / (3LL * w_in + 16), 1LL), 4LL);
+    if (n > kMaxBlocks * rows / h_rows) {
+      set_last_error("tf_resize_u8: %lld frames of %lld rows of %d pixels are too many for one horizontal launch",
+                     (long long)n, h_rows, w_in);
+      return TF_ERR_UNSUPPORTED;
+    }
+  }
+  if (need_v) {
+    const uintptr_t src = reinterpret_cast<uintptr_t>(v_in), dst = reinterpret_cast<uintptr_t>(v_out);
+    const long long per = (3LL * v_w) % 16 == 0 && (src & 15u) == 0 && (dst & 15u) == 0 ? 16 : 4;
+    const long long col_blocks = (3LL * v_w + 128 * per - 1) / (128 * per);
+    if (n > kMaxBlocks / (h * col_blocks)) {
+      set_last_error("tf_resize_u8: %lld frames of %d rows of %d pixels are too many for one vertical launch",
+                     (long long)n, h, v_w);
+      return TF_ERR_UNSUPPORTED;
+    }
+  }
   if (n == 0) return TF_OK;
   if (!in || !out || (need_h && (!h_bounds || !h_coeffs)) || (need_v && (!v_bounds || !v_coeffs)) ||
       (need_h && need_v && !tmp)) {
@@ -327,10 +358,14 @@ int tf_resize_u8(const void* in, int64_t n, int h_in, int w_in, int h, int w, co
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!need_h && !need_v)          // Pillow returns a copy when the size is unchanged
     return check_cuda(cudaMemcpyAsync(out, in, (size_t)n * h * w * 3, cudaMemcpyDeviceToDevice, st), "tf_resize_u8 copy");
+  if (v_first) {
+    if (int e = launched(launch_resize_v(in, n, h_in, h, w_in, v_bounds, v_coeffs, v_taps, tmp, st))) return e;
+    return launched(launch_resize_h(tmp, n * h, w_in, w, h_bounds, h_coeffs, h_taps, out, st));
+  }
   if (need_h)
     if (int e = launched(launch_resize_h(in, n * h_in, w_in, w, h_bounds, h_coeffs, h_taps, need_v ? tmp : out, st)))
       return e;
-  if (need_v) return launched(launch_resize_v(need_h ? tmp : in, n, h_in, h, w, v_bounds, v_coeffs, v_taps, out, st));
+  if (need_v) return launched(launch_resize_v(v_in, n, h_in, h, w, v_bounds, v_coeffs, v_taps, out, st));
   return TF_OK;
 }
 

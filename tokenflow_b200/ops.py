@@ -9,6 +9,7 @@ raises, loudly.  (Tests substitute an oracle-backed op object through
 from __future__ import annotations
 
 import ctypes
+import math
 from pathlib import Path
 from typing import Optional, Sequence, Tuple
 
@@ -533,8 +534,10 @@ class CudaOps:
     def resize_frames(self, frames: torch.Tensor, size: Tuple[int, int], tmp: Optional[torch.Tensor] = None,
                       out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """uint8 RGB frames [N, H_in, W_in, 3] (CUDA) -> [N, H, W, 3] for size = (H, W), bit-equal to PIL's
-        `Image.resize((W, H), Image.LANCZOS)` of every frame.  `tmp` ([N, H_in, W, 3] uint8) and `out` may be given;
-        they are made here otherwise.  Every buffer may start at any element offset (the kernels read and write bytes)."""
+        `Image.resize((W, H), Image.LANCZOS)` of every frame.  `tmp` ([N, H_in, W, 3] uint8, or [N, H, W_in, 3] for a
+        frame more than 100 times taller than wide whose height shrinks: Pillow resizes those vertically first) and
+        `out` may be given; they are made here otherwise.  Every buffer may start at any element offset (the kernels
+        read and write bytes)."""
         assert frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[-1] == 3 and frames.is_cuda
         frames = frames.contiguous()
         n, h_in, w_in, _ = frames.shape
@@ -546,11 +549,13 @@ class CudaOps:
         if out is None:
             out = torch.empty((n, h, w, 3), dtype=torch.uint8, device=dev)
         assert out.shape == (n, h, w, 3) and out.dtype == torch.uint8 and out.is_contiguous()
+        v_first = need_h and need_v and h_in > 100 * w_in and h < h_in
+        tmp_shape = (n, h, w_in, 3) if v_first else (n, h_in, w, 3)
         if need_h and need_v and tmp is None:
-            tmp = torch.empty((n, h_in, w, 3), dtype=torch.uint8, device=dev)
+            tmp = torch.empty(tmp_shape, dtype=torch.uint8, device=dev)
         if tmp is not None:
-            assert tmp.numel() >= n * h_in * w * 3 and tmp.dtype == torch.uint8 and tmp.is_contiguous()
-        work = 3.0 * n * (h_in * w_in + (2 * h_in * w if need_h and need_v else 0) + h * w)
+            assert tmp.numel() >= math.prod(tmp_shape) and tmp.dtype == torch.uint8 and tmp.is_contiguous()
+        work = 3.0 * n * (h_in * w_in + (2 * math.prod(tmp_shape[1:3]) if need_h and need_v else 0) + h * w)
         ptr = lambda t: t.data_ptr() if t is not None else None
         self._launch("tf_resize_u8", work, "tf_resize_u8", frames.data_ptr(), n, h_in, w_in, h, w, ptr(hb), ptr(hk), ht,
                      ptr(vb), ptr(vk), vt, ptr(tmp), out.data_ptr())
