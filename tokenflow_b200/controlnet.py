@@ -109,6 +109,20 @@ class ControlNetModel(nn.Module):
         return self
 
     @classmethod
+    def from_config(cls, config: dict) -> "ControlNetModel":
+        """The ControlNet a diffusers ControlNet `config.json` describes (its dict).  The UNet-encoder keys are read and
+        refused as `sd_unet.encoder_fields` does; conditioning_channels and conditioning_embedding_out_channels are
+        read; a channel order other than rgb and global pooling of the conditions are refused (ValueError naming the
+        key and the value).  A missing key takes diffusers' default."""
+        from .sd_unet import check_fixed, encoder_fields
+        check_fixed("controlnet", config, {"controlnet_conditioning_channel_order": "rgb",
+                                           "global_pool_conditions": False})
+        unet = UNetConfig(**encoder_fields(config, "controlnet"))
+        emb = tuple(int(c) for c in config.get("conditioning_embedding_out_channels", (16, 32, 96, 256)))
+        return cls(ControlNetConfig(unet, conditioning_channels=int(config.get("conditioning_channels", 3)),
+                                    conditioning_embedding_out_channels=emb))
+
+    @classmethod
     def from_unet(cls, unet: UNet2DConditionModel, cfg: Optional[ControlNetConfig] = None) -> "ControlNetModel":
         """diffusers' `ControlNetModel.from_unet`: conv_in, time_embedding, down_blocks and mid_block copied from
         `unet`, the zero convolutions zero, the rest of the conditioning embedding freshly initialised."""

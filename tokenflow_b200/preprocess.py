@@ -100,7 +100,7 @@ class LatentInverter:
         self.comm = comm
 
     def saved_latents(self) -> Dict[int, torch.Tensor]:
-        """{t: [N, 4, h, w]} of the last `ddim_inversion` on the CUDA fp16 path — the tensors it writes as
+        """{t: [N, 4, h, w]} of the last `ddim_inversion` (either path, with `save_latents`) — the tensors it writes as
         `noisy_latents_<t>.pt`, kept in memory so that `TokenFlowEditor(..., source_latents=
         inv.saved_latents().__getitem__)` needs no disk round trip."""
         return self._saved
@@ -144,14 +144,15 @@ class LatentInverter:
         x = latent_frames[lo:hi].clone()
         if save_latents and save_path is not None:
             os.makedirs(os.path.join(save_path, "latents"), exist_ok=True)
+        self._saved = {}
         for i, t in enumerate(ts):
             mu, sigma, mu_prev, sigma_prev = self._alphas(t, ts[i - 1] if i > 0 else None)
             for b in range(0, x.shape[0], batch_size):
                 xb = x[b:b + batch_size]
                 x[b:b + batch_size] = self._update(xb, self._eps(xb, t, cond, lo + b), mu_prev, sigma_prev, mu, sigma)
-            if save_latents and save_path is not None and (t in keep or i == len(ts) - 1):
-                full = self._gathered(x, n)
-                if self.rank == 0:
+            if save_latents and (t in keep or i == len(ts) - 1):
+                full = self._saved[t] = self._gathered(x, n).clone()
+                if save_path is not None and self.rank == 0:
                     torch.save(full, os.path.join(save_path, "latents", f"noisy_latents_{t}.pt"))
         return self._gathered(x, n)
 

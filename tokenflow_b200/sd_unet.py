@@ -43,7 +43,73 @@ class UNetConfig:
     num_heads: Tuple[int, ...] = (8, 8, 8, 8)
     norm_num_groups: int = 32
     use_linear_projection: bool = False
-    sample_size: int = 64
+    sample_size: Optional[int] = 64
+
+
+# diffusers UNet2DConditionModel / ControlNetModel config keys.  `from_config` reads the keys that set the topology
+# (`encoder_fields`); each key below must hold the one value computed here, which is also diffusers' default, so a
+# missing key passes.  Every other key (_class_name, _diffusers_version, upcast_attention, ...) changes nothing.
+_ENCODER_FIXED = {
+    "in_channels": 4, "mid_block_type": "UNetMidBlock2DCrossAttn", "only_cross_attention": False,
+    "dual_cross_attention": False, "class_embed_type": None, "num_class_embeds": None, "addition_embed_type": None,
+    "addition_time_embed_dim": None, "projection_class_embeddings_input_dim": None, "encoder_hid_dim": None,
+    "encoder_hid_dim_type": None, "time_cond_proj_dim": None, "flip_sin_to_cos": True, "freq_shift": 0,
+    "act_fn": "silu", "norm_eps": 1e-5, "downsample_padding": 1, "mid_block_scale_factor": 1,
+    "resnet_time_scale_shift": "default", "attention_type": "default",
+}
+_UNET_FIXED = {
+    "out_channels": 4, "center_input_sample": False, "resnet_skip_time_act": False, "resnet_out_scale_factor": 1.0,
+    "time_embedding_type": "positional", "time_embedding_dim": None, "time_embedding_act_fn": None,
+    "timestep_post_act": None, "conv_in_kernel": 3, "conv_out_kernel": 3, "class_embeddings_concat": False,
+    "mid_block_only_cross_attention": None, "cross_attention_norm": None, "reverse_transformer_layers_per_block": None,
+    "dropout": 0.0,
+}
+
+
+def check_fixed(what: str, config: dict, fixed: dict) -> None:
+    """ValueError naming the key and the value for the first key of `config` that does not hold `fixed[key]`."""
+    for key, value in fixed.items():
+        got = config.get(key, value)
+        if got != value:
+            raise ValueError(f"{what} config {key}={got!r} is not supported (only {value!r})")
+
+
+def check_block_types(what: str, config: dict, key: str, want) -> None:
+    got = list(config.get(key, want))
+    if got != list(want):
+        raise ValueError(f"{what} config {key}={got!r} is not supported (only {list(want)!r})")
+
+
+def encoder_fields(config: dict, what: str) -> dict:
+    """The UNetConfig fields of a diffusers UNet or ControlNet config dict, after refusing the settings the blocks
+    here do not compute: an input other than 4 latent channels (depth: 5, inpainting: 9), SDXL's extra embeddings and
+    several transformer layers per block, class or timestep-condition embeddings, a mid block other than the
+    cross-attention one, block types outside SD's arrangement, and the other keys of `_ENCODER_FIXED`.
+
+    diffusers' naming quirk: without `num_attention_heads`, `attention_head_dim` holds the number of heads per level
+    (SD1.5: 8, SD2.x: [5, 10, 20, 20]), which is how diffusers itself reads it."""
+    check_fixed(what, config, _ENCODER_FIXED)
+    layers = config.get("transformer_layers_per_block", 1)
+    if any(v != 1 for v in (layers if isinstance(layers, (list, tuple)) else [layers])):
+        raise ValueError(f"{what} config transformer_layers_per_block={layers!r} is not supported (only 1)")
+    ch = tuple(int(c) for c in config.get("block_out_channels", (320, 640, 1280, 1280)))
+    n = len(ch)
+    check_block_types(what, config, "down_block_types", ["CrossAttnDownBlock2D"] * (n - 1) + ["DownBlock2D"])
+    per_block = config.get("layers_per_block", 2)
+    if not isinstance(per_block, int):
+        raise ValueError(f"{what} config layers_per_block={per_block!r} is not supported (only one int)")
+    ctx = config.get("cross_attention_dim", 1280)
+    if isinstance(ctx, (list, tuple)):
+        if len(set(ctx)) != 1:
+            raise ValueError(f"{what} config cross_attention_dim={ctx!r} is not supported (only one width)")
+        ctx = ctx[0]
+    heads = config.get("num_attention_heads") or config.get("attention_head_dim", 8)
+    heads = tuple(int(h) for h in heads) if isinstance(heads, (list, tuple)) else (int(heads),) * n
+    if len(heads) != n:
+        raise ValueError(f"{what} config has {len(heads)} head counts for {n} blocks")
+    return dict(block_out_channels=ch, layers_per_block=per_block, cross_attention_dim=int(ctx), num_heads=heads,
+                norm_num_groups=int(config.get("norm_num_groups", 32)),
+                use_linear_projection=bool(config.get("use_linear_projection", False)))
 
 
 def sd15_config() -> UNetConfig:
@@ -444,6 +510,18 @@ class UNet2DConditionModel(nn.Module):
         self.conv_norm_out = GroupNorm(g, ch[0], eps=1e-5)
         self.conv_act = nn.SiLU()
         self.conv_out = nn.Conv2d(ch[0], cfg.out_channels, 3, padding=1)
+
+    @classmethod
+    def from_config(cls, config: dict) -> "UNet2DConditionModel":
+        """The UNet a diffusers `unet/config.json` describes (its dict), built with this module's default init.
+        Raises ValueError, naming the key and the value, on any setting it does not compute (`encoder_fields`, the
+        up blocks, and the UNet-only keys of `_UNET_FIXED`); a missing key takes diffusers' default.
+        `upcast_attention` is accepted and changes nothing (DESIGN.md §1 f-6)."""
+        check_fixed("unet", config, _UNET_FIXED)
+        fields = encoder_fields(config, "unet")
+        n = len(fields["block_out_channels"])
+        check_block_types("unet", config, "up_block_types", ["UpBlock2D"] + ["CrossAttnUpBlock2D"] * (n - 1))
+        return cls(UNetConfig(**fields, sample_size=config.get("sample_size")))
 
     def forward(self, sample, timestep, encoder_hidden_states=None, down_block_additional_residuals=None,
                 mid_block_additional_residual=None, return_dict: bool = True, **_):

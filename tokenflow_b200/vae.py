@@ -30,6 +30,12 @@ from .sd_unet import norm_act
 
 SCALING_FACTOR = 0.18215           # SD's latent scale (reference run_tokenflow_pnp.py:151, :157)
 
+# diffusers AutoencoderKL config keys that must hold the one value computed here (RGB frames, 4 latent channels, SD's
+# latent scale and no shift, both 1x1 quant convolutions, the mid-block attention); each is diffusers' default
+_VAE_FIXED = {"in_channels": 3, "out_channels": 3, "latent_channels": 4, "act_fn": "silu",
+              "scaling_factor": SCALING_FACTOR, "shift_factor": None, "latents_mean": None, "latents_std": None,
+              "use_quant_conv": True, "use_post_quant_conv": True, "mid_block_add_attention": True}
+
 
 @dataclass
 class VAEConfig:
@@ -221,6 +227,21 @@ class AutoencoderKL(nn.Module):
         self.decoder = Decoder(cfg)
         self.quant_conv = nn.Conv2d(2 * cfg.latent_channels, 2 * cfg.latent_channels, 1)
         self.post_quant_conv = nn.Conv2d(cfg.latent_channels, cfg.latent_channels, 1)
+
+    @classmethod
+    def from_config(cls, config: dict) -> "AutoencoderKL":
+        """The VAE a diffusers `vae/config.json` describes (its dict).  Reads block_out_channels, layers_per_block and
+        norm_num_groups; raises ValueError, naming the key and the value, on anything else this restatement and the
+        frame conversions around it do not compute (`_VAE_FIXED`, block types other than DownEncoderBlock2D /
+        UpDecoderBlock2D).  A missing key takes diffusers' default; other keys (sample_size, force_upcast, ...) change
+        nothing."""
+        from .sd_unet import check_block_types, check_fixed
+        check_fixed("vae", config, _VAE_FIXED)
+        ch = tuple(int(c) for c in config.get("block_out_channels", (64,)))
+        check_block_types("vae", config, "down_block_types", ["DownEncoderBlock2D"] * len(ch))
+        check_block_types("vae", config, "up_block_types", ["UpDecoderBlock2D"] * len(ch))
+        return cls(VAEConfig(block_out_channels=ch, layers_per_block=int(config.get("layers_per_block", 1)),
+                             norm_num_groups=int(config.get("norm_num_groups", 32))))
 
     def encode(self, x: torch.Tensor) -> EncoderOutput:
         """x [N, 3, H, W] in [-1, 1] -> posterior over [N, 4, H/8, W/8] (unscaled)."""

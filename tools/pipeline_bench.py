@@ -1,0 +1,145 @@
+"""Where the time of one whole edit goes: a synthetic SD1.5 checkpoint on disk, 40 frames in, edited frames out, through
+`pipeline.load_parts`, `pipeline.preprocess` and `pipeline.edit`, on one GPU.
+
+    python tools/pipeline_bench.py [--frames 40] [--size 512] [--batch 8] [--edit-steps 50] [--inversion-steps 500]
+                                   [--inversion-batch 40] [--out FILE]
+
+The defaults are one C2-sized run: 40 frames at 512², B = 8, 50-step PnP, 500 inversion (+ 500 reconstruction) steps
+saving the 50 sampling timesteps.  The checkpoint (`synthetic_checkpoint.write_checkpoint`: random-init SD1.5 UNet and
+VAE in fp16 safetensors under SD1.5's published configs and file names, a random text encoder of CLIP ViT-L/14's size,
+SD1.5's scheduler config) is written to a temporary directory and removed afterwards; the frames are random smooth uint8
+frames on the host, as if read from disk.
+
+Each stage function the pipeline calls is wrapped with a device synchronise and a host clock before and after, so the
+stages are timed inside the pipeline's own control flow: checkpoint load, text encoding, resize + encode (both stages),
+Canny (none here), inversion, reconstruction, edit (the denoising loop), decode (the reconstruction and the edit).  It
+prints each stage's seconds and share of the wall time, the end-to-end frames/s (frames over the wall time of load +
+preprocess + edit), and the card's name, power limit and SM clock read by nvidia-smi before and after the run.  One run:
+the stages are long (seconds to minutes), not a microbenchmark.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import shutil
+import subprocess
+import sys
+import tempfile
+import time
+from contextlib import ExitStack
+from unittest import mock
+
+REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, REPO)
+
+
+def card():
+    q = "name,power.limit,clocks.sm,clocks.max.sm,temperature.gpu"
+    try:
+        out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader", "-i", "0"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError) as e:
+        out = f"nvidia-smi unavailable: {e}"
+    return dict(zip(q.split(","), [v.strip() for v in out.split(",")])) if "," in out else {"raw": out}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--frames", type=int, default=40)
+    ap.add_argument("--size", type=int, default=512)
+    ap.add_argument("--batch", type=int, default=8)
+    ap.add_argument("--edit-steps", type=int, default=50)
+    ap.add_argument("--inversion-steps", type=int, default=500)
+    ap.add_argument("--inversion-batch", type=int, default=40)
+    ap.add_argument("--out", default=None)
+    args = ap.parse_args()
+
+    import torch
+    from tokenflow_b200 import checkpoint, pipeline
+    from tokenflow_b200 import synthetic_checkpoint as synthetic
+    from tokenflow_b200.editor import TokenFlowEditor
+    from tokenflow_b200.preprocess import LatentInverter
+
+    assert torch.cuda.is_available(), "pipeline_bench.py needs a GPU"
+    torch.cuda.set_device(0)
+    times = {}
+
+    def timed(stage, fn):
+        def run(*a, **k):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            out = fn(*a, **k)
+            torch.cuda.synchronize()
+            times[stage] = times.get(stage, 0.0) + time.perf_counter() - t0
+            return out
+        return run
+
+    root = tempfile.mkdtemp(prefix="tf_b200_pipeline_bench_")
+    try:
+        model_dir, _ = synthetic.write_checkpoint(root, "sd15", dtype=torch.float16, init_device="cuda",
+                                                  deprecated_vae=True, text_config=synthetic.CLIP_L)
+        torch.cuda.empty_cache()
+        g = torch.Generator().manual_seed(0)
+        small = torch.rand(args.frames, 3, args.size // 16, args.size // 16, generator=g)
+        frames = (torch.nn.functional.interpolate(small, size=(args.size, args.size), mode="bilinear") * 255).round()
+        frames = frames.to(torch.uint8).permute(0, 2, 3, 1).contiguous()
+        opt = {"H": args.size, "W": args.size, "steps": args.inversion_steps, "batch_size": args.inversion_batch,
+               "save_steps": args.edit_steps, "inversion_prompt": "a woman running"}
+        config = {"prompt": "a marble sculpture of a woman running, Venus de Milo",
+                  "negative_prompt": "ugly, blurry, low res, unrealistic, unaesthetic", "guidance_scale": 7.5,
+                  "n_timesteps": args.edit_steps, "batch_size": args.batch, "pnp_attn_t": 0.5, "pnp_f_t": 0.8,
+                  "seed": 1, "inversion_prompt": opt["inversion_prompt"]}
+        card_before = card()
+        with ExitStack() as stack:
+            for name, stage in (("resize_frames", "resize+encode"), ("encode_imgs", "resize+encode"),
+                                ("canny_cond", "canny"), ("decode_latents", "decode")):
+                stack.enter_context(mock.patch.object(pipeline, name, timed(stage, getattr(pipeline, name))))
+            stack.enter_context(mock.patch.object(checkpoint, "text_embeds", timed("text", checkpoint.text_embeds)))
+            stack.enter_context(mock.patch.object(LatentInverter, "ddim_inversion",
+                                                  timed("inversion", LatentInverter.ddim_inversion)))
+            stack.enter_context(mock.patch.object(LatentInverter, "ddim_sample",
+                                                  timed("reconstruction", LatentInverter.ddim_sample)))
+            stack.enter_context(mock.patch.object(TokenFlowEditor, "sample_loop",
+                                                  timed("edit", TokenFlowEditor.sample_loop)))
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            parts = timed("load", pipeline.load_parts)(model_dir, "cuda", torch.float16)
+            t1 = time.perf_counter()
+            saved, recon = pipeline.preprocess(parts, frames, opt)
+            torch.cuda.synchronize()
+            t2 = time.perf_counter()
+            torch.manual_seed(1)
+            out = pipeline.edit(parts, frames, config, saved)
+            torch.cuda.synchronize()
+            t3 = time.perf_counter()
+        wall = t3 - t0
+        times["other"] = wall - sum(times.values())
+        result = {
+            "card_before": card_before, "card_after": card(),
+            "run": {"frames": args.frames, "size": args.size, "B": args.batch, "edit_steps": args.edit_steps,
+                    "inversion_steps": args.inversion_steps, "inversion_batch": args.inversion_batch, "mode": "pnp"},
+            "stage_s": {k: round(v, 3) for k, v in times.items()},
+            "stage_share": {k: round(v / wall, 4) for k, v in times.items()},
+            "wall_s": {"total": round(wall, 3), "load": round(t1 - t0, 3), "preprocess": round(t2 - t1, 3),
+                       "edit": round(t3 - t2, 3)},
+            "e2e_frames_per_s": round(args.frames / wall, 4),
+            "edit_stage_frames_per_s": round(args.frames / (t3 - t2), 4),
+            "edit_ms_per_step": round(1e3 * times["edit"] / args.edit_steps, 1),
+            "inversion_ms_per_step": round(1e3 * times["inversion"] / args.inversion_steps, 1),
+            "peak_allocated_gb": round(torch.cuda.max_memory_allocated() / 2 ** 30, 2),
+            "outputs": {"recon": list(recon.shape), "edit": list(out.shape),
+                        "edit_finite_std": float(out.float().std())},
+        }
+    finally:
+        shutil.rmtree(root, ignore_errors=True)
+    text = json.dumps(result, indent=1)
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        with open(args.out, "w") as f:
+            f.write(text)
+    print(text)
+
+
+if __name__ == "__main__":
+    main()
