@@ -105,11 +105,18 @@ def preprocess(parts: Parts, frames_u8: torch.Tensor, opt, world_size: int = 1, 
     return inv.saved_latents(), decode_latents(parts.vae, reconstruction)
 
 
+def edit_mode(config: Dict) -> str:
+    """The editing method of a config: its `mode`, else "pnp" when it has pnp_attn_t, else "sdedit"."""
+    return config.get("mode", "pnp" if "pnp_attn_t" in config else "sdedit")
+
+
 @torch.no_grad()
 def edit(parts: Parts, frames_u8: torch.Tensor, config: Dict, source_latents: Dict[int, torch.Tensor],
-         world_size: int = 1, rank: int = 0, group=None, comm=None) -> torch.Tensor:
+         world_size: int = 1, rank: int = 0, group=None, comm=None, vae_recon: bool = False):
     """uint8 frames [N, H_in, W_in, 3] and the inverted latents of their preprocess ({t: [>= N, 4, h, w]}) -> the
-    edited uint8 frames [N, 8h, 8w, 3].
+    edited uint8 frames [N, 8h, 8w, 3]; with `vae_recon`, (edited frames, the VAE reconstruction of the source
+    frames [N, 8h, 8w, 3]), which is `decode_latents` of the latents the edit starts from (the reference's
+    `save_vae_recon`, run_tokenflow_pnp.py:242-246).
 
     `config` has the keys of the reference's configs/config_pnp.yaml or config_sdedit.yaml (prompt, negative_prompt,
     guidance_scale, n_timesteps, batch_size, pnp_attn_t, pnp_f_t / start, use_ddim_noise), `inversion_prompt` (the
@@ -133,7 +140,7 @@ def edit(parts: Parts, frames_u8: torch.Tensor, config: Dict, source_latents: Di
     latents = encode_imgs(parts.vae, frames)
     edges = canny_cond(frames) if parts.controlnet is not None else None
     cfg = dict(config)
-    cfg.setdefault("mode", "pnp" if "pnp_attn_t" in cfg else "sdedit")
+    cfg["mode"] = edit_mode(cfg)
     cfg.setdefault("fused_pass", True)
     cfg.setdefault("cuda_graph", device.type == "cuda")
     tok, enc = parts.tokenizer, parts.text_encoder
@@ -150,4 +157,5 @@ def edit(parts: Parts, frames_u8: torch.Tensor, config: Dict, source_latents: Di
         eps = torch.randn_like(eps[[0]]).repeat(n, 1, 1, 1)
     x = editor.scheduler.add_noise(latents, eps, editor.scheduler.timesteps[0])
     editor.init_method()
-    return decode_latents(parts.vae, editor.sample_loop(x))
+    edited = decode_latents(parts.vae, editor.sample_loop(x))
+    return (edited, decode_latents(parts.vae, latents)) if vae_recon else edited

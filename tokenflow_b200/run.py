@@ -1,22 +1,33 @@
-"""Command line of the two stages: a diffusers checkpoint directory, a frame directory and a config in, the reference's
-latents directory and edited frames out.
+"""Command line of the two stages: a diffusers checkpoint directory, a video file or frame directory and a config in,
+the reference's latents directory, edited frames and videos out.
 
-    python -m tokenflow_b200.run preprocess --model_dir DIR --data_path FRAMES [--H 512 --W 512 --save_dir latents
-        --sd_version 2.1 --steps 500 --batch_size 40 --save_steps 50 --n_frames 40 --inversion_prompt "..."]
+    python -m tokenflow_b200.run preprocess --model_dir DIR --data_path VIDEO_OR_FRAMES [--H 512 --W 512
+        --save_dir latents --sd_version 2.1 --steps 500 --batch_size 40 --save_steps 50 --n_frames 40
+        --inversion_prompt "..."]
     python -m tokenflow_b200.run edit --config_path configs/config_pnp.yaml --model_dir DIR [--controlnet_dir DIR]
 
-`preprocess` takes the reference's flags (preprocess.py:336-349) and writes its latents directory
-(<save_dir>/sd_<ver>/<name>/steps_<n>/nframes_<n>/latents/noisy_latents_<t>.pt, inversion_prompt.txt, frames/ with the
-reconstruction) and <save_dir>/inversion_prompts.yaml.  `edit` takes the reference's YAML config (config_pnp.yaml or
-config_sdedit.yaml; PnP when it has pnp_attn_t), finds the latents directory the way run_tokenflow_pnp.py does, and
-writes the edited frames as <output_path>/img_ode/%05d.png, and the config as <output_path>/config.yaml.  The config's
-sd_version, data_path, latents_path and n_inversion_steps must name the directory preprocess wrote.  It edits
-min(n_frames, the latents' frame count) frames; unlike the reference's driver it does not trim that count to a
-multiple of batch_size, since the editor takes a short last keyframe group (INTEGRATION.md §6).
+`preprocess` takes the reference's flags (preprocess.py:336-349).  A `--data_path` that is a file is a video: as
+preprocess.py:351-354 does, every frame is decoded (`video.read_video`, OpenCV's FFmpeg) and resized to --W x --H,
+rank 0 writes them to data/<stem>/%05d.png under the working directory, and the first `n_frames` of them are
+preprocessed as if `--data_path data/<stem>` had been given; a video shorter than `n_frames` is refused before any
+model loads.  Every torchrun rank decodes and resizes the video itself: the resize is integer arithmetic, so the
+ranks hold the same frames.  A directory is read as %05d.png, else %05d.jpg (util.load_imgs), with PIL.  `preprocess`
+writes the reference's latents directory (<save_dir>/sd_<ver>/<name>/steps_<n>/nframes_<n>/latents/
+noisy_latents_<t>.pt, inversion_prompt.txt, frames/ and inverted.mp4 at 10 fps with the reconstruction) and
+<save_dir>/inversion_prompts.yaml.
 
-Frames are read from `data_path` as %05d.png, else %05d.jpg (util.load_imgs), with PIL; video containers are out of
-scope.  `--controlnet_dir` adds a Canny ControlNet to both stages.  Under torchrun every process edits on its local
-GPU (`LOCAL_RANK`): frames are sharded over the ranks and the all-gathers run through `ops.Communicator`; rank 0 writes
+`edit` takes the reference's YAML config (config_pnp.yaml or config_sdedit.yaml; PnP when it has pnp_attn_t), finds
+the latents directory the way run_tokenflow_pnp.py does, and writes under <output_path>: the edited frames as
+img_ode/%05d.png, tokenflow_PnP_fps_{10,20,30}.mp4 or tokenflow_SDEdit_fps_{10,20,30}.mp4 of them, config.yaml,
+and for PnP the VAE reconstruction of the source frames as vae_recon/%05d.png and vae_recon_{10,20,30}.mp4
+(run_tokenflow_pnp.py:242-261, run_tokenflow_sdedit.py:201-203).  The mp4 files are MPEG-4 Part 2 (`mp4v`,
+`util.save_video`), not the reference's H.264.  The config's sd_version, data_path, latents_path and
+n_inversion_steps must name the directory preprocess wrote.  It edits min(n_frames, the latents' frame count)
+frames; unlike the reference's driver it does not trim that count to a multiple of batch_size, since the editor
+takes a short last keyframe group (INTEGRATION.md §6).
+
+`--controlnet_dir` adds a Canny ControlNet to both stages.  Under torchrun every process edits on its local GPU
+(`LOCAL_RANK`): frames are sharded over the ranks and the all-gathers run through `ops.Communicator`; rank 0 writes
 the files.  With `--device cpu` the processes run on the CPU and gather over gloo.
 """
 from __future__ import annotations
@@ -118,22 +129,42 @@ def main(argv: Optional[List[str]] = None) -> None:
             dist.destroy_process_group()
 
 
+def read_video_input(args, rank: int, device: torch.device) -> torch.Tensor:
+    """preprocess.py:351-354 for a video `--data_path`: every frame decoded and resized to (--H, --W) on `device`,
+    written by rank 0 to data/<stem>/%05d.png; `args.data_path` becomes that folder.  Returns the first `n_frames`
+    frames, or raises ValueError when the video has fewer."""
+    from .video import read_video
+    video = args.data_path
+    frames, _ = read_video(video, (args.H, args.W), device)
+    if args.n_frames > frames.shape[0]:
+        raise ValueError(f"--n_frames {args.n_frames} but {video!r} has {frames.shape[0]} frames")
+    args.data_path = os.path.join("data", Path(video).stem)
+    if rank == 0:
+        write_frames(frames, args.data_path)
+    return frames[:args.n_frames]
+
+
 def _run(args, world: int, rank: int, comm, device: torch.device) -> None:
     import yaml
     from . import pipeline
-    from .util import add_dict_to_yaml_file, seed_everything
+    from .util import add_dict_to_yaml_file, save_video, seed_everything
+    video_frames = None
+    if args.stage == "preprocess" and os.path.isfile(args.data_path):   # decoded first: a bad video fails fast
+        video_frames = read_video_input(args, rank, device)
     dtype = torch.float16 if device.type == "cuda" else torch.float32
     parts = pipeline.load_parts(args.model_dir, device, dtype, args.controlnet_dir, args.variant)
     dist_kw = dict(world_size=world, rank=rank, comm=comm)
 
     if args.stage == "preprocess":
         seed_everything(1)                                                   # preprocess.py:303
-        frames = read_frames(args.data_path, args.n_frames)
+        frames = video_frames if video_frames is not None else read_frames(args.data_path, args.n_frames)
         _, recon = pipeline.preprocess(parts, frames, args, **dist_kw)
         if rank == 0:
             add_dict_to_yaml_file(os.path.join(args.save_dir, "inversion_prompts.yaml"), Path(args.data_path).stem,
                                   args.inversion_prompt)
-            write_frames(recon, os.path.join(pipeline.latents_dir(args, frames.shape[0]), "frames"))
+            path = pipeline.latents_dir(args, frames.shape[0])
+            write_frames(recon, os.path.join(path, "frames"))
+            save_video(recon, os.path.join(path, "inverted.mp4"), fps=10)        # preprocess.py:329-330
         return
 
     with open(args.config_path) as f:
@@ -145,12 +176,22 @@ def _run(args, world: int, rank: int, comm, device: torch.device) -> None:
     n = min(int(config["n_frames"]), next(iter(source.values())).shape[0])
     seed_everything(int(config.get("seed", 1)))                              # run_tokenflow_pnp.py:277
     frames = read_frames(config["data_path"], n)
-    out = pipeline.edit(parts, frames, config, source, **dist_kw)
+    pnp = pipeline.edit_mode(config) == "pnp"
+    out = pipeline.edit(parts, frames, config, source, vae_recon=pnp and rank == 0, **dist_kw)
     if rank == 0:
-        os.makedirs(config["output_path"], exist_ok=True)
-        with open(os.path.join(config["output_path"], "config.yaml"), "w") as f:
+        out_dir = config["output_path"]
+        os.makedirs(out_dir, exist_ok=True)
+        with open(os.path.join(out_dir, "config.yaml"), "w") as f:
             yaml.dump(config, f)
-        write_frames(out, os.path.join(config["output_path"], "img_ode"))
+        videos = {}
+        if pnp:                                                  # run_tokenflow_pnp.py:242-249 `save_vae_recon`
+            out, videos["vae_recon"] = out
+            write_frames(videos["vae_recon"], os.path.join(out_dir, "vae_recon"))
+        write_frames(out, os.path.join(out_dir, "img_ode"))
+        videos["tokenflow_PnP_fps" if pnp else "tokenflow_SDEdit_fps"] = out
+        for name, frames_u8 in videos.items():
+            for fps in (10, 20, 30):
+                save_video(frames_u8, os.path.join(out_dir, f"{name}_{fps}.mp4"), fps=fps)
 
 
 if __name__ == "__main__":

@@ -94,26 +94,25 @@ def load_imgs(data_path, n_frames, device="cuda", pil=False):
 
 
 def save_video_frames(video_path, img_size=(512, 512)):
-    """Reference util.py:18-29: decode a video into data/<name>/%05d.png resized to img_size (OpenCV decode,
-    Lanczos resize like the reference)."""
+    """Reference util.py:18-29: decode a video into data/<name>/%05d.png resized to img_size = (W, H) with PIL's
+    Lanczos, and return the number of frames.  Decoding is `video.decoded_chunks`; like the reference, a `.mov` file
+    is rotated by -90 degrees before the resize (`video.read_video` does not do this)."""
     import os
     from pathlib import Path
 
-    import cv2
     from PIL import Image
+
+    from .preprocess import resize_frames
+    from .video import decoded_chunks
 
     name = Path(video_path).stem
     os.makedirs(f"data/{name}", exist_ok=True)
-    cap = cv2.VideoCapture(video_path)
+    _, chunks = decoded_chunks(video_path)
     i = 0
-    while True:
-        ok, frame = cap.read()
-        if not ok:
-            break
-        img = Image.fromarray(cv2.cvtColor(frame, cv2.COLOR_BGR2RGB))
-        if video_path.endswith(".mov"):
-            img = img.rotate(-90, expand=True)
-        img.resize(img_size, resample=Image.Resampling.LANCZOS).save(f"data/{name}/{str(i).zfill(5)}.png")
-        i += 1
-    cap.release()
+    for frames in chunks:
+        if video_path.endswith(".mov"):                  # PIL's rotate(-90, expand=True): a quarter turn clockwise
+            frames = frames.rot90(-1, (1, 2)).contiguous()
+        for f in resize_frames(frames, (img_size[1], img_size[0])).numpy():
+            Image.fromarray(f).save(f"data/{name}/{str(i).zfill(5)}.png")
+            i += 1
     return i
