@@ -22,6 +22,7 @@ to the source stream as well, as the reference's inversion does.  It composes wi
 from __future__ import annotations
 
 import contextlib
+import gc
 import os
 from typing import Callable, Dict, Optional
 
@@ -448,6 +449,10 @@ class TokenFlowEditor(nn.Module):
                 run()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
+        # A step graph of an editor or inverter the caller has dropped can still be held by a reference cycle.  If
+        # the garbage collector freed it during the capture below, destroying that graph would be refused while the
+        # stream captures, and the capture would fail.  Free such cycles (and their graph pools) now.
+        gc.collect()
         graph = torch.cuda.CUDAGraph()
         events = [] if saved_timing is not None else None
         launches0 = ops.launch_count() if ops is not None else 0

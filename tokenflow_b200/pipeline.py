@@ -47,14 +47,26 @@ class Parts:
 
 
 def load_parts(model_dir: str, device="cuda", dtype=torch.float16, controlnet_dir: Optional[str] = None,
-               variant: Optional[str] = None) -> Parts:
-    """Every model of a diffusers checkpoint directory (and a ControlNet folder), as `checkpoint` loads them."""
-    tokenizer, text_encoder = checkpoint.load_text_encoder(model_dir, device, dtype)
-    return Parts(unet=checkpoint.load_unet(model_dir, device, dtype, variant),
-                 vae=checkpoint.load_vae(model_dir, device, dtype, variant),
-                 scheduler=checkpoint.load_scheduler(model_dir), tokenizer=tokenizer, text_encoder=text_encoder,
-                 controlnet=(checkpoint.load_controlnet(controlnet_dir, device, dtype, variant)
-                             if controlnet_dir else None))
+               variant: Optional[str] = None, weights: Optional[str] = None) -> Parts:
+    """Every model of a diffusers checkpoint directory (and a ControlNet folder), as `checkpoint` loads them.
+
+    With `weights`, a single-file SD checkpoint in the LDM layout, the UNet, VAE and text encoder take its weights,
+    on the architectures, tokenizer and scheduler of `model_dir` (`checkpoint.load_single_file_models`).  A
+    `controlnet_dir` that is a file is a cldm ControlNet (`checkpoint.load_controlnet_file`).  `variant` names the
+    weight files of the folders that are read for weights."""
+    if weights is None:
+        tokenizer, text_encoder = checkpoint.load_text_encoder(model_dir, device, dtype)
+        unet = checkpoint.load_unet(model_dir, device, dtype, variant)
+        vae = checkpoint.load_vae(model_dir, device, dtype, variant)
+    else:
+        unet, vae, tokenizer, text_encoder = checkpoint.load_single_file_models(weights, model_dir, device, dtype)
+    controlnet = None
+    if controlnet_dir and os.path.isfile(controlnet_dir):
+        controlnet = checkpoint.load_controlnet_file(controlnet_dir, model_dir, device, dtype)
+    elif controlnet_dir:
+        controlnet = checkpoint.load_controlnet(controlnet_dir, device, dtype, variant)
+    return Parts(unet=unet, vae=vae, scheduler=checkpoint.load_scheduler(model_dir), tokenizer=tokenizer,
+                 text_encoder=text_encoder, controlnet=controlnet)
 
 
 def _opt(opt, key: str, default=None):

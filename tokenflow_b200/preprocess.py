@@ -24,6 +24,7 @@ Two paths compute the same steps:
 """
 from __future__ import annotations
 
+import gc
 import os
 from typing import Dict, Iterable, List, Optional, Tuple
 
@@ -250,6 +251,7 @@ class LatentInverter:
                     step()
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
+            gc.collect()                    # no dead step graph may be freed during the capture (editor._capture)
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph, pool=self._graph_pool, capture_error_mode="thread_local"):
                 step()

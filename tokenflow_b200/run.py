@@ -26,7 +26,10 @@ n_inversion_steps must name the directory preprocess wrote.  It edits min(n_fram
 frames; unlike the reference's driver it does not trim that count to a multiple of batch_size, since the editor
 takes a short last keyframe group (INTEGRATION.md §6).
 
-`--controlnet_dir` adds a Canny ControlNet to both stages.  Under torchrun every process edits on its local GPU
+`--controlnet_dir` adds a Canny ControlNet to both stages, from a diffusers folder or a single cldm file.
+`--weights FILE` takes the UNet, VAE and text encoder weights from a single-file checkpoint in the original LDM
+layout; `--model_dir` must then be a diffusers folder of the same family, which gives the architectures, the
+tokenizer and the scheduler.  Under torchrun every process edits on its local GPU
 (`LOCAL_RANK`): frames are sharded over the ranks and the all-gathers run through `ops.Communicator`; rank 0 writes
 the files.  With `--device cpu` the processes run on the CPU and gather over gloo.
 """
@@ -102,8 +105,14 @@ def main(argv: Optional[List[str]] = None) -> None:
         p = sub.add_parser(name)
         p.add_argument("--model_dir", required=True, help="diffusers checkpoint directory (unet/, vae/, scheduler/, "
                                                           "text_encoder/, tokenizer/)")
-        p.add_argument("--controlnet_dir", default=None, help="diffusers ControlNet directory (Canny)")
-        p.add_argument("--variant", default=None, help="weights variant, e.g. fp16")
+        p.add_argument("--weights", default=None,
+                       help="single-file SD checkpoint in the original LDM layout (.safetensors, .ckpt); its UNet, "
+                            "VAE and text encoder weights replace --model_dir's, which still gives the architectures, "
+                            "tokenizer and scheduler")
+        p.add_argument("--controlnet_dir", default=None,
+                       help="diffusers ControlNet directory (Canny), or a single-file ControlNet (.pth, .safetensors) "
+                            "built on --model_dir's UNet config")
+        p.add_argument("--variant", default=None, help="weights variant of the folders read, e.g. fp16")
         p.add_argument("--device", default="cuda")
     p = sub.choices["preprocess"]
     p.add_argument("--data_path", type=str, default="data/woman-running")
@@ -152,7 +161,7 @@ def _run(args, world: int, rank: int, comm, device: torch.device) -> None:
     if args.stage == "preprocess" and os.path.isfile(args.data_path):   # decoded first: a bad video fails fast
         video_frames = read_video_input(args, rank, device)
     dtype = torch.float16 if device.type == "cuda" else torch.float32
-    parts = pipeline.load_parts(args.model_dir, device, dtype, args.controlnet_dir, args.variant)
+    parts = pipeline.load_parts(args.model_dir, device, dtype, args.controlnet_dir, args.variant, args.weights)
     dist_kw = dict(world_size=world, rank=rank, comm=comm)
 
     if args.stage == "preprocess":
