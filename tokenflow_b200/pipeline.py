@@ -20,11 +20,12 @@ import copy
 import os
 from dataclasses import dataclass
 from pathlib import Path
-from typing import Any, Dict, Optional, Tuple
+from typing import Any, Dict, Optional, Sequence, Tuple
 
 import torch
 
 from . import checkpoint
+from . import lora
 from . import tokenflow_utils
 from .editor import TokenFlowEditor
 from .preprocess import (LatentInverter, canny_cond, ddim_eps, decode_latents, encode_imgs, resize_frames,
@@ -47,13 +48,15 @@ class Parts:
 
 
 def load_parts(model_dir: str, device="cuda", dtype=torch.float16, controlnet_dir: Optional[str] = None,
-               variant: Optional[str] = None, weights: Optional[str] = None) -> Parts:
+               variant: Optional[str] = None, weights: Optional[str] = None,
+               loras: Optional[Sequence[Tuple[str, float]]] = None) -> Parts:
     """Every model of a diffusers checkpoint directory (and a ControlNet folder), as `checkpoint` loads them.
 
     With `weights`, a single-file SD checkpoint in the LDM layout, the UNet, VAE and text encoder take its weights,
     on the architectures, tokenizer and scheduler of `model_dir` (`checkpoint.load_single_file_models`).  A
     `controlnet_dir` that is a file is a cldm ControlNet (`checkpoint.load_controlnet_file`).  `variant` names the
-    weight files of the folders that are read for weights."""
+    weight files of the folders that are read for weights.  `loras`, `[(LoRA file, scale), ...]`, are merged into the
+    loaded UNet and text encoder (`lora.merge`), whichever way their weights were read."""
     if weights is None:
         tokenizer, text_encoder = checkpoint.load_text_encoder(model_dir, device, dtype)
         unet = checkpoint.load_unet(model_dir, device, dtype, variant)
@@ -65,6 +68,8 @@ def load_parts(model_dir: str, device="cuda", dtype=torch.float16, controlnet_di
         controlnet = checkpoint.load_controlnet_file(controlnet_dir, model_dir, device, dtype)
     elif controlnet_dir:
         controlnet = checkpoint.load_controlnet(controlnet_dir, device, dtype, variant)
+    if loras:
+        lora.merge(unet, text_encoder, loras)
     return Parts(unet=unet, vae=vae, scheduler=checkpoint.load_scheduler(model_dir), tokenizer=tokenizer,
                  text_encoder=text_encoder, controlnet=controlnet)
 

@@ -29,9 +29,13 @@ takes a short last keyframe group (INTEGRATION.md §6).
 `--controlnet_dir` adds a Canny ControlNet to both stages, from a diffusers folder or a single cldm file.
 `--weights FILE` takes the UNet, VAE and text encoder weights from a single-file checkpoint in the original LDM
 layout; `--model_dir` must then be a diffusers folder of the same family, which gives the architectures, the
-tokenizer and the scheduler.  Under torchrun every process edits on its local GPU
-(`LOCAL_RANK`): frames are sharded over the ranks and the all-gathers run through `ops.Communicator`; rank 0 writes
-the files.  With `--device cpu` the processes run on the CPU and gather over gloo.
+tokenizer and the scheduler.  `--lora FILE[:SCALE]` (repeatable, SCALE 1.0 by default) merges a LoRA into the UNet
+and the text encoder once they are loaded (`lora.merge`).  It applies to the stage it is given to: to invert with the
+base model and edit with the LoRA, give it to `edit` only.  The latents directory's name does not depend on it;
+`edit` records the LoRAs in its config.yaml (`loras: [{path, scale}]`).  Under torchrun every process edits on its
+local GPU (`LOCAL_RANK`), and reads and merges each LoRA itself: frames are sharded over the ranks and the
+all-gathers run through `ops.Communicator`; rank 0 writes the files.  With `--device cpu` the processes run on the
+CPU and gather over gloo.
 """
 from __future__ import annotations
 
@@ -41,7 +45,7 @@ import os
 import re
 import sys
 from pathlib import Path
-from typing import List, Optional
+from typing import List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -80,6 +84,18 @@ def read_latents(path: str) -> dict:
             for f in files}
 
 
+def parse_lora(arg: str) -> Tuple[str, float]:
+    """(path, scale) of a `--lora FILE[:SCALE]` argument: a suffix after the last `:` that parses as a float is the
+    scale, else the whole argument is the path and the scale is 1.0."""
+    path, sep, tail = arg.rpartition(":")
+    if sep:
+        try:
+            return path, float(tail)
+        except ValueError:
+            pass
+    return arg, 1.0
+
+
 def _distributed(device: str):
     """(world_size, rank, communicator, device) of this process: under torchrun one GPU per process (`LOCAL_RANK`)
     with the library's NCCL all-gather, or CPU processes over gloo with `--device cpu`; else one process."""
@@ -113,6 +129,9 @@ def main(argv: Optional[List[str]] = None) -> None:
                        help="diffusers ControlNet directory (Canny), or a single-file ControlNet (.pth, .safetensors) "
                             "built on --model_dir's UNet config")
         p.add_argument("--variant", default=None, help="weights variant of the folders read, e.g. fp16")
+        p.add_argument("--lora", action="append", default=[], type=parse_lora, metavar="FILE[:SCALE]",
+                       help="LoRA file (kohya, diffusers or PEFT layout) merged into the UNet and text encoder of this "
+                            "stage at SCALE (default 1.0); repeatable")
         p.add_argument("--device", default="cuda")
     p = sub.choices["preprocess"]
     p.add_argument("--data_path", type=str, default="data/woman-running")
@@ -161,7 +180,8 @@ def _run(args, world: int, rank: int, comm, device: torch.device) -> None:
     if args.stage == "preprocess" and os.path.isfile(args.data_path):   # decoded first: a bad video fails fast
         video_frames = read_video_input(args, rank, device)
     dtype = torch.float16 if device.type == "cuda" else torch.float32
-    parts = pipeline.load_parts(args.model_dir, device, dtype, args.controlnet_dir, args.variant, args.weights)
+    parts = pipeline.load_parts(args.model_dir, device, dtype, args.controlnet_dir, args.variant, args.weights,
+                                args.lora)
     dist_kw = dict(world_size=world, rank=rank, comm=comm)
 
     if args.stage == "preprocess":
@@ -190,6 +210,8 @@ def _run(args, world: int, rank: int, comm, device: torch.device) -> None:
     if rank == 0:
         out_dir = config["output_path"]
         os.makedirs(out_dir, exist_ok=True)
+        if args.lora:
+            config["loras"] = [{"path": path, "scale": scale} for path, scale in args.lora]
         with open(os.path.join(out_dir, "config.yaml"), "w") as f:
             yaml.dump(config, f)
         videos = {}

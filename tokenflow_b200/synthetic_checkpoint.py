@@ -7,10 +7,14 @@ variant or in shards, the VAE's mid-block attentions optionally under the deprec
 VAE files use, a random CLIP text encoder (small, or of CLIP ViT-L/14's size) and a CLIP tokenizer over single letters,
 so every word of a prompt is several tokens.
 
+`write_lora` writes random LoRAs for the loaded models in the kohya-ss, diffusers, PEFT and attention-processor layouts
+`lora.read` takes.
+
 The SD1.5, SD2.1 (768, v) and sd-controlnet-canny configs are the published config.json values of those checkpoints.
 """
 import json
 import os
+import re
 
 import torch
 
@@ -172,3 +176,73 @@ def write_checkpoint(root, kind="tiny", scheduler=SD15_SCHEDULER, controlnet=Fal
         cn = build_controlnet(kind, seed=3)
         write_model(cn_dir, cn, TINY_CANNY if kind == "tiny" else SD15_CANNY, variant, dtype, fmt, shards)
     return model_dir, cn_dir
+
+
+# kohya-ss's target classes: its default LoRA (Transformer2DModel; CLIPAttention and CLIPMLP of the text encoder) and
+# LoCon's convolution blocks
+_TARGET_CLASSES = {"transformer": ("Transformer2DModel",), "conv": ("ResnetBlock2D", "Downsample2D", "Upsample2D"),
+                   "text_encoder": ("CLIPAttention", "CLIPMLP")}
+
+
+def lora_targets(unet, text_encoder, targets):
+    """[(model, module path)] of the `targets`, in `named_modules` order: "attention" (the UNet attentions' to_q,
+    to_k, to_v and to_out.0), and kohya's sets "transformer" (every Linear and Conv2d inside a Transformer2DModel: 192
+    on SD), "conv" (inside ResnetBlock2D, Downsample2D and Upsample2D: LoCon) and "text_encoder" (inside CLIPAttention
+    and CLIPMLP)."""
+    out = []
+    for model, net in (("unet", unet), ("text_encoder", text_encoder)):
+        classes = sum((_TARGET_CLASSES[t] for t in targets if t != "attention"), ())
+        inside = [n for n, m in net.named_modules() if type(m).__name__ in classes]
+        for name, m in net.named_modules():
+            if not isinstance(m, (torch.nn.Linear, torch.nn.Conv2d)):
+                continue
+            attention = (model == "unet" and "attention" in targets
+                         and re.search(r"\.attn[12]\.(to_q|to_k|to_v|to_out\.0)$", name) is not None)
+            if attention or any(name.startswith(p + ".") for p in inside):
+                out.append((model, name))
+    return out
+
+
+def _lora_stem(layout, model, name):
+    if layout == "kohya":
+        return {"unet": "lora_unet_", "text_encoder": "lora_te_"}[model] + name.replace(".", "_")
+    if layout in ("diffusers", "peft"):
+        return f"{model}.{name}"
+    head, _, proj = name.rpartition(".attn")
+    attn, _, proj = proj.partition(".")
+    if model != "unet" or proj not in ("to_q", "to_k", "to_v", "to_out.0"):
+        raise ValueError(f"the attention-processor layout has no key for {model} module {name!r}")
+    return f"unet.{head}.attn{attn}.processor.{proj.split('.')[0]}_lora"
+
+
+_LORA_SUFFIX = {"kohya": (".lora_down.weight", ".lora_up.weight"),
+                "diffusers": (".lora.down.weight", ".lora.up.weight"),
+                "peft": (".lora_A.weight", ".lora_B.weight"), "processor": (".down.weight", ".up.weight")}
+
+
+def write_lora(path, unet, text_encoder, layout="kohya", rank=4, targets=("attention",), alpha=None, seed=0):
+    """A random LoRA of rank `rank` for the `lora_targets` of `targets` in `layout` ("kohya", "diffusers", "peft" or
+    "processor"), written with safetensors (a `.bin` / `.pt` path with torch.save) in fp16, as LoRAs are published.
+    The values depend only on the targets' shapes, `rank` and `seed`, never on the layout: down ~ N(0, 1/fan_in) [rank, in, (kh, kw)], up ~ N(0, 1/rank)
+    [out, rank, (1, 1)], so a merged update is about as large as the default init's weights.  `alpha` (a number) is
+    written as each module's `.alpha`; None writes none.  Returns the targets."""
+    from safetensors.torch import save_file
+    g = torch.Generator().manual_seed(seed)
+    found = lora_targets(unet, text_encoder, targets)
+    nets = {"unet": unet, "text_encoder": text_encoder}
+    down_sfx, up_sfx = _LORA_SUFFIX[layout]
+    state = {}
+    for model, name in found:
+        shape = nets[model].get_submodule(name).weight.shape
+        fan_in = shape[1:].numel()
+        down = torch.randn((rank, *shape[1:]), generator=g) / fan_in ** 0.5
+        up = torch.randn((shape[0], rank, *([1, 1] if len(shape) == 4 else [])), generator=g) / rank ** 0.5
+        stem = _lora_stem(layout, model, name)
+        state[stem + down_sfx], state[stem + up_sfx] = down.half(), up.half()
+        if alpha is not None:
+            state[stem + ".alpha"] = torch.tensor(float(alpha), dtype=torch.float16)
+    if str(path).endswith(".safetensors"):
+        save_file(state, str(path))
+    else:
+        torch.save(state, str(path))
+    return found
