@@ -9,7 +9,9 @@ the UNet's encoder (`conv_in`, `time_embedding`, `down_blocks`, `mid_block`, the
     block, SiLU between the convolutions, and a zero-initialised conv_out to the UNet's first width (320);
   * `controlnet_down_blocks.0-11`: zero-initialised 1x1 convolutions, one per UNet skip;
   * `controlnet_mid_block`: a zero-initialised 1x1 convolution on the mid-block output.
-The state-dict names and shapes are diffusers', so real weights load with `strict=True`.
+The state-dict names and shapes are diffusers', so real weights load with `strict=True`.  Every lllyasviel ControlNet
+of the v1.1 family (depth, softedge, lineart, tile, ip2p, ...) has this architecture; `MultiControlNetModel` runs
+several of them on one UNet call, as diffusers' does.
 
 The blocks are `sd_unet`'s, so a CUDA fp16 channels_last ControlNet runs its GroupNorm and GEGLU sites on the
 library's kernels like the UNet body does.  Its attention stays plain: the TokenFlow hooks patch the UNet they are
@@ -162,6 +164,68 @@ class ControlNetModel(nn.Module):
         return tuple(down), mid
 
 
+class MultiControlNetModel(nn.Module):
+    """diffusers' `MultiControlNetModel`: several ControlNets on one UNet call, with `ControlNetModel`'s call signature.
+
+    `controlnet_cond` is one tensor [N, Σ c_k, H, W], the nets' conditionings concatenated along channels in net order;
+    it is split by each net's `conditioning_channels`, so every caller that gathers or slices the conditioning by frame
+    handles one tensor whatever the number of nets.  Each net's residuals are scaled by its own scale, then added in net
+    order in the residuals' dtype (one rounding per add in fp16), as diffusers sums them; the UNet adds the sum to its
+    skips as it adds one net's residuals."""
+
+    def __init__(self, nets):
+        super().__init__()
+        self.nets = nn.ModuleList(nets)
+        if len(self.nets) == 0:
+            raise ValueError("MultiControlNetModel needs at least one ControlNet")
+
+    @property
+    def conditioning_channels(self) -> Tuple[int, ...]:
+        return tuple(net.config.conditioning_channels for net in self.nets)
+
+    def forward(self, sample, timestep, encoder_hidden_states=None, controlnet_cond=None, conditioning_scale=1.0,
+                return_dict: bool = False, **_):
+        """(down_block_res_samples, mid_block_res_sample) of the nets' summed residuals.  `conditioning_scale` is a
+        float for every net or a list of one per net."""
+        scales = conditioning_scale_for(self, conditioning_scale)
+        if controlnet_cond is None or controlnet_cond.shape[1] != sum(self.conditioning_channels):
+            got = None if controlnet_cond is None else controlnet_cond.shape[1]
+            raise ValueError(f"MultiControlNetModel needs controlnet_cond with {sum(self.conditioning_channels)} "
+                             f"channels {self.conditioning_channels}, got {got}")
+        down, mid = None, None
+        for net, cond, scale in zip(self.nets, controlnet_cond.split(self.conditioning_channels, dim=1), scales):
+            d, m = net(sample, timestep, encoder_hidden_states, controlnet_cond=cond, conditioning_scale=scale)
+            if down is None:
+                down, mid = d, m
+            else:
+                down = tuple(a + b for a, b in zip(down, d))
+                mid = mid + m
+        return down, mid
+
+
+def controlnets(controlnet) -> list:
+    """The ControlNets `controlnet` runs: [] for None, its nets for a MultiControlNetModel, else [controlnet]."""
+    if controlnet is None:
+        return []
+    return list(controlnet.nets) if isinstance(controlnet, MultiControlNetModel) else [controlnet]
+
+
+def conditioning_scale_for(controlnet, scale):
+    """`scale` (a number, or a list of one per net) as `controlnet` takes it: a float for a ControlNetModel (a list of
+    one is unwrapped), a list of floats for a MultiControlNetModel (a number applies to every net).  A list of another
+    length raises ValueError naming both lengths.  Without a ControlNet there is no scale: None."""
+    if controlnet is None:
+        return None
+    k = len(controlnets(controlnet))
+    if isinstance(scale, (list, tuple)):
+        if len(scale) != k:
+            raise ValueError(f"{len(scale)} ControlNet conditioning scales for {k} ControlNets")
+        scales = [float(s) for s in scale]
+    else:
+        scales = [float(scale)] * k
+    return scales if isinstance(controlnet, MultiControlNetModel) else scales[0]
+
+
 def build_controlnet(kind: str = "sd15", seed: int = 1, device="cpu", dtype=torch.float32) -> ControlNetModel:
     """Random-init ControlNet (default PyTorch inits for every parameter, the zero convolutions included, so that the
     residuals are not zero, as with trained weights), drawn on the CPU from `seed` and moved."""
@@ -175,9 +239,9 @@ def build_controlnet(kind: str = "sd15", seed: int = 1, device="cpu", dtype=torc
     return net.to(device=device, dtype=dtype).eval()
 
 
-def controlnet_residuals(controlnet, x, t, ctx, cond, scale: float = 1.0):
+def controlnet_residuals(controlnet, x, t, ctx, cond, scale=1.0):
     """The first half of the reference's `controlnet_pred` (preprocess.py:130-137): the UNet keyword arguments of one
-    call, {} when there is no ControlNet."""
+    call, {} when there is no ControlNet.  `scale` is as `conditioning_scale_for` returns it."""
     if controlnet is None:
         return {}
     down, mid = controlnet(x, t, encoder_hidden_states=ctx, controlnet_cond=cond, conditioning_scale=scale,

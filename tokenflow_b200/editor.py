@@ -41,7 +41,9 @@ class TokenFlowEditor(nn.Module):
         guidance_scale, mode ('pnp' | 'sdedit'), pnp_attn_t, pnp_f_t, start (sdedit), latents_path,
         controlnet_conditioning_scale (default 1.0).
         text_embeds: [2, L, C] (uncond, cond);  pnp_guidance_embeds: [1, L, C] (inversion prompt).
-        controlnet, controlnet_cond: an optional ControlNet and the [N, 3, H, W] conditioning of all N frames."""
+        controlnet, controlnet_cond: an optional ControlNet (or a MultiControlNetModel of K nets) and the [N, 3, H, W]
+        ([N, 3K, H, W]) conditioning of all N frames; controlnet_conditioning_scale is a number, or a list of one per
+        net."""
         super().__init__()
         if (controlnet is None) != (controlnet_cond is None):
             raise ValueError("TokenFlowEditor needs both controlnet and controlnet_cond, or neither")
@@ -94,6 +96,9 @@ class TokenFlowEditor(nn.Module):
         self._text_cache = {}
         self._shard_cache = {}
         self._ccond = None
+        from .controlnet import conditioning_scale_for
+        self._controlnet_scale = conditioning_scale_for(controlnet,
+                                                        self.config.get("controlnet_conditioning_scale", 1.0))
         if controlnet is not None:
             cl = next(controlnet.parameters()).is_contiguous(memory_format=torch.channels_last)
             self._ccond = controlnet_cond.to(self.device, next(controlnet.parameters()).dtype).contiguous(
@@ -102,8 +107,7 @@ class TokenFlowEditor(nn.Module):
     def _residuals(self, latent_model_input, t, text, cond):
         """UNet keyword arguments of one call: the ControlNet's residuals for `cond`, or {} without a ControlNet."""
         from .controlnet import controlnet_residuals
-        return controlnet_residuals(self.controlnet, latent_model_input, t, text, cond,
-                                    float(self.config.get("controlnet_conditioning_scale", 1.0)))
+        return controlnet_residuals(self.controlnet, latent_model_input, t, text, cond, self._controlnet_scale)
 
     # ------------------------------------------------------------------------------------
     def init_method(self):

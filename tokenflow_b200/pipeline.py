@@ -4,9 +4,9 @@
 Both take the loaded models (`Parts`, `load_parts`) and uint8 frames, and hold only the drivers' control flow; every
 step is a stage function of this package, the chain INTEGRATION.md §6 writes out:
 
-    preprocess: resize_frames -> encode_imgs [-> canny_cond] -> LatentInverter.ddim_inversion / ddim_sample ->
+    preprocess: resize_frames -> encode_imgs [-> control_cond] -> LatentInverter.ddim_inversion / ddim_sample ->
                 decode_latents
-    edit:       resize_frames -> encode_imgs [-> canny_cond] -> ddim_eps -> add_noise -> TokenFlowEditor.sample_loop ->
+    edit:       resize_frames -> encode_imgs [-> control_cond] -> ddim_eps -> add_noise -> TokenFlowEditor.sample_loop ->
                 decode_latents
 
 With a CUDA fp16 UNet the inversion runs its captured step (`tf_ddim` / `tf_ddim_v`) and the edit its fused, captured
@@ -20,7 +20,7 @@ import copy
 import os
 from dataclasses import dataclass
 from pathlib import Path
-from typing import Any, Dict, Optional, Sequence, Tuple
+from typing import Any, Dict, Optional, Sequence, Tuple, Union
 
 import torch
 
@@ -28,7 +28,8 @@ from . import checkpoint
 from . import lora
 from . import tokenflow_utils
 from .editor import TokenFlowEditor
-from .preprocess import (LatentInverter, canny_cond, ddim_eps, decode_latents, encode_imgs, resize_frames,
+from .controlnet import MultiControlNetModel, controlnets
+from .preprocess import (LatentInverter, control_cond, ddim_eps, decode_latents, encode_imgs, resize_frames,
                          write_inversion_prompt)
 
 
@@ -40,22 +41,25 @@ class Parts:
     scheduler: Any
     tokenizer: Any
     text_encoder: Any
-    controlnet: Any = None
+    controlnet: Any = None          # a ControlNetModel, or a MultiControlNetModel of several
 
     @property
     def device(self) -> torch.device:
         return next(self.unet.parameters()).device
 
 
-def load_parts(model_dir: str, device="cuda", dtype=torch.float16, controlnet_dir: Optional[str] = None,
+def load_parts(model_dir: str, device="cuda", dtype=torch.float16,
+               controlnet_dir: Union[None, str, Sequence[str]] = None,
                variant: Optional[str] = None, weights: Optional[str] = None,
                loras: Optional[Sequence[Tuple[str, float]]] = None) -> Parts:
     """Every model of a diffusers checkpoint directory (and a ControlNet folder), as `checkpoint` loads them.
 
     With `weights`, a single-file SD checkpoint in the LDM layout, the UNet, VAE and text encoder take its weights,
-    on the architectures, tokenizer and scheduler of `model_dir` (`checkpoint.load_single_file_models`).  A
-    `controlnet_dir` that is a file is a cldm ControlNet (`checkpoint.load_controlnet_file`).  `variant` names the
-    weight files of the folders that are read for weights.  `loras`, `[(LoRA file, scale), ...]`, are merged into the
+    on the architectures, tokenizer and scheduler of `model_dir` (`checkpoint.load_single_file_models`).
+    `controlnet_dir` is one ControlNet or a sequence of them, each a diffusers folder or a cldm file
+    (`checkpoint.load_controlnet_file`); one stays a plain ControlNetModel, two or more become a
+    `MultiControlNetModel` in the order given.  `variant` names the weight files of the folders that are read for
+    weights.  `loras`, `[(LoRA file, scale), ...]`, are merged into the
     loaded UNet and text encoder (`lora.merge`), whichever way their weights were read."""
     if weights is None:
         tokenizer, text_encoder = checkpoint.load_text_encoder(model_dir, device, dtype)
@@ -63,11 +67,10 @@ def load_parts(model_dir: str, device="cuda", dtype=torch.float16, controlnet_di
         vae = checkpoint.load_vae(model_dir, device, dtype, variant)
     else:
         unet, vae, tokenizer, text_encoder = checkpoint.load_single_file_models(weights, model_dir, device, dtype)
-    controlnet = None
-    if controlnet_dir and os.path.isfile(controlnet_dir):
-        controlnet = checkpoint.load_controlnet_file(controlnet_dir, model_dir, device, dtype)
-    elif controlnet_dir:
-        controlnet = checkpoint.load_controlnet(controlnet_dir, device, dtype, variant)
+    paths = [controlnet_dir] if isinstance(controlnet_dir, (str, os.PathLike)) else list(controlnet_dir or [])
+    nets = [checkpoint.load_controlnet_file(path, model_dir, device, dtype) if os.path.isfile(path) else
+            checkpoint.load_controlnet(path, device, dtype, variant) for path in paths]
+    controlnet = None if not nets else nets[0] if len(nets) == 1 else MultiControlNetModel(nets).eval()
     if loras:
         lora.merge(unet, text_encoder, loras)
     return Parts(unet=unet, vae=vae, scheduler=checkpoint.load_scheduler(model_dir), tokenizer=tokenizer,
@@ -76,6 +79,26 @@ def load_parts(model_dir: str, device="cuda", dtype=torch.float16, controlnet_di
 
 def _opt(opt, key: str, default=None):
     return opt.get(key, default) if isinstance(opt, dict) else getattr(opt, key, default)
+
+
+def conditioning(parts: Parts, frames: torch.Tensor, controls=None) -> Optional[torch.Tensor]:
+    """The ControlNet conditioning of the resized uint8 `frames` (`control_cond`), None without a ControlNet.
+    `controls` has one source per net ("canny", "frames" or a uint8 tensor of maps); None is Canny for every net.
+    ValueError for a count that does not match the nets, and for a net whose conditioning_channels is not 3 (every
+    source is RGB)."""
+    nets = controlnets(parts.controlnet)
+    if not nets:
+        if controls is not None:
+            raise ValueError(f"{len(controls)} controls given but no ControlNet")
+        return None
+    for i, net in enumerate(nets):
+        if net.config.conditioning_channels != 3:
+            raise ValueError(f"ControlNet {i} takes {net.config.conditioning_channels} conditioning channels: every "
+                             "control source is RGB (3)")
+    controls = ["canny"] * len(nets) if controls is None else list(controls)
+    if len(controls) != len(nets):
+        raise ValueError(f"{len(controls)} controls for {len(nets)} ControlNets")
+    return control_cond(frames, controls)
 
 
 def latents_dir(opt, n_frames: int) -> str:
@@ -87,13 +110,15 @@ def latents_dir(opt, n_frames: int) -> str:
 
 @torch.no_grad()
 def preprocess(parts: Parts, frames_u8: torch.Tensor, opt, world_size: int = 1, rank: int = 0, group=None,
-               comm=None) -> Tuple[Dict[int, torch.Tensor], torch.Tensor]:
+               comm=None, controls=None) -> Tuple[Dict[int, torch.Tensor], torch.Tensor]:
     """uint8 frames [N, H_in, W_in, 3] -> ({t: inverted latents [N, 4, h, w]}, reconstruction uint8 [N, H, W, 3]).
 
     `opt` (an argparse namespace or a dict) has the reference's preprocess flags: H, W, steps, batch_size, save_steps,
     inversion_prompt, and, to write the reference's latents directory (`latents_dir`: latents/noisy_latents_<t>.pt and
-    inversion_prompt.txt), save_dir, sd_version and data_path; without save_dir nothing is written.  Square frames are
-    resized to 512², others to (H, W), as the reference does.  The latents of the `save_steps` sampling timesteps and of
+    inversion_prompt.txt), save_dir, sd_version and data_path; without save_dir nothing is written.  With a ControlNet,
+    `controls` gives each net its conditioning source (`conditioning`; None: Canny), and `controlnet_conditioning_scale`
+    (default 1.0; a number or a list of one per net) scales its residuals.  The latents directory's name does not
+    depend on the ControlNets.  Square frames are resized to 512², others to (H, W), as the reference does.  The latents of the `save_steps` sampling timesteps and of
     the last inversion step are kept, as `get_timesteps(..., strength=1.0)` selects them (preprocess.py:17-24,
     :297-301)."""
     device = parts.device
@@ -101,7 +126,7 @@ def preprocess(parts: Parts, frames_u8: torch.Tensor, opt, world_size: int = 1, 
     square = frames.shape[1] == frames.shape[2]
     frames = resize_frames(frames, 512 if square else (int(_opt(opt, "H")), int(_opt(opt, "W"))))
     latents = encode_imgs(parts.vae, frames)
-    edges = canny_cond(frames) if parts.controlnet is not None else None
+    ccond = conditioning(parts, frames, controls)
     sampling = copy.deepcopy(parts.scheduler)
     sampling.set_timesteps(int(_opt(opt, "save_steps")))
     save_path = None
@@ -110,7 +135,8 @@ def preprocess(parts: Parts, frames_u8: torch.Tensor, opt, world_size: int = 1, 
         if rank == 0:
             write_inversion_prompt(save_path, _opt(opt, "inversion_prompt"))
     inv = LatentInverter(parts.unet, copy.deepcopy(parts.scheduler), int(_opt(opt, "steps")), world_size, rank, group,
-                         controlnet=parts.controlnet, controlnet_cond=edges)
+                         controlnet=parts.controlnet, controlnet_cond=ccond,
+                         controlnet_conditioning_scale=_opt(opt, "controlnet_conditioning_scale", 1.0))
     if comm is not None:
         inv.attach_communicator(comm)
     prompt = _opt(opt, "inversion_prompt")
@@ -129,7 +155,7 @@ def edit_mode(config: Dict) -> str:
 
 @torch.no_grad()
 def edit(parts: Parts, frames_u8: torch.Tensor, config: Dict, source_latents: Dict[int, torch.Tensor],
-         world_size: int = 1, rank: int = 0, group=None, comm=None, vae_recon: bool = False):
+         world_size: int = 1, rank: int = 0, group=None, comm=None, vae_recon: bool = False, controls=None):
     """uint8 frames [N, H_in, W_in, 3] and the inverted latents of their preprocess ({t: [>= N, 4, h, w]}) -> the
     edited uint8 frames [N, 8h, 8w, 3]; with `vae_recon`, (edited frames, the VAE reconstruction of the source
     frames [N, 8h, 8w, 3]), which is `decode_latents` of the latents the edit starts from (the reference's
@@ -142,9 +168,10 @@ def edit(parts: Parts, frames_u8: torch.Tensor, config: Dict, source_latents: Di
     step, captured into CUDA graphs on a CUDA UNet, unless the config says otherwise.  The frames are resized to the
     latents' size times 8 (square ones come out of preprocess at 512²).  SDEdit with `use_ddim_noise: False` draws
     one noise latent from the global generator and repeats it over the frames (run_tokenflow_sdedit.py:198); the
-    keyframes come from the global CPU generator too, as in the reference, so seed before calling.
+    keyframes come from the global CPU generator too, as in the reference, so seed before calling.  `controls` is as
+    in `preprocess`; the scale is `config["controlnet_conditioning_scale"]`.
 
-    With several ranks every rank resizes, encodes (and runs Canny on) all N frames, since the editor holds the
+    With several ranks every rank resizes, encodes (and conditions) all N frames, since the editor holds the
     latents of all frames, and decodes all N edited frames; only the denoising work is split.  The same holds for
     `preprocess`'s encode and reconstruction decode.  These stages take about 3 % of a single-GPU C2 run."""
     device = parts.device
@@ -155,7 +182,7 @@ def edit(parts: Parts, frames_u8: torch.Tensor, config: Dict, source_latents: Di
     h, w = next(iter(source.values())).shape[-2:]
     frames = resize_frames(frames_u8.to(device), (8 * h, 8 * w))
     latents = encode_imgs(parts.vae, frames)
-    edges = canny_cond(frames) if parts.controlnet is not None else None
+    ccond = conditioning(parts, frames, controls)
     cfg = dict(config)
     cfg["mode"] = edit_mode(cfg)
     cfg.setdefault("fused_pass", True)
@@ -166,7 +193,7 @@ def edit(parts: Parts, frames_u8: torch.Tensor, config: Dict, source_latents: Di
     pnp = checkpoint.text_embeds(tok, enc, inv_prompt, inv_prompt).chunk(2)[0]
     editor = TokenFlowEditor(parts.unet, copy.deepcopy(parts.scheduler), tokenflow_utils, cfg, text, pnp,
                              source_latents=source.__getitem__, world_size=world_size, rank=rank, group=group,
-                             controlnet=parts.controlnet, controlnet_cond=edges)
+                             controlnet=parts.controlnet, controlnet_cond=ccond)
     if comm is not None:
         editor.attach_communicator(comm)
     eps = ddim_eps(latents, source, editor.scheduler)

@@ -8,11 +8,11 @@ run_tokenflow_pnp.py:145-163, on `vae.AutoencoderKL`), and the edit's starting n
     encode_imgs -> LatentInverter.ddim_inversion -> saved_latents() -> ddim_eps -> scheduler.add_noise ->
     TokenFlowEditor.sample_loop -> decode_latents
 
-With a ControlNet (controlnet.py) and the Canny conditioning of the frames (`canny_cond`), every UNet call of both
-directions is the reference's `controlnet_pred` (preprocess.py:129-149): the ControlNet on the batch's frames of the
-conditioning, then the UNet with its residuals.  The CLIP text encoder and the depth variant stay out of scope.  The
-latents directory is still written in the reference's format, so it can be read back by `TokenFlowEditor` / the
-reference drivers (`tokenflow_utils.load_source_latents_t`).  Frames are independent in this stage, so with several ranks each rank
+With a ControlNet (controlnet.py) and the conditioning of the frames (`canny_cond`, or `control_cond` for other
+sources and several nets), every UNet call of both directions is the reference's `controlnet_pred`
+(preprocess.py:129-149): the ControlNet on the batch's frames of the conditioning, then the UNet with its residuals.
+The CLIP text encoder and the depth variant stay out of scope.  The latents directory is still written in the
+reference's format, so it can be read back by `TokenFlowEditor` / the reference drivers (`tokenflow_utils.load_source_latents_t`).  Frames are independent in this stage, so with several ranks each rank
 inverts its own contiguous share and the saved tensors are all-gathered.
 
 Two paths compute the same steps:
@@ -76,15 +76,18 @@ def saved_timesteps(ts_up: List[int], timesteps_to_save: Optional[Iterable[int]]
 
 class LatentInverter:
     def __init__(self, unet, scheduler, n_timesteps: int, world_size: int = 1, rank: int = 0, group=None,
-                 controlnet=None, controlnet_cond: Optional[torch.Tensor] = None):
+                 controlnet=None, controlnet_cond: Optional[torch.Tensor] = None, controlnet_conditioning_scale=1.0):
         """`scheduler.set_timesteps(n_timesteps)` defines the inversion grid (reference default: 500 steps, of which
-        the 50 sampling timesteps are saved).  `controlnet` and `controlnet_cond` ([N, 3, H, W], the Canny
-        conditioning of all N frames, `canny_cond`) run every UNet call as the reference's `controlnet_pred`; each
-        rank reads the conditioning of its own frames."""
+        the 50 sampling timesteps are saved).  `controlnet` and `controlnet_cond` ([N, 3, H, W], the conditioning of
+        all N frames, `control_cond`; [N, 3K, H, W] for a MultiControlNetModel of K nets) run every UNet call as the
+        reference's `controlnet_pred`, at `controlnet_conditioning_scale` (a number, or a list of one per net; the
+        reference's 1.0 by default); each rank reads the conditioning of its own frames."""
+        from .controlnet import conditioning_scale_for
         if (controlnet is None) != (controlnet_cond is None):
             raise ValueError("LatentInverter needs both controlnet and controlnet_cond, or neither")
         self.unet, self.scheduler = unet, scheduler
         self.controlnet, self.controlnet_cond = controlnet, controlnet_cond
+        self.controlnet_scale = conditioning_scale_for(controlnet, controlnet_conditioning_scale)
         self.device = next(unet.parameters()).device
         self.scheduler.set_timesteps(n_timesteps, device=self.device)
         self.world_size, self.rank, self.group = world_size, rank, group
@@ -120,7 +123,7 @@ class LatentInverter:
         ccond = None
         if self.controlnet is not None:
             ccond = self.controlnet_cond[frame0:frame0 + x.shape[0]].to(x.device)
-        res = controlnet_residuals(self.controlnet, x, t_dev, ctx, ccond)
+        res = controlnet_residuals(self.controlnet, x, t_dev, ctx, ccond, self.controlnet_scale)
         out = self.unet(x, t_dev, encoder_hidden_states=ctx, **res)
         return out["sample"] if isinstance(out, dict) else out.sample
 
@@ -233,7 +236,8 @@ class LatentInverter:
             for b in range(0, share, bs):
                 xb = x[b:b + bs]
                 ctx = st["cond"][:xb.shape[0]]
-                res = controlnet_residuals(self.controlnet, xb, st["t"], ctx, st["ccond"][b:b + bs]) \
+                res = controlnet_residuals(self.controlnet, xb, st["t"], ctx, st["ccond"][b:b + bs],
+                                           self.controlnet_scale) \
                     if self.controlnet is not None else {}
                 out = self.unet(xb, st["t"], encoder_hidden_states=ctx, **res)
                 outs.append(out["sample"] if isinstance(out, dict) else out.sample)
@@ -360,6 +364,44 @@ def canny_cond(frames_u8: torch.Tensor, low: float = 100, high: float = 200) -> 
     edges = np.stack([cv2.Canny(f, low, high) for f in frames_u8.contiguous().numpy()])
     image = np.concatenate([edges[..., None]] * 3, axis=-1)
     return torch.from_numpy(image.astype(np.float32) / 255.0).permute(0, 3, 1, 2).to(torch.float16)
+
+
+def _unit_rgb(frames_u8: torch.Tensor) -> torch.Tensor:
+    """uint8 [N, H, W, 3] -> fp16 [N, 3, H, W] (channels_last strides): diffusers' control-image conversion,
+    `np.float32(v) / 255` then the model's dtype.  fp32 division is IEEE's on both devices, so the CUDA values are
+    the host's."""
+    return frames_u8.permute(0, 3, 1, 2).float().div(255).half()
+
+
+def control_cond(frames_u8: torch.Tensor, sources) -> torch.Tensor:
+    """The conditioning of one ControlNet per entry of `sources`, for uint8 RGB frames [N, H, W, 3] at the size they
+    are edited at: fp16 [N, 3K, H, W] for K sources, the nets' conditionings concatenated along channels in order (as
+    `MultiControlNetModel` splits them).  Each source is
+      * "canny": `canny_cond(frames_u8)`, the reference's Canny conditioning;
+      * "frames": the frames themselves, for the tile and ip2p ControlNets;
+      * a uint8 [M, h, w, 3] tensor of control maps (depth, softedge, lineart, ... from the user's own annotator):
+        the first N are resized to (H, W) by `resize_frames`, the Lanczos resize diffusers' control image processor
+        uses too.  M < N raises ValueError naming both counts.
+    "frames" and maps take diffusers' control-image conversion, `np.float32(v) / 255` then fp16.  CUDA frames are
+    converted on the device; the result has channels_last strides, as `canny_cond`'s."""
+    assert frames_u8.dtype == torch.uint8 and frames_u8.dim() == 4 and frames_u8.shape[-1] == 3
+    n, h, w = frames_u8.shape[:3]
+    conds = []
+    for src in sources:
+        if isinstance(src, str):
+            if src not in ("canny", "frames"):
+                raise ValueError(f"control source {src!r}: expected 'canny', 'frames' or a uint8 [M, h, w, 3] tensor")
+            conds.append(canny_cond(frames_u8) if src == "canny" else _unit_rgb(frames_u8))
+            continue
+        if not torch.is_tensor(src) or src.dtype != torch.uint8 or src.dim() != 4 or src.shape[-1] != 3:
+            raise ValueError("control maps must be a uint8 [M, h, w, 3] tensor, got "
+                             f"{tuple(src.shape) if torch.is_tensor(src) else type(src).__name__}")
+        if src.shape[0] < n:
+            raise ValueError(f"{src.shape[0]} control maps for {n} frames")
+        conds.append(_unit_rgb(resize_frames(src[:n].to(frames_u8.device), (h, w))))
+    if not conds:
+        raise ValueError("control_cond needs at least one source")
+    return conds[0] if len(conds) == 1 else torch.cat(conds, dim=1)
 
 
 def _native_vae(vae) -> bool:

@@ -4,7 +4,8 @@ the reference's latents directory, edited frames and videos out.
     python -m tokenflow_b200.run preprocess --model_dir DIR --data_path VIDEO_OR_FRAMES [--H 512 --W 512
         --save_dir latents --sd_version 2.1 --steps 500 --batch_size 40 --save_steps 50 --n_frames 40
         --inversion_prompt "..."]
-    python -m tokenflow_b200.run edit --config_path configs/config_pnp.yaml --model_dir DIR [--controlnet_dir DIR]
+    python -m tokenflow_b200.run edit --config_path configs/config_pnp.yaml --model_dir DIR [--controlnet_dir DIR
+        [--control SOURCE]] ...
 
 `preprocess` takes the reference's flags (preprocess.py:336-349).  A `--data_path` that is a file is a video: as
 preprocess.py:351-354 does, every frame is decoded (`video.read_video`, OpenCV's FFmpeg) and resized to --W x --H,
@@ -26,7 +27,15 @@ n_inversion_steps must name the directory preprocess wrote.  It edits min(n_fram
 frames; unlike the reference's driver it does not trim that count to a multiple of batch_size, since the editor
 takes a short last keyframe group (INTEGRATION.md §6).
 
-`--controlnet_dir` adds a Canny ControlNet to both stages, from a diffusers folder or a single cldm file.
+`--controlnet_dir` adds a ControlNet to both stages, from a diffusers folder or a single cldm file; repeated, it adds
+several, whose residuals are summed (`MultiControlNetModel`).  `--control SOURCE`, repeatable, pairs with
+`--controlnet_dir` by position and gives that net its conditioning: `canny` (the Canny edges of the frames), `frames`
+(the frames themselves, for tile and ip2p), or control maps from the user's own annotator as a video file
+(`video.read_video`) or a %05d.png / %05d.jpg folder (`read_frames`), resized to the size the frames are edited at.
+Without `--control` every net gets Canny; other counts are refused before any model loads.  `preprocess` takes
+`--controlnet_conditioning_scale S [S ...]` (one scale for every net, or one per net; default 1.0), `edit` the config
+key of that name.  The latents directory's name does not depend on the ControlNets; `edit` records them in its
+config.yaml (`controlnets: [{path, control, scale}]`).  Under torchrun every rank reads the control maps itself.
 `--weights FILE` takes the UNet, VAE and text encoder weights from a single-file checkpoint in the original LDM
 layout; `--model_dir` must then be a diffusers folder of the same family, which gives the architectures, the
 tokenizer and the scheduler.  `--lora FILE[:SCALE]` (repeatable, SCALE 1.0 by default) merges a LoRA into the UNet
@@ -125,9 +134,13 @@ def main(argv: Optional[List[str]] = None) -> None:
                        help="single-file SD checkpoint in the original LDM layout (.safetensors, .ckpt); its UNet, "
                             "VAE and text encoder weights replace --model_dir's, which still gives the architectures, "
                             "tokenizer and scheduler")
-        p.add_argument("--controlnet_dir", default=None,
-                       help="diffusers ControlNet directory (Canny), or a single-file ControlNet (.pth, .safetensors) "
-                            "built on --model_dir's UNet config")
+        p.add_argument("--controlnet_dir", action="append", default=[],
+                       help="diffusers ControlNet directory, or a single-file ControlNet (.pth, .safetensors) built on "
+                            "--model_dir's UNet config; repeatable, the nets' residuals are summed")
+        p.add_argument("--control", action="append", default=[], metavar="SOURCE",
+                       help="conditioning of the --controlnet_dir at the same position: canny, frames, a video file "
+                            "or a %%05d.png / %%05d.jpg folder of control maps; repeatable (default: canny for every "
+                            "net)")
         p.add_argument("--variant", default=None, help="weights variant of the folders read, e.g. fp16")
         p.add_argument("--lora", action="append", default=[], type=parse_lora, metavar="FILE[:SCALE]",
                        help="LoRA file (kohya, diffusers or PEFT layout) merged into the UNet and text encoder of this "
@@ -144,6 +157,8 @@ def main(argv: Optional[List[str]] = None) -> None:
     p.add_argument("--save_steps", type=int, default=50)
     p.add_argument("--n_frames", type=int, default=40)
     p.add_argument("--inversion_prompt", type=str, default="a woman running")
+    p.add_argument("--controlnet_conditioning_scale", type=float, nargs="+", default=[1.0], metavar="S",
+                   help="ControlNet residual scale: one for every net, or one per --controlnet_dir")
     sub.choices["edit"].add_argument("--config_path", type=str, default="configs/config_pnp.yaml")
     args = ap.parse_args(argv)
     world, rank, comm, device = _distributed(args.device)
@@ -172,10 +187,47 @@ def read_video_input(args, rank: int, device: torch.device) -> torch.Tensor:
     return frames[:args.n_frames]
 
 
+def check_controls(controlnet_dirs: List[str], controls: List[str], scale) -> None:
+    """Refuses `--control` and scale counts that do not pair with the `--controlnet_dir`s (ValueError naming both)."""
+    k = len(controlnet_dirs)
+    if controls and len(controls) != k:
+        raise ValueError(f"{len(controls)} --control for {k} --controlnet_dir")
+    if k and isinstance(scale, (list, tuple)) and len(scale) != k:
+        raise ValueError(f"{len(scale)} controlnet_conditioning_scale values for {k} --controlnet_dir")
+
+
+def read_control(source: str, n: int):
+    """The `control_cond` source of one `--control`: "canny" and "frames" as they are, else the first (up to) `n`
+    control maps of a video file or a %05d.png / %05d.jpg folder, uint8 [M, h, w, 3] on the host at their own size
+    (`control_cond` resizes them and refuses fewer than the frames)."""
+    if source in ("canny", "frames"):
+        return source
+    if os.path.isfile(source):
+        from .video import read_video
+        return read_video(source)[0][:n]
+    if os.path.isdir(source):
+        ext = "png" if os.path.exists(os.path.join(source, "00000.png")) else "jpg"
+        m = 0
+        while m < n and os.path.exists(os.path.join(source, f"{m:05d}.{ext}")):
+            m += 1
+        return read_frames(source, m) if m else torch.zeros((0, 1, 1, 3), dtype=torch.uint8)
+    raise ValueError(f"--control {source!r} is not canny, frames, a video file or a frame folder")
+
+
 def _run(args, world: int, rank: int, comm, device: torch.device) -> None:
     import yaml
     from . import pipeline
     from .util import add_dict_to_yaml_file, save_video, seed_everything
+    config = None
+    if args.stage == "preprocess":
+        s = args.controlnet_conditioning_scale
+        args.controlnet_conditioning_scale = s[0] if len(s) == 1 else s
+        scale = args.controlnet_conditioning_scale
+    else:
+        with open(args.config_path) as f:
+            config = yaml.safe_load(f)
+        scale = config.get("controlnet_conditioning_scale", 1.0)
+    check_controls(args.controlnet_dir, args.control, scale)
     video_frames = None
     if args.stage == "preprocess" and os.path.isfile(args.data_path):   # decoded first: a bad video fails fast
         video_frames = read_video_input(args, rank, device)
@@ -187,7 +239,8 @@ def _run(args, world: int, rank: int, comm, device: torch.device) -> None:
     if args.stage == "preprocess":
         seed_everything(1)                                                   # preprocess.py:303
         frames = video_frames if video_frames is not None else read_frames(args.data_path, args.n_frames)
-        _, recon = pipeline.preprocess(parts, frames, args, **dist_kw)
+        controls = [read_control(c, frames.shape[0]) for c in args.control] or None
+        _, recon = pipeline.preprocess(parts, frames, args, controls=controls, **dist_kw)
         if rank == 0:
             add_dict_to_yaml_file(os.path.join(args.save_dir, "inversion_prompts.yaml"), Path(args.data_path).stem,
                                   args.inversion_prompt)
@@ -196,8 +249,6 @@ def _run(args, world: int, rank: int, comm, device: torch.device) -> None:
             save_video(recon, os.path.join(path, "inverted.mp4"), fps=10)        # preprocess.py:329-330
         return
 
-    with open(args.config_path) as f:
-        config = yaml.safe_load(f)
     path = find_latents(config)
     with open(os.path.join(path, "inversion_prompt.txt")) as f:
         config["inversion_prompt"] = f.read()
@@ -205,13 +256,19 @@ def _run(args, world: int, rank: int, comm, device: torch.device) -> None:
     n = min(int(config["n_frames"]), next(iter(source.values())).shape[0])
     seed_everything(int(config.get("seed", 1)))                              # run_tokenflow_pnp.py:277
     frames = read_frames(config["data_path"], n)
+    controls = [read_control(c, n) for c in args.control] or None
     pnp = pipeline.edit_mode(config) == "pnp"
-    out = pipeline.edit(parts, frames, config, source, vae_recon=pnp and rank == 0, **dist_kw)
+    out = pipeline.edit(parts, frames, config, source, vae_recon=pnp and rank == 0, controls=controls, **dist_kw)
     if rank == 0:
         out_dir = config["output_path"]
         os.makedirs(out_dir, exist_ok=True)
         if args.lora:
             config["loras"] = [{"path": path, "scale": scale} for path, scale in args.lora]
+        if args.controlnet_dir:
+            scales = scale if isinstance(scale, (list, tuple)) else [scale] * len(args.controlnet_dir)
+            config["controlnets"] = [{"path": p, "control": c, "scale": float(s)} for p, c, s in
+                                     zip(args.controlnet_dir, args.control or ["canny"] * len(args.controlnet_dir),
+                                         scales)]
         with open(os.path.join(out_dir, "config.yaml"), "w") as f:
             yaml.dump(config, f)
         videos = {}

@@ -8,10 +8,13 @@ the device) at 512 x 512 and 384 x 672, with GB/s of the algorithmic bytes (the 
 threading off), and a thread pool of one worker per core.  The device edges are compared with cv2's (or, where cv2
 is not installed, with oracle/canny.py), bytes equal.
 
-Edit step: the C2 workload (SD1.5, 40 frames, B = 8, 50-step PnP, random-init fp16 UNet and ControlNet in
-channels_last, fused pass, CUDA-graphed step) with and without the ControlNet, alternated over rounds: ms per
-denoising step.  Inversion: ms per graph-replayed step of the inversion stage (40 frames at 512 x 512 in one UNet
-call per step), with and without the ControlNet, alternated likewise.  The card's name, power limit and SM clock are
+Edit step: the C2 workload (SD1.5, 40 frames, B = 8, 50-step PnP, random-init fp16 UNet and ControlNets in
+channels_last, fused pass, CUDA-graphed step) with 0, 1 and 2 ControlNets (the second a `MultiControlNetModel` of
+the Canny net and another random net on the frames themselves), alternated over rounds: ms per denoising step.
+Inversion: ms per graph-replayed step of the inversion stage (40 frames at 512 x 512 in one UNet call per step), with
+0, 1 and 2 ControlNets, alternated likewise.  Each arm also reports its peak allocated memory: the most
+`torch.cuda.max_memory_allocated` rose above what was allocated before the arm was built, while its models were
+built and its steps captured and run once.  The card's name, power limit and SM clock are
 read by nvidia-smi before and after.  One JSON line at the end.
 """
 from __future__ import annotations
@@ -98,7 +101,7 @@ def main():
     from vae_bench import card
     from tokenflow_b200 import ops as tf_ops
     from tokenflow_b200 import preprocess, sd_unet, tokenflow_utils as tfu
-    from tokenflow_b200.controlnet import build_controlnet
+    from tokenflow_b200.controlnet import MultiControlNetModel, build_controlnet
     from tokenflow_b200.editor import TokenFlowEditor, synthetic_inputs
     from tokenflow_b200.scheduler import DDIMScheduler
 
@@ -116,10 +119,26 @@ def main():
     n, lat = c["n_frames"], c["latent"]
     rng = np.random.default_rng(1)
     frames = torch.from_numpy(np.stack([gg.make_frame("smooth", 8 * lat, 8 * lat, rng) for _ in range(n)])).cuda()
-    ccond = preprocess.canny_cond(frames)
-    cn = build_controlnet("sd15", seed=3, device="cuda", dtype=torch.float16).to(memory_format=torch.channels_last)
+    net = lambda seed: build_controlnet("sd15", seed=seed, device="cuda", dtype=torch.float16).to(
+        memory_format=torch.channels_last)
+    controls = {"plain": (None, None), "controlnet": (net(3), preprocess.canny_cond(frames)),
+                "two_controlnets": (MultiControlNetModel([net(3), net(4)]),
+                                    preprocess.control_cond(frames, ["canny", "frames"]))}
+    peaks = {}
+
+    def begin():
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        return torch.cuda.memory_allocated()
+
+    def peak_since(base):
+        torch.cuda.synchronize()
+        return round((torch.cuda.max_memory_allocated() - base) / 2 ** 30, 2)
+
     arms = {}
-    for arm in ("plain", "controlnet"):            # one UNet per editor: the hooks live on its modules
+    for arm in controls:                           # one UNet per editor: the hooks live on its modules
+        base = begin()
+        cn, ccond = controls[arm]
         unet = sd_unet.build_unet("sd15", seed=1, device="cuda", dtype=torch.float16, init_on_device=True)
         unet = unet.to(memory_format=torch.channels_last)
         cfg = {"n_frames": n, "batch_size": c["batch"], "n_timesteps": c["n_timesteps"], "guidance_scale": 7.5,
@@ -128,11 +147,13 @@ def main():
         x, text, pnp, src = synthetic_inputs(n, lat, unet.config.cross_attention_dim, c["n_timesteps"], seed=1,
                                              device="cuda", dtype=torch.float16)
         ed = TokenFlowEditor(unet, DDIMScheduler(), tfu, cfg, text, pnp, source_latents=lambda t, s=src: s[t],
-                             controlnet=cn if arm == "controlnet" else None,
-                             controlnet_cond=ccond if arm == "controlnet" else None)
+                             controlnet=cn, controlnet_cond=ccond)
         ed.init_method()
         for i in (0, 30, 45):                      # capture all three step variants
             ed.step_index(x, i)
+        # the ControlNets' weights are shared with the inversion arms below, so they count in these peaks
+        peaks[arm] = peak_since(base) + (0 if cn is None else round(
+            sum(p.numel() * p.element_size() for p in cn.parameters()) / 2 ** 30, 2))
         arms[arm] = (ed, x, unet)
     torch.cuda.synchronize()
     times = {a: [] for a in arms}
@@ -152,7 +173,8 @@ def main():
     for arm in arms:
         med = statistics.median(times[arm])
         result["edit"][arm] = {"ms_per_step": round(med, 2), "ms_per_step_all_rounds": [round(t, 2) for t in times[arm]],
-                               "frames_per_s": round(n / (med * c["n_steps"] / 1e3), 3)}
+                               "frames_per_s": round(n / (med * c["n_steps"] / 1e3), 3),
+                               "peak_alloc_GiB": peaks[arm]}
         print(f"edit {arm}: {result['edit'][arm]}")
     del arms, ed, unet
     torch.cuda.empty_cache()
@@ -164,12 +186,16 @@ def main():
     g = torch.Generator().manual_seed(1)
     x0 = torch.randn(n, 4, lat, lat, generator=g).half().cuda()
     cond = torch.randn(1, 77, unet.config.cross_attention_dim, generator=g).half().cuda()
-    invs = {"plain": preprocess.LatentInverter(unet, DDIMScheduler(), 500),
-            "controlnet": preprocess.LatentInverter(unet, DDIMScheduler(), 500, controlnet=cn, controlnet_cond=ccond)}
     K = args.inv_steps
-    for inv in invs.values():
+    invs, ipeaks = {}, {}
+    for arm, (cn, ccond) in controls.items():
+        base = begin()
+        inv = invs[arm] = preprocess.LatentInverter(unet, DDIMScheduler(), 500, controlnet=cn, controlnet_cond=ccond)
         coef, _, ts_up, _ = inv._device_tables()
         inv._run_steps(x0, cond, n, coef[:3], ts_up[:3])              # capture and warm up
+        # the UNet and the ControlNets are resident before `base`: their weights are added
+        ipeaks[arm] = round(peak_since(base) + sum(p.numel() * p.element_size() for m in (unet, cn) if m is not None
+                                                   for p in m.parameters()) / 2 ** 30, 2)
     torch.cuda.synchronize()
     itimes = {a: [] for a in invs}
     for r in range(args.rounds):
@@ -183,10 +209,11 @@ def main():
             itimes[arm].append((time.perf_counter() - t0) * 1e3 / K)
     for arm in invs:
         result["inversion"][arm] = {"ms_per_step": round(statistics.median(itimes[arm]), 2),
-                                    "ms_per_step_all_rounds": [round(t, 2) for t in itimes[arm]]}
+                                    "ms_per_step_all_rounds": [round(t, 2) for t in itimes[arm]],
+                                    "peak_alloc_GiB": ipeaks[arm]}
         print(f"inversion {arm}: {result['inversion'][arm]}")
     result["workload"] = (f"C2: SD1.5, {n} frames at {8 * lat}^2, B = {c['batch']}, PnP, random-init fp16 UNet and "
-                          "ControlNet, channels_last; inversion: one UNet call of 40 frames per step")
+                          "0, 1 or 2 ControlNets, channels_last; inversion: one UNet call of 40 frames per step")
     result["card_after"] = card()
     text = json.dumps(result, indent=1)
     if args.out:
